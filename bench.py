@@ -1,8 +1,9 @@
 #!/usr/bin/env python
 """bench.py -- audio-sec/sec (RTF^-1) and p50 chunk latency of the WhisperLive per-chunk hot path
-(PCM -> log-mel -> encoder -> beam-search decoder) on N B200s of one node.
+(PCM -> log-mel -> encoder -> beam-search decoder) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 5 --warmup 3
+    python bench.py --gpus 1 --steps 5 --warmup 3 --dump-outputs DIR   # + what the last timed step computed, as .npy
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # the CPU arm (oracle port; CT2/faster-whisper are absent)
@@ -20,6 +21,11 @@ One "step" = one pass of the hot path over the batch of chunks:
           library stream, max over ranks)
   e2e   : the public API call B200WhisperModel.transcribe_batch(host numpy PCM) -> Segment lists on the
           host; H2D of the PCM/features and D2H of features/token ids inside the timed region
+
+--dump-outputs DIR writes, after the timed steps, what the last step of each timed path returned to its caller (rank 0's
+streams): the best hypothesis' token ids, scores and no-speech probabilities of the resident step's generate call, a fixed
+seeded sample of its encoder output, and the token ids of the e2e step's segments.  Inputs and weights are seeded, so two
+builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -64,6 +70,8 @@ def parse_args():
     ap.add_argument("--word-timestamps", action="store_true", help="BASELINE config 4: K14 word alignment on every chunk (e2e only)")
     ap.add_argument("--no-streaming", action="store_true", help="skip the staggered-arrival latency phase (RoundScheduler, step-level admission)")
     ap.add_argument("--stream-load", type=float, default=0.6, help="offered load of the streaming phase as a fraction of the batch throughput")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32 / float64, <= 64 MB in all)")
     return ap.parse_args()
 
 
@@ -78,7 +86,7 @@ def make_streams(n_total: int):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -192,7 +200,7 @@ def main():
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py: no CUDA device -- the B200 path has no CPU fallback (use --impl reference for the CPU arm)")
+        raise SystemExit("bench.py: no CUDA device -- the CUDA path has no CPU fallback (use --impl reference for the CPU arm)")
     torch.cuda.set_device(local)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
@@ -232,10 +240,13 @@ def main():
             dist.barrier()
         torch.cuda.synchronize()
 
+    last = {}   # what the most recent step of each timed path returned (--dump-outputs)
+
     def e2e_step():
         t0 = time.perf_counter()
         out = dist_tr.transcribe_batch(waves, all_kws)      # whole batch in, whole batch out on every rank
         n_ids = sum(len(s.tokens) for segs, _ in out for s in (segs or []))
+        last["e2e"] = out
         return time.perf_counter() - t0, n_ids
 
     # ---- resident-input step: PCM / features already in HBM, device-timed
@@ -251,7 +262,7 @@ def main():
         rc = eng.lib.wl_encode_resident(eng.ctx, len(slots), _lib.ptr(slots, C.c_int32))
         _lib.check(eng.lib, eng.ctx, rc, "wl_encode_resident")
         ms += eng.last_device_ms(1)
-        eng.generate(feats_cache["enc"], feats_cache["prompts"], **feats_cache["gen_kw"])
+        last["resident"] = eng.generate(feats_cache["enc"], feats_cache["prompts"], **feats_cache["gen_kw"])
         ms += eng.last_device_ms(2)
         return ms / 1000.0
 
@@ -290,6 +301,8 @@ def main():
     t_res = [resident_step() for _ in range(args.steps)]
     barrier()
     launches_res = eng.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:   # read before the e2e steps run through the same engine
+        last["encoder_sample"] = encoder_sample(feats_cache["enc"])
     # ---- timed: e2e (host buffers through the public API)
     barrier()
     t0 = time.perf_counter()
@@ -303,6 +316,8 @@ def main():
     barrier()
     t_e2e = time.perf_counter() - t0
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last["resident"], last["encoder_sample"], last["e2e"])
 
     loop_ms, loop_steps = eng.last_device_ms(2), getattr(eng, "last_steps", None)   # the last e2e step's decode loop
     # ---- streaming phase: staggered arrivals through the product scheduler (N=1 rank-local; reported, not the headline)
@@ -352,7 +367,7 @@ def main():
                                    f"{world} GPU(s), beam {args.beam}, chunks U[5,30] s (sum {audio_sec_total:.0f} s audio/step), "
                                    "decode length pinned to ceil(3.2*s)+8 tokens (EOT suppressed)",
                        "streams": args.streams, "streams_per_gpu": n_local, "beam": args.beam, "parallelism": f"dp{world}",
-                       "l2": "working set (3.1 GB weights + 246 MB/stream cross-KV) >> 126 MB L2, no flush needed"},
+                       "l2": "working set (3.1 GB weights + 246 MB/stream cross-KV) >> 50 MB L2, no flush needed"},
             "p50_chunk_latency_ms": 1000 * statistics.median(lat),
             "streaming": streaming,
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(h2d), "d2h_bytes_per_step": int(d2h),
@@ -367,6 +382,38 @@ def main():
         print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def encoder_sample(enc, enc_rows=4096, seed=0):
+    """Encoder output rows (float32) at a fixed seeded sample of (stream, frame) positions -- the whole output would be
+    ~250 MB at 32 large-v3 streams -- and the positions (float64 [n, 2])."""
+    full = np.asarray(enc, dtype=np.float32)                   # [streams, 1500, d_model]
+    rng = np.random.default_rng(seed)
+    n = min(enc_rows, full.shape[0] * full.shape[1])
+    flat = np.sort(rng.choice(full.shape[0] * full.shape[1], size=n, replace=False))
+    rows = np.stack([flat // full.shape[1], flat % full.shape[1]], 1).astype(np.float64)
+    return full.reshape(-1, full.shape[2])[flat], rows
+
+
+def dump_outputs(out_dir, gen, enc_sample, e2e):
+    """The last timed step's results as DIR/<name>.npy: token ids padded with -1 (float64), scores and no-speech
+    probabilities (float64), the encoder output sample of encoder_sample(), and the e2e segments' token ids (float64,
+    padded)."""
+    os.makedirs(out_dir, exist_ok=True)
+
+    def padded(seqs):
+        width = max([len(q) for q in seqs] + [1])
+        a = np.full((len(seqs), width), -1.0, dtype=np.float64)
+        for i, q in enumerate(seqs):
+            a[i, :len(q)] = q
+        return a
+
+    np.save(os.path.join(out_dir, "tokens.npy"), padded([r.sequences_ids[0] if r.sequences_ids else [] for r in gen]))
+    np.save(os.path.join(out_dir, "scores.npy"), np.array([r.scores[0] if r.scores else np.nan for r in gen], dtype=np.float64))
+    np.save(os.path.join(out_dir, "no_speech_prob.npy"), np.array([r.no_speech_prob for r in gen], dtype=np.float64))
+    np.save(os.path.join(out_dir, "encoder_output_sample.npy"), enc_sample[0])
+    np.save(os.path.join(out_dir, "encoder_output_rows.npy"), enc_sample[1])
+    np.save(os.path.join(out_dir, "e2e_tokens.npy"), padded([[t for s in (segs or []) for t in s.tokens] for segs, _ in e2e]))
 
 
 def streaming_latency(model, waves, kws, durs, batch_step_s: float, load: float, cycles: int = 3, step_tokens: int = 16):
@@ -429,13 +476,8 @@ def dominant_kernel_roofline(eng, dims, n_streams, beam, feats_cache, loop_ms, l
     section 4) -- HBM-bound.  Its launch duration is measured live: a short graph-less generate pass over the
     bench's own resident encoder outputs with CUDA events around every launch on the library stream
     (wl_profile_cross_attn).  `step` keeps the whole decode loop (weights + cross-KV + self-KV per token) for context."""
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
-    which = "measured burst copy bandwidth (MEASURED_PEAKS.json)" if "hbm_gbs" in peaks else "fallback (B200_PROFILING.md)"
+    peak = 3350.0
+    which = "H100 SXM data sheet HBM3 bandwidth (a bound, not a reached figure)"
     d, L, V = dims.d_model, dims.dec_layers, dims.vocab
     # whole decode loop of the last timed generate call
     steps, ms = loop_steps, loop_ms
@@ -462,24 +504,12 @@ def dominant_kernel_roofline(eng, dims, n_streams, beam, feats_cache, loop_ms, l
         eng.profile_cross_attn(False)
         eng.use_cuda_graph = graph0
     alg = n_streams * 2 * 1500 * d * 2          # bytes one launch has to read: K and V of every stream, fp16
-    traffic = None
-    try:   # DRAM bytes per launch from the committed ncu --set full capture of this kernel at this configuration
-        for fn in ("traffic_r2.json", "traffic_r1.json"):      # newest committed ncu --set full capture of this kernel
-            path = os.path.join(ROOT, "profiles", fn)
-            if not os.path.exists(path):
-                continue
-            t = json.load(open(path)).get("cross_attn_kernel", {})
-            if int(t.get("streams", -1)) == n_streams and t.get("model") == dims.name:
-                traffic = float(t["dram_bytes_per_launch"])
-                break
-    except Exception:
-        pass
     if avg_ms <= 0:
         return {"bound": "hbm", "kernel": "cross_attn_kernel (K11)", "achieved": None, "peak": peak, "unit": "GB/s", "frac": None,
-                "traffic": traffic, "peak_source": which, "step": step_info}
+                "peak_source": which, "step": step_info}
     achieved = alg / (avg_ms / 1000.0) / 1e9
     return {"bound": "hbm", "kernel": "cross_attn_kernel (K11 decoder cross-attention, one launch per decoder layer per token)",
-            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic,
+            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
             "algorithmic_bytes_per_launch": int(alg), "avg_launch_us": 1000.0 * avg_ms, "launches_timed": n_launch,
             "timing": "CUDA events around each launch on the library stream (includes the launch gap), graph-less pass",
             "peak_source": which, "step": step_info}

@@ -1,4 +1,4 @@
-/* libwlb200 -- C ABI of the B200-native Whisper hot path behind WhisperLive's transcriber.
+/* libwlb200 -- C ABI of the H100-native Whisper hot path behind WhisperLive's transcriber.
  *
  * Every entry point replaces one call the reference makes into its native engine
  * (ctranslate2.models.Whisper + faster_whisper.FeatureExtractor; neither is in the reference tree,
@@ -133,7 +133,7 @@ int wl_align(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* start_
 /* teacher-forced logits: tokens concatenated at tok_off[B+1]; logits_out [sum T, vocab] float32 */
 int wl_decode_logits(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* tokens, const int32_t* tok_off,
                      float* logits_out);
-/* C[z] = A[z] (MxK) * B[z]^T (NxK) (+bias[n]) on the tcgen05 path (use_simt=0) or the CUDA-core checker */
+/* C[z] = A[z] (MxK) * B[z]^T (NxK) (+bias[n]) on the wgmma path (use_simt=0) or the CUDA-core checker */
 int wl_test_gemm(wl_ctx* ctx, const uint16_t* a_f16, const uint16_t* b_f16, const float* bias, float* c, int32_t M, int32_t N,
                  int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt);
 /* test hook of the small-batch decode GEMM (csrc/wgemm.cu, R <= 32): out[R][n_out] = X[R][K] W[n_out][K]^T with the fused

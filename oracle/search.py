@@ -128,10 +128,12 @@ def sample_begin(prompt: Sequence[int], spec: VocabSpec) -> int:
 
 
 def apply_processors(logits: torch.Tensor, gen: List[int], spec: VocabSpec, opts: GenOptions,
-                     use_timestamps: bool, prefix: Sequence[int] = ()) -> torch.Tensor:
+                     use_timestamps: bool, prefix: Sequence[int] = (), rule_margin: Optional[List[float]] = None) -> torch.Tensor:
     """One row: raw logits [V] f32 -> log-probabilities [V] f32 after all masks.  ``gen`` are the generated tokens,
     ``prefix`` the prompt tokens after the sot sequence (history of the timestamp rules = prefix + gen; blank
-    suppression is keyed to the first generated step)."""
+    suppression is keyed to the first generated step).  ``rule_margin``, when given, receives |log P(any timestamp) -
+    max log P(text token)| if the timestamp-probability rule was evaluated: that rule is a decision of its own, and a
+    near-tie in it changes the next token however large the sampling / arg-max margin is."""
     x = logits.clone()
     if len(opts.suppress_tokens):
         x[torch.as_tensor(list(opts.suppress_tokens), dtype=torch.long)] = NEG_INF
@@ -160,6 +162,8 @@ def apply_processors(logits: torch.Tensor, gen: List[int], spec: VocabSpec, opts
                 x[tb:cutoff] = NEG_INF
             logp = torch.log_softmax(x, dim=-1)
             ts_lp = torch.logsumexp(logp[tb:], dim=-1)
+            if rule_margin is not None:
+                rule_margin.append(abs(float(ts_lp - logp[:tb].max())))
             if ts_lp > logp[:tb].max():
                 x[:tb] = NEG_INF
     return torch.log_softmax(x, dim=-1)
@@ -191,7 +195,8 @@ class StreamResult:
     scores: List[float] = field(default_factory=list)
     no_speech_prob: float = 0.0
     steps: int = 0
-    # per-step decision margins (top1 - top2 of the ranked candidates) for divergence-aware comparison
+    # per-step decision margins (top1 - top2 of the ranked candidates, or the timestamp-rule margin when that is smaller)
+    # for divergence-aware comparison
     margins: List[float] = field(default_factory=list)
     # beam search only, when GenOptions.trace: per step {"alive": [token tuples], "cand": [(beam, token, total)]}
     # with 2K+2 ranked candidates -- lets a test name the near-tie behind a pruning difference
@@ -250,7 +255,9 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
                 if done[r]:
                     nxt.append(spec.eot)
                     continue
-                logp = apply_processors(logits[r], gens[r], spec, opts, use_ts, prefix)
+                rule = []
+                logp = apply_processors(logits[r], gens[r], spec, opts, use_ts, prefix, rule)
+                rule_m = min(rule) if rule else float("inf")
                 if sampling:
                     z = logp / opts.sampling_temperature
                     if opts.sampling_topk > 0:
@@ -259,14 +266,14 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
                     z = z + torch.from_numpy(gumbel_noise(opts.seed, stream_index * 64 + r, step, spec.vocab))
                     zv, zi = topk_stable(z, 2)
                     tok = int(zi[0])
-                    res.row_margins.setdefault(r, []).append(float(zv[0] - zv[1]))
+                    res.row_margins.setdefault(r, []).append(min(float(zv[0] - zv[1]), rule_m))
                     if r == 0:
-                        res.margins.append(float(zv[0] - zv[1]))
+                        res.margins.append(min(float(zv[0] - zv[1]), rule_m))
                 else:
                     vals, idx = topk_stable(logp, 2)
                     tok = int(idx[0])
                     if r == 0:
-                        res.margins.append(float(vals[0] - vals[1]))
+                        res.margins.append(min(float(vals[0] - vals[1]), rule_m))
                 cums[r] += float(logp[tok])
                 if tok == spec.eot:
                     done[r] = True

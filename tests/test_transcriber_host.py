@@ -161,10 +161,10 @@ def test_window_batch_buffer_equals_pad_and_stack():
     assert not np.shares_memory(other["buf"], got2)          # a second thread never sees this thread's buffer
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/whisper_live"), reason="reference tree only exists in the build container")
 def test_host_helpers_match_reference_code_live():
-    """Differential run against the reference's own functions (imported with ctranslate2 / faster_whisper stubbed) on
-    ~1400 randomised inputs: timestamp splitting, prompt assembly, suppress list, punctuation merge, compression ratio."""
+    """Differential run against the reference's own functions on ~1400 seeded randomised inputs: timestamp splitting,
+    prompt assembly, suppress list, punctuation merge, compression ratio, language detection.  What the reference returned
+    (imported with ctranslate2 / faster_whisper stubbed) is recorded in tests/golden/host_reference.json."""
     import json
     import subprocess
     import sys

@@ -1,5 +1,5 @@
-"""Short hot-path pass for ncu: large-v3-shaped engine, S streams, a few decode steps.
-    ncu --profile-from-start off ... python tools/profile_step.py [--model large-v3] [--streams 8] [--tokens 6] [--beam 4]
+"""Short hot-path pass for a profiler: large-v3-shaped engine, S streams, a few decode steps.
+    python tools/profile_step.py [--model large-v3] [--streams 8] [--tokens 6] [--beam 4]
 The profiled region (cudaProfilerStart/Stop) is one mel + encode + generate pass after a warm-up pass."""
 import argparse
 import ctypes

@@ -74,7 +74,7 @@ if ServeClientBase is not None:
             self.websocket.send(json.dumps({"uid": self.client_uid, "message": self.SERVER_READY, "backend": "faster_whisper"}))
 
         def create_model(self):
-            """Build the shared transcriber (CUDA engine). Raises when no B200 / library is available."""
+            """Build the shared transcriber (CUDA engine). Raises when no H100 / library is available."""
             if ServeClientB200.MODEL_FACTORY is not None:
                 return ServeClientB200.MODEL_FACTORY(self.model_size_or_path)
             from .parallel import MultiDeviceWhisperModel, devices_from_env

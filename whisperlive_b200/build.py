@@ -1,4 +1,4 @@
-"""Build whisperlive_b200/libwlb200.so (sm_100a only) with nvcc.  In-tree so the .so travels to
+"""Build whisperlive_b200/libwlb200.so (sm_90a only) with nvcc.  In-tree so the .so travels to
 the GPU box with the repository snapshot.  `python -m whisperlive_b200.build [--force] [--verbose]`"""
 from __future__ import annotations
 
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libwlb200.so")
 SOURCES = ["gemm.cu", "dec_gemm.cu", "wgemm.cu", "mel.cu", "elementwise.cu", "attention.cu", "flash_attn.cu", "search.cu", "prefill.cu", "misc.cu", "engine.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC"]
 
 
@@ -45,7 +45,7 @@ def build(force: bool = False, verbose: bool = False, timeline: bool = False) ->
 
     with cf.ThreadPoolExecutor(max_workers=8) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [NVCC, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a"]
+    cmd = [NVCC, "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_90a,code=sm_90a"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

@@ -148,8 +148,8 @@ __global__ void __launch_bounds__(SA_WARPS * 32) self_attn_kernel(DecodeState s,
   const float inv = 1.f / warp_sum(lsum);
   __syncwarp();
   // weighted V sum: lane = (position group pg = lane / 8, 16-byte dim chunk c8 = lane % 8).  The 4 groups stride over
-  // the cached positions with independent 16-byte loads (8 in flight per lane), then fold with two shuffles; round 1
-  // walked the positions one by one with a dependent (index -> V row) load pair each: ~0.25 us per cached position.
+  // the cached positions with independent 16-byte loads (8 in flight per lane), then fold with two shuffles, instead of
+  // walking the positions one by one with a dependent (index -> V row) load pair each.
   float acc[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) acc[i] = 0.f;
@@ -207,7 +207,7 @@ void decoder_self_attn(cudaStream_t st, const DecodeState& s, const PartialSrc& 
 // Per (stream, head, key range): S = q K^T and O = P V on the warp-level tensor-core path (mma.sync m16n8k16,
 // fp16 operands, fp32 accumulate; N = 8 = the stream's beam rows).  The kernel is an HBM stream of the encoder
 // K/V (246 MB per layer at 32 streams) -- the arithmetic is ~0.1 GFLOP per CTA, so it stays on mma.sync rather
-// than tcgen05 (M = 128 x N >= 16 tiles + TMEM round trips buy nothing here); what matters is that the consumer
+// than wgmma (M = 64-row warpgroup tiles buy nothing here); what matters is that the consumer
 // warps issue ~40 instructions per 16 KB chunk instead of ~400 on the CUDA-core path, which left the kernel
 // issue-bound at half of the HBM rate.
 //   * K/V chunks (128 keys x 64 dims, 16 KB contiguous) arrive by cp.async.bulk into a ring of XA_STAGES buffers.
@@ -581,9 +581,8 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
 }
 
 // Merge the nsplit partial softmaxes of every (row, head), in key-range order.  A separate (tiny) kernel on purpose:
-// merging inside cross_attn_kernel (last key range to arrive, found with a fence + atomic) was measured at the same
-// cost at 4 streams and 5 us WORSE at 32 streams, where every persistent CTA pays the fence/atomic round trip once per
-// item in the middle of its K/V stream (in-graph timeline, profiles/timeline_r2.md).
+// merging inside cross_attn_kernel (last key range to arrive, found with a fence + atomic) makes every persistent CTA
+// pay the fence/atomic round trip once per item in the middle of its K/V stream, which grows with the stream count.
 __global__ void __launch_bounds__(64) cross_attn_combine_kernel(DecodeState s, const float* __restrict__ part, __half* __restrict__ out,
                                                                 int rows_per_stream, int H, int d, int nsplit) {
   const int r = blockIdx.y, h = blockIdx.x, dd = threadIdx.x;

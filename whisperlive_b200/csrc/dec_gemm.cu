@@ -1,13 +1,12 @@
 // Decode-step GEMM (K9 / K12): Y^T[n_out, R] = W[n_out, K] * X[R, K]^T, weight-streaming, split over K.
 //
-// Why a second GEMM kernel next to gemm.cu: the decode step is a chain of ~200 dependent launches per token, and the
-// in-graph timeline (tools/timeline.py, DESIGN.md section 5) showed that what each of them costs is not the kernel
-// boundary (1.1 us for a trivial kernel inside the graph, tools/ubench_chain.cu) but COLD INSTRUCTION FETCH: the general
-// tcgen05 kernel is 50-86 KB of SASS (four epilogues, batching, tile walks, the fused post-op), the kernels of one layer
-// together overflow the SM's instruction caches, so every launch streams its code from L2 again (~0.2 us per KB).
-// This kernel is the same tcgen05 / TMA / TMEM pipeline cut down to what the decode step needs:
-//   * one tile per CTA (grid = feature tiles x K ranges x row tiles), no persistent tile walk, one TMEM accumulator;
-//   * one epilogue: the raw fp32 partial sum of this K range, stored transposed (lane = feature, coalesced);
+// Why a second GEMM kernel next to gemm.cu: the decode step is a chain of ~200 dependent launches per token, and what
+// each of them costs is dominated by fetching its instructions, not by the kernel boundary: the general GEMM kernel
+// carries four epilogues, batching, tile walks and the fused post-op, the kernels of one layer together overflow the
+// SM's instruction caches, so every launch streams its code from L2 again (tools/timeline.py measures this per kernel).
+// This kernel is the same TMA / wgmma pipeline cut down to what the decode step needs:
+//   * one tile per CTA (grid = feature tiles x K ranges x row tiles), no persistent tile walk;
+//   * one epilogue: the raw fp32 partial sum of this K range, stored transposed (consecutive features per store);
 //     whoever consumes it adds the ranges and the bias in index order (bit-reproducible, no atomics);
 //   * the vocabulary projection is the same thing with one K range and the logits buffer as the output.
 // The weight k-blocks of the first STAGES stages are requested before griddepcontrol.wait (PDL): they stream while the
@@ -31,50 +30,14 @@ struct DecGemmParams {
 
 constexpr int DG_BM = 128, DG_BK = 64, DG_A_BYTES = DG_BM * DG_BK * 2;
 
+// The pipeline both decode GEMMs share.  CTA = 384 threads: warp 0 is the TMA producer (its first STAGES weight k-blocks
+// are requested before the dependency wait), warpgroups 1 and 2 multiply feature rows 0-63 / 64-127 of the tile into
+// acc.  Returns true on the consumer threads, whose acc then holds this CTA's K range of the tile.
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(BN >= 64 ? 384 : 256, 1)
-dec_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DecGemmParams p) {
-  extern __shared__ uint8_t dg_smem_raw[];
-  uint8_t* base = dg_smem_raw + ((1024u - (smem_u32(dg_smem_raw) & 1023u)) & 1023u);
+__device__ __forceinline__ bool dg_pipeline(const CUtensorMap& tmW, const CUtensorMap& tmX, uint8_t* sA, uint8_t* sB, uint64_t* full,
+                                            uint64_t* empty, int tile_m, int tile_n, int kb0, int num_kb, float (&acc)[BN / 2]) {
   constexpr int B_BYTES = BN * DG_BK * 2;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
-  uint8_t* sA = base;
-  uint8_t* sB = base + STAGES * DG_A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
-  uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
-
   const int warp = threadIdx.x >> 5;
-  const int tile_m = blockIdx.x % p.tiles_m;
-  const int rest = blockIdx.x / p.tiles_m;
-  const int split = rest % p.nsplit, tile_n = rest / p.nsplit;
-  const int kb0 = split * p.kb_per_split;
-  const int num_kb = min(p.kb_per_split, p.kb_total - kb0);
-  pdl_trigger();
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmW);
-    tma_prefetch_desc(&tmX);
-  }
-  if (warp == 1 && elect_one()) {
-#pragma unroll 1
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(acc_full, 1);
-    mbar_fence_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
-
   if (warp == 0) {
     if (elect_one()) {
       const int pre = min(num_kb, STAGES);
@@ -100,66 +63,74 @@ dec_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(DG_BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint64_t adesc = umma_desc_sw128(smem_u32(sA + stage * DG_A_BYTES));
-        const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + stage * B_BYTES));
-#pragma unroll
-        for (int k = 0; k < DG_BK / 16; ++k)
-          umma_f16(tmem_acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-        umma_commit(&empty[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(acc_full);
-    }
-  } else if (warp >= 4) {
-    // warps 4-7 own TMEM lanes (= features) 32q..32q+31; with BN >= 64 warps 8-11 take the upper half of the columns
-    const int q = warp & 3;
-    constexpr int NH = BN >= 64 ? 2 : 1, HC = BN / NH;
-    const int c_lo = ((warp - 4) >> 2) * HC;
-    const int m = tile_m * DG_BM + q * 32 + lane_id();
-    float* dst = p.out + (long)split * p.part_stride + m;
-    pdl_wait();   // the partial buffer may still be read by the kernels before this one
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    const uint32_t lane_addr = tmem_acc + ((uint32_t)(q * 32) << 16);
-    if constexpr (BN >= 32) {
-#pragma unroll 1
-      for (int c = c_lo; c < c_lo + HC; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(lane_addr + c, v);
-        tmem_ld_wait();
-        if (m < p.M) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            const int n = tile_n * BN + c + i;
-            if (n < p.N) dst[(long)n * p.ldn] = __uint_as_float(v[i]);
-          }
-        }
-      }
-    } else {
-      uint32_t v[16];
-      tmem_ld_32x16(lane_addr, v);
-      tmem_ld_wait();
-      if (m < p.M) {
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const int n = tile_n * BN + i;
-          if (n < p.N) dst[(long)n * p.ldn] = __uint_as_float(v[i]);
-        }
-      }
-    }
+    return false;
   }
-  tc_fence_before();
+  if (warp < 4) return false;
+  const int wg = (warp >> 2) - 1;
+  int stage = 0, prev = -1;   // acc needs no initialisation: the first k-step of k-block 0 overwrites it (scale-d 0)
+  uint32_t phase = 0;
+#pragma unroll 1
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full[stage], phase);
+    wgmma_fence();
+    wgmma_tile_k64<BN>(acc, sA + stage * DG_A_BYTES, sB + stage * B_BYTES, wg, kb > 0);
+    wgmma_commit();
+    wgmma_wait<1>();
+    if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
+    prev = stage;
+    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+  }
+  wgmma_wait<0>();
+  wgmma_fence_regs(acc);
+  return true;
+}
+
+template <int BN, int STAGES>
+__device__ __forceinline__ void dg_init_barriers(const CUtensorMap& tmW, const CUtensorMap& tmX, uint64_t* full, uint64_t* empty) {
+  const int warp = threadIdx.x >> 5;
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&tmW);
+    tma_prefetch_desc(&tmX);
+  }
+  if (warp == 1 && elect_one()) {
+#pragma unroll 1
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 8);   // one arrival per consumer warp
+    }
+    mbar_fence_init();
+  }
   __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_acc, TMEM_COLS);
+}
+
+template <int BN, int STAGES>
+__global__ void __launch_bounds__(384, 1)
+dec_gemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const DecGemmParams p) {
+  extern __shared__ uint8_t dg_smem_raw[];
+  uint8_t* base = dg_smem_raw + ((1024u - (smem_u32(dg_smem_raw) & 1023u)) & 1023u);
+  constexpr int B_BYTES = BN * DG_BK * 2;
+  uint8_t* sA = base;
+  uint8_t* sB = base + STAGES * DG_A_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
+  uint64_t* empty = full + STAGES;
+
+  const int tile_m = blockIdx.x % p.tiles_m;
+  const int rest = blockIdx.x / p.tiles_m;
+  const int split = rest % p.nsplit, tile_n = rest / p.nsplit;
+  const int kb0 = split * p.kb_per_split;
+  const int num_kb = min(p.kb_per_split, p.kb_total - kb0);
+  pdl_trigger();
+  dg_init_barriers<BN, STAGES>(tmW, tmX, full, empty);
+  float acc[BN / 2];
+  if (!dg_pipeline<BN, STAGES>(tmW, tmX, sA, sB, full, empty, tile_m, tile_n, kb0, num_kb, acc)) return;
+  // thread rows = features (8 consecutive per store instruction), stored transposed: out[split][row][feature]
+  const int m0 = tile_m * DG_BM + (((threadIdx.x >> 5) >> 2) - 1) * 64;
+  float* dst = p.out + (long)split * p.part_stride;
+  pdl_wait();   // the partial buffer may still be read by the kernels before this one
+  wgmma_acc_foreach(acc, [&](int r, int c, float v) {
+    const int m = m0 + r, n = tile_n * BN + c;
+    if (m < p.M && n < p.N) dst[(long)n * p.ldn + m] = v;
+  });
 }
 
 template <int BN, int STAGES>
@@ -167,7 +138,7 @@ static constexpr int dg_smem() { return STAGES * (DG_A_BYTES + BN * DG_BK * 2) +
 
 template <int BN, int STAGES>
 static void dg_launch(cudaStream_t st, const CUtensorMap& tw, const CUtensorMap& tx, const DecGemmParams& p, int grid) {
-  launch_kernel(dec_gemm_kernel<BN, STAGES>, dim3(grid), dim3(BN >= 64 ? 384 : 256), (size_t)dg_smem<BN, STAGES>(), st, tw, tx, p);
+  launch_kernel(dec_gemm_kernel<BN, STAGES>, dim3(grid), dim3(384), (size_t)dg_smem<BN, STAGES>(), st, tw, tx, p);
 }
 template <int BN, int STAGES>
 static void dg_prime() {
@@ -259,125 +230,33 @@ struct CGemmParams {
 };
 
 template <int BN, int STAGES>
-__global__ void __launch_bounds__(BN >= 64 ? 384 : 256, 1)
+__global__ void __launch_bounds__(384, 1)
 cgemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmX, const CGemmParams p) {
   extern __shared__ uint8_t dg_smem_raw[];
   uint8_t* base = dg_smem_raw + ((1024u - (smem_u32(dg_smem_raw) & 1023u)) & 1023u);
   constexpr int B_BYTES = BN * DG_BK * 2;
-  constexpr uint32_t TMEM_COLS = BN < 32 ? 32 : BN;
-  constexpr int NTHREADS = BN >= 64 ? 384 : 256;
+  constexpr int NTHREADS = 384;
   static_assert(BN * DG_BM * 4 <= STAGES * DG_A_BYTES, "the accumulator tile is parked in the weight stages");
   uint8_t* sA = base;
   uint8_t* sB = base + STAGES * DG_A_BYTES;
   uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_full + 1);
   float* red = reinterpret_cast<float*>(sA);   // [BN rows][128 features] once the MMAs are done
 
-  const int warp = threadIdx.x >> 5;
   const int split = blockIdx.x % p.nsplit;     // = rank in the cluster (cluster = nsplit consecutive CTAs)
   const int rest = blockIdx.x / p.nsplit;
   const int tile_m = rest % p.tiles_m, tile_n = rest / p.tiles_m;
   const int kb0 = split * p.kb_per_split;
   const int num_kb = min(p.kb_per_split, p.kb_total - kb0);
   pdl_trigger();
-
-  if (warp == 0 && elect_one()) {
-    tma_prefetch_desc(&tmW);
-    tma_prefetch_desc(&tmX);
+  dg_init_barriers<BN, STAGES>(tmW, tmX, full, empty);
+  float tile_acc[BN / 2];
+  if (dg_pipeline<BN, STAGES>(tmW, tmX, sA, sB, full, empty, tile_m, tile_n, kb0, num_kb, tile_acc)) {
+    // both consumer warpgroups have retired every MMA before either overwrites the stages with its tile
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    const int m0 = (((threadIdx.x >> 5) >> 2) - 1) * 64;
+    wgmma_acc_foreach(tile_acc, [&](int r, int c, float v) { red[c * DG_BM + m0 + r] = v; });
   }
-  if (warp == 1 && elect_one()) {
-#pragma unroll 1
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    mbar_init(acc_full, 1);
-    mbar_fence_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
-
-  if (warp == 0) {
-    if (elect_one()) {
-      const int pre = min(num_kb, STAGES);
-#pragma unroll 1
-      for (int kb = 0; kb < pre; ++kb) {   // weights do not depend on the preceding kernel
-        mbar_expect_tx(&full[kb], DG_A_BYTES + B_BYTES);
-        tma_load_4d(sA + kb * DG_A_BYTES, &tmW, &full[kb], (kb0 + kb) * DG_BK, tile_m * DG_BM, 0, 0);
-      }
-      if (blockIdx.x == 0) tl_stamp_any(TL_GEMM_PART, 0);
-      pdl_wait();
-      if (blockIdx.x == 0) tl_stamp_any(TL_GEMM_PART, 1);
-      int stage = 0;
-      uint32_t phase = 0;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        const int k0 = (kb0 + kb) * DG_BK;
-        if (kb >= pre) {
-          mbar_wait(&empty[stage], phase ^ 1);
-          mbar_expect_tx(&full[stage], DG_A_BYTES + B_BYTES);
-          tma_load_4d(sA + stage * DG_A_BYTES, &tmW, &full[stage], k0, tile_m * DG_BM, 0, 0);
-        }
-        tma_load_4d(sB + stage * B_BYTES, &tmX, &full[stage], k0, tile_n * BN, 0, 0);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(DG_BM, BN);
-      int stage = 0;
-      uint32_t phase = 0;
-#pragma unroll 1
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[stage], phase);
-        tc_fence_after();
-        const uint64_t adesc = umma_desc_sw128(smem_u32(sA + stage * DG_A_BYTES));
-        const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + stage * B_BYTES));
-#pragma unroll
-        for (int k = 0; k < DG_BK / 16; ++k)
-          umma_f16(tmem_acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-        umma_commit(&empty[stage]);
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      umma_commit(acc_full);
-    }
-  } else if (warp >= 4) {
-    // warps 4-7 own TMEM lanes (= features) 32q..32q+31; with BN >= 64 warps 8-11 take the upper half of the columns.
-    // acc_full fires when every MMA has retired, i.e. nothing reads the stages any more: park the tile there.
-    const int q = warp & 3;
-    constexpr int NH = BN >= 64 ? 2 : 1, HC = BN / NH;
-    const int c_lo = ((warp - 4) >> 2) * HC;
-    float* dst = red + q * 32 + lane_id();
-    mbar_wait(acc_full, 0);
-    tc_fence_after();
-    const uint32_t lane_addr = tmem_acc + ((uint32_t)(q * 32) << 16);
-    if constexpr (BN >= 32) {
-#pragma unroll 1
-      for (int c = c_lo; c < c_lo + HC; c += 32) {
-        uint32_t v[32];
-        tmem_ld_32x32(lane_addr + c, v);
-        tmem_ld_wait();
-#pragma unroll
-        for (int i = 0; i < 32; ++i) dst[(c + i) * DG_BM] = __uint_as_float(v[i]);
-      }
-    } else {
-      uint32_t v[16];
-      tmem_ld_32x16(lane_addr, v);
-      tmem_ld_wait();
-#pragma unroll
-      for (int i = 0; i < 16; ++i) dst[i * DG_BM] = __uint_as_float(v[i]);
-    }
-  }
-  tc_fence_before();
-  __syncwarp();
   cluster_sync_all();   // every K range of this tile is parked (also orders this CTA's own warps)
   pdl_wait();           // (resolved long ago; every thread below touches memory of the preceding kernels)
   {
@@ -396,7 +275,7 @@ cgemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CU
       const long o = (long)ng * p.M + m;
       float resid = 0.f;
       if (p.mode == 1 && m < p.M) resid = p.out_f32[o];
-      float part[8];   // all ranks' loads in flight together (the serial version cost ~5 us per launch: bench, round 2)
+      float part[8];   // all ranks' loads in flight together rather than one rank after the other
 #pragma unroll
       for (int r = 0; r < 8; ++r) {
         part[r] = 0.f;
@@ -413,7 +292,6 @@ cgemm_kernel(const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CU
     }
   }
   cluster_sync_all();   // nobody leaves while a peer may still read its tile
-  if (warp == 2) tmem_dealloc(tmem_acc, TMEM_COLS);
 }
 
 static std::atomic<long> g_cgemm_launches{0};
@@ -424,7 +302,7 @@ static void cg_launch(cudaStream_t st, const CUtensorMap& tw, const CUtensorMap&
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(BN >= 64 ? 384 : 256);
+  cfg.blockDim = dim3(384);
   cfg.dynamicSmemBytes = (size_t)dg_smem<BN, STAGES>();
   cfg.stream = st;
   cudaLaunchAttribute attr[2];

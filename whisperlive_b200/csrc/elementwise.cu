@@ -18,7 +18,7 @@ __global__ void cast_weight_kernel(const float* __restrict__ in, __half* __restr
 }
 void cast_weight_f16(cudaStream_t st, const float* in, __half* out, long a, long b, long k) {
   const long n = a * b * k;
-  const int grid = (int)std::min<long>((n + 255) / 256, 148L * 16);
+  const int grid = (int)std::min<long>((n + 255) / 256, 132L * 16);
   cast_weight_kernel<<<grid, 256, 0, st>>>(in, out, n, b, k);
   WL_CUDA(cudaGetLastError());
 }
@@ -130,8 +130,7 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 // Decode-step variant: one block of d/4 threads per row, ONE float4 per thread -- no column loop, no bounds checks, a
 // hundred-odd instructions in all.  The decode step launches this ~100 times per token on a handful of rows; what a
 // launch costs there is the instruction fetch of whatever it executes (the kernels of a layer do not fit the SM's
-// instruction caches together), so it is written for size: round 1's generic version was 11 KB of SASS and took 5 us
-// inside the graph.  It also folds in the residual update that the preceding split-K GEMM left as partial sums:
+// instruction caches together), so it is written for size rather than generality.  It also folds in the residual update that the preceding split-K GEMM left as partial sums:
 // x += bias + sum_s partial_s, in a fixed order (bit-reproducible).
 constexpr int PF_PIECE = 32 * 1024;   // bytes per cp.async.bulk.prefetch.L2
 

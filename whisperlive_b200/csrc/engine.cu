@@ -57,7 +57,7 @@ struct wl_ctx {
   cudaEvent_t pev0 = nullptr, pev1 = nullptr;
   double prof_cross_ms = 0.0;
   long prof_cross_n = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   int d, H, Le, Ld, n_mels, V, Vld, Bm, Km, Rm, NS;
   bool finalized = false;
   std::vector<void*> allocs;
@@ -233,7 +233,7 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     WL_CUDA(cudaSetDevice(cfg->device));
     cudaDeviceProp prop;
     WL_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
-    WL_CHECK(prop.major == 10, WL_ERR_CUDA, "libwlb200 is built for sm_100a only; device is sm_%d%d", prop.major, prop.minor);
+    WL_CHECK(prop.major == 9 && prop.minor == 0, WL_ERR_CUDA, "libwlb200 is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
     c->num_sms = prop.multiProcessorCount;
     c->d = cfg->d_model; c->H = cfg->n_heads; c->Le = cfg->enc_layers; c->Ld = cfg->dec_layers;
     c->n_mels = cfg->n_mels; c->V = cfg->vocab; c->Vld = (cfg->vocab + 3) / 4 * 4;
@@ -484,8 +484,8 @@ extern "C" int wl_finalize_weights(wl_ctx* c) {
 
   // ---- encoder workspaces (EB streams per pass, AB streams per attention sub-pass)
   const int H = c->H;
-  // streams per encoder pass: 16 x 1500 = 24000 rows fill the 148 SMs' tile waves better than 12000 (7 waves at 91 % vs
-  // 13 at 98 % for the 2560-wide projection); the workspaces are ~1 GB at large-v3, nothing next to 180 GB
+  // streams per encoder pass: 16 x 1500 = 24000 rows give the GEMMs many full tile waves on 132 SMs; the workspaces are
+  // ~1 GB at large-v3, small next to 80 GB
   static const int enc_batch = [] { const char* e = getenv("WLB200_ENC_BATCH"); return e ? std::max(1, atoi(e)) : 16; }();
   c->EB = std::min(c->Bm, enc_batch);
   c->AB = std::min(c->EB, d >= 1024 ? 2 : 4);
@@ -578,8 +578,8 @@ extern "C" int wl_mel(wl_ctx* c, const float* pcm, const int64_t* offsets, int32
 }
 
 // K1 with the result kept on the device: PCM up, log-mel stays in HBM until the next wl_mel_device call; the windows the
-// encoder consumes are gathered from it on the device (wl_encode_windows).  Round 1 copied the features to the host,
-// zero-padded them there and copied them back (110 MB of PCIe traffic and ~28 ms per 32-stream step).
+// encoder consumes are gathered from it on the device (wl_encode_windows), instead of copying the features to the host,
+// zero-padding them there and copying them back (110 MB of PCIe traffic per 32-stream step).
 extern "C" int wl_mel_device(wl_ctx* c, const float* pcm, const int64_t* offsets, int32_t B, int32_t* frames_out) {
   API_BEGIN(c)
   WL_CHECK(c->finalized, WL_ERR_STATE, "weights not finalized");
@@ -832,9 +832,8 @@ static int xa_prefetch_streams() {
   const char* e = getenv("WLB200_XA_PREFETCH");
   return e ? atoi(e) : 0;
 }
-// Measured on B200 (bench.py, large-v3, beam 4): the cluster split-K GEMM (cgemm) made the token step SLOWER than split-K
-// partials summed by the consumers -- 3.81 vs 2.87 ms at 32 streams, 262 vs 206 ms per 8-stream batch -- so it is off by
-// default; what it costs is the serial DSMEM reduction and two cluster barriers after the MMAs (DESIGN.md section 5.1).
+// The cluster split-K GEMM (cgemm) is off by default: in place of the consumers summing split-K partials it adds a serial
+// DSMEM reduction and two cluster barriers after the MMAs (DESIGN.md section 5.1).
 static bool cgemm_enabled() {
   const char* e = getenv("WLB200_CGEMM");
   return e ? atoi(e) != 0 : false;
@@ -858,10 +857,9 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
   // ranges and the bias in a fixed order -- no atomics, bit-reproducible, and no separate reduction kernel.
   // part1 holds activations (qkv, q_cross, fc1), part2 the residual updates (out-proj, fc2) until the next LayerNorm.
   // WLB200_FUSE_POST=1 (default OFF): run the LayerNorm-update after out-proj / FC2 and the GELU-cast after FC1 inside
-  // the producing split-K GEMM behind a grid barrier (13 -> 9 launches per layer).  Measured slower on B200 than the
-  // separate kernels chained by programmatic dependent launch (32 streams: 116 vs 99 ms per 26 tokens; 4 streams:
-  // 59 vs 49 ms): the barrier gates every CTA on the slowest one and the row work then runs on 70 CTAs instead of
-  // 128.  Kept as a switch for the round-2 persistent-layer work.
+  // the producing split-K GEMM behind a grid barrier (13 -> 9 launches per layer).  The barrier gates every CTA on the
+  // slowest one and the row work then runs on fewer CTAs than the separate kernels chained by programmatic dependent
+  // launch get.
   static const bool fuse_env = [] { const char* e = getenv("WLB200_FUSE_POST"); return e ? atoi(e) != 0 : false; }();
   static const bool simt_env = [] { const char* e = getenv("WLB200_GEMM_SIMT"); return e && atoi(e) != 0; }();
   const bool fuse = fuse_env && splitk && !simt_env;
@@ -926,12 +924,12 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
   // whose epilogue writes FINAL values (bias, residual, GELU fused), so LayerNorm / attention read one value instead of
   // summing partials and the GELU-cast launch is gone: 12 launches per layer instead of 13, each a fraction of the code.
   static const bool wg_env = [] { const char* e = getenv("WLB200_WGEMM"); return e ? atoi(e) != 0 : true; }();
-  // (one m16 tile only: with two, every CTA re-reads 82 KB of X from L2 and the launch costs 8 us -- measured; rows
-  // 17..32 take the tcgen05 path below until the K split moves into a cluster)
+  // (one m16 tile only: with two, every CTA re-reads 82 KB of X from L2; rows
+  // 17..32 take the wgmma path below until the K split moves into a cluster)
   static const int wg_max_rows = [] { const char* e = getenv("WLB200_WGEMM_ROWS"); return e ? atoi(e) : 16; }();
   const bool use_wg = wg_env && R <= wg_max_rows && wgemm_supported(R, d) && wgemm_supported(R, ff);
   // Above that: split-K partials summed by the consumers (13 launches per layer), or with WLB200_CGEMM=1 cgemm, the
-  // tcgen05 pipeline with the K split inside a cluster (dec_gemm.cu) -- same fused epilogues as wgemm, 12 launches.
+  // wgmma pipeline with the K split inside a cluster (dec_gemm.cu) -- same fused epilogues as wgemm, 12 launches.
   const bool cg_env = cgemm_enabled();
   const bool small = !simt_env && !fuse && (use_wg || cg_env);
   auto plain = [](const float* ptr) { PartialSrc ps; ps.ptr = ptr; ps.nsplit = 1; ps.stride = 0; ps.bias = nullptr; return ps; };

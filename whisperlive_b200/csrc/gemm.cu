@@ -1,8 +1,7 @@
-// tcgen05 GEMM: TMA (SWIZZLE_128B) -> smem ring -> tcgen05.mma (single issuing thread) -> TMEM
-// accumulator -> tcgen05.ld epilogue (bias / GELU / residual / layout transforms fused).
+// wgmma GEMM: TMA (SWIZZLE_128B) -> smem ring -> wgmma (two consumer warpgroups, fp32 accumulators in registers) ->
+// epilogue (bias / GELU / residual / layout transforms fused).
 //
-// CTA = 384 threads: warp0 TMA producer, warp1 MMA issuer, warp2 TMEM allocator, warps4-11 epilogue
-// (lane i of TMEM = accumulator row i; two warps per 32-row group split the columns).  Tile 128 x BN x 64.
+// CTA = 384 threads: warp 0 TMA producer, warps 4-11 two consumer warpgroups of 64 tile rows each.  Tile 128 x BN x 64.
 #include "gemm.cuh"
 
 #include <algorithm>
@@ -42,7 +41,7 @@ enum EpiKind : int { EPI_ROW = 0, EPI_COL = 1, EPI_PART = 2, EPI_HEADSPLIT = 3 }
 
 template <int cnt, int KIND>
 __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int n0, const uint32_t (&v)[cnt], int i1, int i2,
-                                               int split = 0, const float4* rpre = nullptr) {
+                                               int split = 0) {
   const GemmEpilogue& e = p.e;
   if (m >= p.M) return;
   if constexpr (KIND == EPI_PART) {
@@ -115,7 +114,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
       }
       if (e.resid) {
         const float* r = e.resid + rbase + n;
-        const float4 r0 = rpre ? rpre[i / 4] : *reinterpret_cast<const float4*>(r), r1 = rpre ? rpre[i / 4 + 1] : *reinterpret_cast<const float4*>(r + 4);
+        const float4 r0 = *reinterpret_cast<const float4*>(r), r1 = *reinterpret_cast<const float4*>(r + 4);
         x[0] += r0.x; x[1] += r0.y; x[2] += r0.z; x[3] += r0.w;
         x[4] += r1.x; x[5] += r1.y; x[6] += r1.z; x[7] += r1.w;
       }
@@ -285,9 +284,21 @@ __device__ __forceinline__ void tile_decode(const GemmKParams& p, int t, int til
   }
 }
 
+// Epilogue staging: each consumer warpgroup turns its register accumulator into a row per thread through shared memory,
+// EPI_CH columns at a time, so that the epilogue stores whole 16-byte pieces of one output row.
+template <int BN>
+struct EpiStage {
+  static constexpr int CH = BN < 64 ? BN : 64;   // columns per staged chunk
+  static constexpr int LD = CH + 4;              // padded row pitch (floats): conflict-free float4 reads
+  static constexpr int BYTES = 2 * 64 * LD * 4;  // both consumer warpgroups
+};
+template <int BN, int STAGES>
+__host__ __device__ constexpr int gemm_smem_bytes() { return STAGES * (A_STAGE_BYTES + BN * BK * 2) + EpiStage<BN>::BYTES + 1024 + 512; }
+
 // Persistent: each CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  (tile_m fastest, so CTAs
-// running side by side share the B (weight) tile in L2).  Two TMEM accumulator stages: the epilogue warps drain
-// tile i while the MMA warp already accumulates tile i+1.
+// running side by side share the B (weight) tile in L2).
+// CTA = 384 threads: warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 the wgmma consumers of tile rows 0-63 and
+// 64-127, each keeping its 64 x BN fp32 accumulator in registers and running the epilogue of its rows.
 template <int BN, int STAGES, int MIN_CTAS, int KIND>
 __global__ void __launch_bounds__(384, MIN_CTAS)
 gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -295,16 +306,13 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);   // pointer arithmetic keeps the shared address space (LDS/STS)
   constexpr int B_STAGE_BYTES = BN * BK * 2;
-  constexpr uint32_t ACC_COLS = BN < 32 ? 32 : BN;
-  constexpr uint32_t TMEM_COLS = 2 * ACC_COLS;
+  using ES = EpiStage<BN>;
   uint8_t* sA = base;
   uint8_t* sB = base + STAGES * A_STAGE_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_STAGE_BYTES);
+  float* stg_all = reinterpret_cast<float*>(sB + STAGES * B_STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + ES::BYTES);
   uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;   // [2]
-  uint64_t* acc_empty = acc_full + 2;    // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
-  float* post_red = reinterpret_cast<float*>(tmem_slot + 2);   // [16]
+  float* post_red = reinterpret_cast<float*>(empty + STAGES);   // [16]
 
   const int warp = threadIdx.x >> 5;
   const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
@@ -319,22 +327,11 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp == 1 && elect_one()) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full[s], 1);
-      mbar_init(&empty[s], 1);
-    }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&acc_full[s], 1);
-      mbar_init(&acc_empty[s], BN >= 64 ? 8 : 4);
+      mbar_init(&empty[s], 8);   // one arrival per consumer warp
     }
     mbar_fence_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_slot, TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_acc = *tmem_slot;
 
   if (warp == 0) {
     if (elect_one()) {
@@ -388,98 +385,62 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) {
-      constexpr uint32_t idesc = umma_idesc_f16(BM, BN);
-      int stage = 0, as = 0;
-      uint32_t phase = 0, aphase = 0;
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        const int zz = t / (tiles_m * tiles_n);
-        const int kb0 = KIND == EPI_PART ? zz * p.kb_per_split : 0;
-        const int num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - kb0) : total_kb;
-        mbar_wait(&acc_empty[as], aphase ^ 1);   // epilogue has drained this accumulator stage
-        tc_fence_after();
-        const uint32_t acc = tmem_acc + as * ACC_COLS;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          const uint64_t adesc = umma_desc_sw128(smem_u32(sA + stage * A_STAGE_BYTES));
-          const uint64_t bdesc = umma_desc_sw128(smem_u32(sB + stage * B_STAGE_BYTES));
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k) {
-            // advance 16 halves = 32 bytes along K inside the 128-byte swizzle row: +2 in (addr>>4) units
-            umma_f16(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), idesc, (kb | k) != 0 ? 1u : 0u);
-          }
-          umma_commit(&empty[stage]);  // smem slot reusable once these MMAs have read it
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(&acc_full[as]);
-        if (++as == 2) { as = 0; aphase ^= 1; }
-      }
-    }
-  } else if (warp >= 4 && (BN >= 64 || warp < 8)) {
-    // 8 epilogue warps (2 per SM sub-partition): warps 4-7 drain the left half of the accumulator columns,
-    // warps 8-11 the right half; narrow tiles (BN < 64) use warps 4-7 only.
-    const int q = warp & 3;
-    constexpr int NH = BN >= 64 ? 2 : 1, HC = BN / NH;   // column halves, columns per half
-    const int c_lo = ((warp - 4) >> 2) * HC;
-    int as = 0;
-    uint32_t aphase = 0;
+  } else if (warp >= 4) {
+    const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows 64 wg .. 64 wg + 63
+    const int tw = threadIdx.x & 127;
+    float* stg = stg_all + wg * 64 * ES::LD;
+    int stage = 0;
+    uint32_t phase = 0;
     pdl_wait();   // the residual / output buffers belong to the preceding kernels
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
       int tile_m, tile_n, zz;
-        tile_decode(p, t, tiles_m, tiles_n, tile_m, tile_n, zz);
+      tile_decode(p, t, tiles_m, tiles_n, tile_m, tile_n, zz);
       const int z = KIND == EPI_PART ? 0 : zz, split = KIND == EPI_PART ? zz : 0;
       const int i1 = z % p.zn1, i2 = z / p.zn1;
-      mbar_wait(&acc_full[as], aphase);
-      tc_fence_after();
-      const long m = (long)tile_m * BM + q * 32 + lane_id();
-      const uint32_t lane_addr = tmem_acc + as * ACC_COLS + ((uint32_t)(q * 32) << 16);
-      if constexpr (BN >= 32) {
-#pragma unroll 1
-        for (int c = c_lo; c < c_lo + HC; c += 32) {
-          uint32_t v[32];
-          // fp32 residual of this thread's 32 columns: requested before the accumulator read so that the 8 loads
-          // are in flight together (out may alias resid, which keeps the compiler from hoisting them itself)
-          float4 rr[8];
-          bool rr_ok = false;
-          if constexpr (KIND == EPI_ROW) {
-            const int n0 = tile_n * BN + c;
-            if (p.e.resid != nullptr && m < p.M && n0 + 32 <= p.N) {
-              const float4* r4 = reinterpret_cast<const float4*>(p.e.resid + (long)i1 * p.e.rb1 + (long)i2 * p.e.rb2 + m * p.e.rldm + n0);
+      const int kb0 = KIND == EPI_PART ? split * p.kb_per_split : 0;
+      const int num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - kb0) : total_kb;
+      float acc[BN / 2];
 #pragma unroll
-              for (int j = 0; j < 8; ++j) rr[j] = r4[j];
-              rr_ok = true;
-            }
-          }
-          tmem_ld_32x32(lane_addr + c, v);
-          tmem_ld_wait();
-          if (c + 32 >= c_lo + HC) {  // this warp's columns are in registers: hand the TMEM stage back before the stores
-            tc_fence_before();
-            __syncwarp();
-            if (lane_id() == 0) mbar_arrive(&acc_empty[as]);
-          }
-          if constexpr (KIND == EPI_ROW) {
-            if (rr_ok) epilogue_chunk<32, KIND>(p, m, tile_n * BN + c, v, i1, i2, split, rr);
-            else epilogue_chunk<32, KIND>(p, m, tile_n * BN + c, v, i1, i2, split);
-          } else {
-            epilogue_chunk<32, KIND>(p, m, tile_n * BN + c, v, i1, i2, split);
-          }
-        }
-      } else {
-        uint32_t v[16];
-        tmem_ld_32x16(lane_addr, v);
-        tmem_ld_wait();
-        tc_fence_before();
-        __syncwarp();
-        if (lane_id() == 0) mbar_arrive(&acc_empty[as]);
-        epilogue_chunk<16, KIND>(p, m, tile_n * BN, v, i1, i2, split);
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(&full[stage], phase);
+        wgmma_fence();
+        wgmma_tile_k64<BN>(acc, sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, wg, kb > 0);
+        wgmma_commit();
+        // one k-block of MMAs stays in flight; the stage read by the one before it is handed back to the producer
+        wgmma_wait<1>();
+        if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
-      if (++as == 2) { as = 0; aphase ^= 1; }
+      wgmma_wait<0>();
+      wgmma_fence_regs(acc);
+      if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
+      const int row = tw & 63, half = tw >> 6;
+      const long m = (long)tile_m * BM + wg * 64 + row;
+#pragma unroll
+      for (int ch = 0; ch < BN / ES::CH; ++ch) {
+        wgmma_acc_foreach(acc, [&](int r, int c, float v) {
+          if (c >= ch * ES::CH && c < (ch + 1) * ES::CH) stg[r * ES::LD + c - ch * ES::CH] = v;
+        });
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
+        constexpr int CNT = ES::CH / 2;
+        uint32_t v[CNT];
+        const float4* src = reinterpret_cast<const float4*>(stg + row * ES::LD + half * CNT);
+#pragma unroll
+        for (int i = 0; i < CNT / 4; ++i) {
+          const float4 q = src[i];
+          v[4 * i] = __float_as_uint(q.x); v[4 * i + 1] = __float_as_uint(q.y);
+          v[4 * i + 2] = __float_as_uint(q.z); v[4 * i + 3] = __float_as_uint(q.w);
+        }
+        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the next chunk reuses the staging buffer
+        epilogue_chunk<CNT, KIND>(p, m, tile_n * BN + ch * ES::CH + half * CNT, v, i1, i2, split);
+      }
     }
     if constexpr (KIND == EPI_PART) {
       if (p.e.post != GEMM_POST_NONE) {
-        constexpr int NT = BN >= 64 ? 256 : 128;   // epilogue threads of this configuration
+        constexpr int NT = 256;                    // consumer threads
         const int te = threadIdx.x - 128;
         __threadfence();                           // this thread's partial sums are visible device-wide
         epi_sync<NT>();
@@ -489,9 +450,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) tmem_dealloc(tmem_acc, TMEM_COLS);
 }
 
 // ------------------------------------------------------------------------------------ host side
@@ -573,7 +531,7 @@ static TmapInfo get_tmap(const GemmOperand& op, int box_rows, int box_k) {
 
 template <int BN, int STAGES, int MIN_CTAS, int KIND>
 static void launch_cfg(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, int Z) {
-  constexpr int smem = STAGES * (A_STAGE_BYTES + BN * BK * 2) + 1024 + 512;
+  constexpr int smem = gemm_smem_bytes<BN, STAGES>();
   static int sms = 0;
   if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   GemmKParams q = p;
@@ -586,7 +544,7 @@ static void launch_cfg(cudaStream_t stream, const CUtensorMap& ta, const CUtenso
 
 template <int BN, int STAGES, int MIN_CTAS, int KIND>
 static void prime_cfg() {
-  constexpr int smem = STAGES * (A_STAGE_BYTES + BN * BK * 2) + 1024 + 512;
+  constexpr int smem = gemm_smem_bytes<BN, STAGES>();
   WL_CUDA(cudaFuncSetAttribute(gemm_tn_kernel<BN, STAGES, MIN_CTAS, KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
 }
 
@@ -595,9 +553,8 @@ template <int KIND>
 static void prime_kind() {
   prime_cfg<16, 8, 1, KIND>();
   prime_cfg<32, 8, 1, KIND>();
-  prime_cfg<64, 8, 1, KIND>();
+  prime_cfg<64, 6, 1, KIND>();
   prime_cfg<128, 5, 1, KIND>();
-  prime_cfg<256, 4, 1, KIND>();
 }
 void gemm_tl_bind(unsigned long long* p) { tl_bind_tu(p); }
 void gemm_prime() {
@@ -612,9 +569,8 @@ static void launch_kind(int bn, cudaStream_t stream, const CUtensorMap& ta, cons
   switch (bn) {
     case 16: launch_cfg<16, 8, 1, KIND>(stream, ta, tb, p, Z); break;
     case 32: launch_cfg<32, 8, 1, KIND>(stream, ta, tb, p, Z); break;
-    case 64: launch_cfg<64, 8, 1, KIND>(stream, ta, tb, p, Z); break;
+    case 64: launch_cfg<64, 6, 1, KIND>(stream, ta, tb, p, Z); break;
     case 128: launch_cfg<128, 5, 1, KIND>(stream, ta, tb, p, Z); break;
-    case 256: launch_cfg<256, 4, 1, KIND>(stream, ta, tb, p, Z); break;
     default: WL_CHECK(false, WL_ERR_ARG, "unsupported BN %d", bn);
   }
 }
@@ -680,8 +636,7 @@ void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, in
   else if (N <= 16) bn = 16;
   else if (N <= 32) bn = 32;
   else if (N <= 64) bn = 64;
-  else if (N >= 512 && M >= 512 && epi.ldn == 1) bn = 256;
-  else bn = 128;
+  else bn = 128;   // 64 x 128 fp32 accumulator per consumer warpgroup = 64 registers a thread
   if (epi.mode == GEMM_HEADSPLIT && bn < 64) bn = 64;
   if (epi.partials > 0) {
     WL_CHECK(Z == 1 && epi.out_f32 && !epi.gelu && !epi.resid && !epi.bias && epi.mode == GEMM_STORE, WL_ERR_ARG,

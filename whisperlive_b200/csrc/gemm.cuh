@@ -1,4 +1,4 @@
-// tcgen05 / TMA / TMEM GEMM used by every dense contraction on the hot path (K2-K9, K12).
+// TMA / wgmma GEMM used by every dense contraction on the hot path (K2-K9, K12).
 //   C[z][m][n] = epilogue( sum_k A[z][m][k] * B[z][n][k] )      fp16 in, fp32 accumulate
 // Both operands are K-major ("TN"): activations [rows, K] and nn.Linear weights [out, K].
 #pragma once

@@ -3,7 +3,7 @@
 // A prompt of P tokens (sot_prev + hotwords + previous text + sot sequence, up to ~450 tokens:
 // whisper_live/transcriber/transcriber_faster_whisper.py:1480-1513) used to be fed one token per decode step, i.e. P - 1
 // full weight streams before the first generated token.  The prefill pass pushes all prompt positions of all streams
-// through the decoder stack at once -- M = sum(P_b - 1) rows per GEMM on the encoder's tcgen05 kernel, causal
+// through the decoder stack at once -- M = sum(P_b - 1) rows per GEMM on the encoder's wgmma kernel, causal
 // self-attention over the cached positions, cross-attention in groups of 8 rows per K/V stream -- and leaves the
 // self-attention cache and the decode state exactly where token-by-token feeding would have left them.
 //

@@ -396,7 +396,8 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
     for (int p = tid; p <= pos_old; p += 128) sh_src[j][p] = s.src[(long)(row0 + j) * T_MAX + p];
   }
   // candidate lists and cumulative scores of the alive rows -> shared memory with one parallel load: the merge below is
-  // one thread walking <= 8 x 16 entries, and as dependent global loads that walk alone was ~12 us of the token step
+  // one thread walking <= 8 x 16 entries, which as a chain of dependent global loads would sit on the token step's
+  // critical path
   __shared__ float sh_cval[MAX_ROWS_PER_STREAM][MAX_CAND];
   __shared__ int sh_ctok[MAX_ROWS_PER_STREAM][MAX_CAND];
   __shared__ float sh_cum[MAX_ROWS_PER_STREAM];

@@ -5,9 +5,9 @@
 //   * the CTA's whole weight slice (NF output features x <= 1280 of K, <= 105 KB) is requested with cp.async.bulk
 //     BEFORE griddepcontrol.wait, i.e. while the kernel that produces X is still running; after the wait the only
 //     global traffic on the critical path is X itself (16 rows x K fp16, an L2 hit);
-//   * warp-level mma.sync m16n8k16 (M = the 16 decoder rows, N = 8 output features): no TMEM allocation, no tensor
+//   * warp-level mma.sync m16n8k16 (M = the 16 decoder rows, N = 8 output features): no warpgroup MMA, no tensor
 //     maps, no mbarrier ring -- and about 3 KB of SASS (the decode step's launches are instruction-fetch bound, see
-//     dec_gemm.cu); tcgen05's 128-row tiles would be 87 % padding at 16 rows;
+//     dec_gemm.cu); the 128-row wgmma tiles would be 87 % padding at 16 rows;
 //   * the 8 warps split K, reduce through shared memory in a fixed order (bit-reproducible), and the epilogue writes
 //     FINAL values: + bias, + residual (in place), GELU -> fp16, or a raw partial sum when K is split over CTAs
 //     (FC2, K = 4d) -- so LayerNorm, self- and cross-attention read one value instead of summing 4-8 partials,
@@ -190,8 +190,8 @@ void wgemm(cudaStream_t st, const __half* W, int n_out, int K, const __half* X, 
   WgemmParams p;
   p.W = W; p.X = X; p.bias = bias; p.out_f32 = out_f32; p.out_f16 = out_f16; p.part_stride = part_stride;
   p.n_out = n_out; p.K = K; p.R = R; p.ksplit = ksplit; p.mode = mode;
-  // (prefetch_ptr / prefetch_bytes: an L2 prefetch of the next layer's weights from here was measured -- 65.0 vs 64.4 ms
-  // per 42 tokens at 4 streams, no gain: the slices are already requested 3 us ahead of the dependency -- and removed)
+  // (prefetch_ptr / prefetch_bytes: an L2 prefetch of the next layer's weights from here gained nothing -- the slices are
+  // already requested ahead of the dependency -- and was removed)
   (void)prefetch_ptr; (void)prefetch_bytes;
   // K range per CTA: equal ranges, multiples of 32
   p.kr = cdiv(cdiv(K, ksplit), 32) * 32;

@@ -102,7 +102,7 @@ class B200Whisper:
                  compute_type: str = "float16", max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
                  alignment_heads: Optional[List[Tuple[int, int]]] = None, use_cuda_graph: bool = True):
         if compute_type not in ("float16", "default", "auto"):
-            raise ValueError(f"compute_type {compute_type!r}: the B200 engine computes in float16 with fp32 accumulation")
+            raise ValueError(f"compute_type {compute_type!r}: the engine computes in float16 with fp32 accumulation")
         self.lib = _lib.load()
         self.dims = dims
         self.device = "cuda"
@@ -486,7 +486,7 @@ class B200Whisper:
 
     def test_gemm(self, a: np.ndarray, b: np.ndarray, bias: Optional[np.ndarray] = None, transposed_store: bool = False,
                   gelu: bool = False, use_simt: bool = False) -> np.ndarray:
-        """C[z] = A[z] @ B[z]^T through the tcgen05 kernel (or the CUDA-core checker)."""
+        """C[z] = A[z] @ B[z]^T through the wgmma kernel (or the CUDA-core checker)."""
         a16 = np.ascontiguousarray(a, dtype=np.float16)
         b16 = np.ascontiguousarray(b, dtype=np.float16)
         if a16.ndim == 2:

@@ -1,7 +1,7 @@
 """Multi-GPU placement of streams (SURVEY.md §8e): the batch dimension is sharded, nothing else.
 
 Streams are independent units (one WebSocket client each, whisper_live/server.py:344); every tensor op of
-the hot path fits one B200, so there is no tensor/pipeline parallelism and NO data-path collective:
+the hot path fits one H100, so there is no tensor/pipeline parallelism and NO data-path collective:
 weights are replicated, a stream's encoder K/V and self-attention cache live on the GPU that owns it
 (sticky placement ``stream i -> device i mod G``), and the only exchange is one all-gather of the
 emitted token ids (+ segment times) per batch so that every rank -- and the scheduler on rank 0 --

@@ -8,7 +8,7 @@ result records (``Word`` :33, ``Segment`` :49, ``TranscriptionOptions`` :72,
 ``max_length``, ``frames_per_second``, ``_split_segments_by_timestamps``;
 whisper_live/batch_inference.py:257-402).
 
-B200-first differences in *structure* (results are the reference's):
+GPU-first differences in *structure* (results are the reference's):
   * the unit of work is a batch of streams: ``transcribe_batch`` advances every
     stream's 30 s-window state machine in lockstep so mel, encoder and the decode loop
     run once per step for all live streams (the reference loops streams serially, or
