@@ -133,9 +133,17 @@ int wl_align(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* start_
 /* teacher-forced logits: tokens concatenated at tok_off[B+1]; logits_out [sum T, vocab] float32 */
 int wl_decode_logits(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* tokens, const int32_t* tok_off,
                      float* logits_out);
-/* C[z] = A[z] (MxK) * B[z]^T (NxK) (+bias[n]) on the wgmma path (use_simt=0) or the CUDA-core checker */
+/* C[z] = A[z] (MxK) * B[z]^T (NxK) (+bias[n]) on the wgmma path (use_simt=0) or the CUDA-core checker.  opts:
+ *   bits 0-1 output: 0 fp32; 1 fp32 plus the fp32 residual read from c and updated in place; 2 fp16;
+ *            3 fp16 head-split layout (cross-KV cache) of M / hs rows per stream into slots in reverse stream order,
+ *            c = [slot][N / 64][hs][64] with the 16-byte pieces of a row XOR-swizzled by (s & 7), hs = opts >> 8
+ *   bit 2: A is one matrix shared by the batch (a holds M x K); bit 3: the same for B
+ *   bits 4-5 kernel: 0 as gemm_tn picks it, 1 the classic kernel, 2 the ping-pong kernel (N tiles of 128 only)
+ *   bit 6: bias indexed by m with the row-major store (always so with transposed_store) */
 int wl_test_gemm(wl_ctx* ctx, const uint16_t* a_f16, const uint16_t* b_f16, const float* bias, float* c, int32_t M, int32_t N,
-                 int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt);
+                 int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt, int32_t opts);
+/* the GEMM kernel gemm_tn picks for this shape on this device: 1 classic, 2 ping-pong */
+int wl_gemm_variant(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t* variant_out);
 /* test hook of the small-batch decode GEMM (csrc/wgemm.cu, R <= 32): out[R][n_out] = X[R][K] W[n_out][K]^T with the fused
  * epilogue `mode` -- 0: + bias; 1: out += acc + bias (residual in place); 2: gelu(acc + bias) through fp16;
  * 3: split-K partial sums (K > 1280), summed by the hook; mode | 8 (8, 9, 10): the cluster split-K GEMM (cgemm, any R)
@@ -145,7 +153,8 @@ int wl_test_wgemm(wl_ctx* ctx, const uint16_t* w_f16, const uint16_t* x_f16, con
 /* device-resident timing of the GEMM kernel: C = A(MxK) * B(NxK)^T, `iters` launches between CUDA events;
  * bn = 0 picks the tile like the engine does. ms_out = average milliseconds per launch. */
 int wl_bench_gemm(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,
-                  float* ms_out); /* flags: 1 transposed store, 2 bias, 4 GELU, 8 fp32 output + fp32 residual */
+                  float* ms_out); /* flags: 1 transposed store, 2 bias, 4 GELU, 8 fp32 output + fp32 residual,
+                                   16 bias indexed by m, 32 A shared by the batch, 64 output row pitch padded to 64 */
 /* launches of library kernels since wl_init (gpu_launches accounting in bench.py) */
 int64_t wl_kernel_launches(wl_ctx* ctx);
 /* time (ms, CUDA events on the library stream) of the last wl_mel / wl_encode / wl_generate device work;

@@ -64,7 +64,8 @@ SIGNATURES = {
                            C.c_int32, c_i32p, c_f32p]),
     "wl_decode_logits": (C.c_int, [C.c_void_p, c_i32p, C.c_int32, c_i32p, c_i32p, c_f32p]),
     "wl_test_gemm": (C.c_int, [C.c_void_p, c_u16p, c_u16p, c_f32p, c_f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
-                               C.c_int32, C.c_int32, C.c_int32]),
+                               C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "wl_gemm_variant": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_i32p]),
     "wl_test_wgemm": (C.c_int, [C.c_void_p, c_u16p, c_u16p, c_f32p, c_f32p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "wl_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_f32p]),
     "wl_kernel_launches": (C.c_int64, [C.c_void_p]),

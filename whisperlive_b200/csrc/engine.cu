@@ -1858,40 +1858,77 @@ extern "C" int wl_align(wl_ctx* c, const int32_t* slots, int32_t B, const int32_
 
 // ------------------------------------------------------------------------------------------ test hook
 extern "C" int wl_test_gemm(wl_ctx* c, const uint16_t* a_f16, const uint16_t* b_f16, const float* bias, float* cc, int32_t M,
-                            int32_t N, int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt) {
+                            int32_t N, int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt,
+                            int32_t opts) {
   API_BEGIN(c)
-  __half *da = nullptr, *db = nullptr;
+  const int out_kind = opts & 3, variant = (opts >> 4) & 3, hs_S = opts >> 8;
+  const bool a_shared = opts & 4, b_shared = opts & 8, bias_on_m = transposed_store || (opts & 64);
+  const bool f16_out = out_kind == 2 || out_kind == 3;
+  WL_CHECK(variant <= GEMM_PINGPONG && (out_kind != 3 || (hs_S > 0 && M % hs_S == 0 && N % 64 == 0 && batch == 1)), WL_ERR_ARG,
+           "wl_test_gemm: bad opts %d", opts);
+  __half *da = nullptr, *db = nullptr, *dh = nullptr;
   float *dbias = nullptr, *dc = nullptr;
-  const size_t na = (size_t)batch * M * K, nb = (size_t)batch * N * K, nc = (size_t)batch * M * N;
+  int* dslots = nullptr;
+  const size_t na = (size_t)(a_shared ? 1 : batch) * M * K, nb = (size_t)(b_shared ? 1 : batch) * N * K, nc = (size_t)batch * M * N;
   WL_CUDA(cudaMalloc((void**)&da, na * 2));
   WL_CUDA(cudaMalloc((void**)&db, nb * 2));
   WL_CUDA(cudaMalloc((void**)&dc, nc * 4));
+  WL_CUDA(cudaMalloc((void**)&dh, nc * 2));
   WL_CUDA(cudaMemcpy(da, a_f16, na * 2, cudaMemcpyHostToDevice));
   WL_CUDA(cudaMemcpy(db, b_f16, nb * 2, cudaMemcpyHostToDevice));
-  WL_CUDA(cudaMemset(dc, 0, nc * 4));
+  if (out_kind == 1) WL_CUDA(cudaMemcpy(dc, cc, nc * 4, cudaMemcpyHostToDevice));   // the residual, updated in place
+  else WL_CUDA(cudaMemset(dc, 0, nc * 4));
+  WL_CUDA(cudaMemset(dh, 0, nc * 2));
   if (bias) {
     WL_CUDA(cudaMalloc((void**)&dbias, (size_t)std::max(M, N) * 4));
-    WL_CUDA(cudaMemcpy(dbias, bias, (size_t)(transposed_store ? M : N) * 4, cudaMemcpyHostToDevice));
+    WL_CUDA(cudaMemcpy(dbias, bias, (size_t)(bias_on_m ? M : N) * 4, cudaMemcpyHostToDevice));
+  }
+  if (out_kind == 3) {   // head-split into slots in reverse stream order: out[slot][h][s][64], s-swizzled 16-byte pieces
+    const int ns = M / hs_S;
+    std::vector<int> slots(ns);
+    for (int b = 0; b < ns; ++b) slots[b] = ns - 1 - b;
+    WL_CUDA(cudaMalloc((void**)&dslots, ns * sizeof(int)));
+    WL_CUDA(cudaMemcpy(dslots, slots.data(), ns * sizeof(int), cudaMemcpyHostToDevice));
   }
   // the copies / memset above ran on the legacy default stream, the GEMM runs on the library's non-blocking stream:
   // without this the kernel may overtake the memset of its own output buffer
   WL_CUDA(cudaDeviceSynchronize());
   GemmEpilogue e;
-  e.out = dc; e.out_f32 = 1; e.gelu = gelu; e.bias = dbias;
-  if (transposed_store) { e.ldm = 1; e.ldn = M; e.bias_on_m = 1; }   // C^T stored: [N][M]
+  e.out = f16_out ? (void*)dh : (void*)dc; e.out_f32 = f16_out ? 0 : 1; e.gelu = gelu; e.bias = dbias;
+  if (transposed_store) { e.ldm = 1; e.ldn = M; }   // C^T stored: [N][M]
   else { e.ldm = N; e.ldn = 1; }
+  e.bias_on_m = bias_on_m;
   e.ob1 = (long)M * N;
+  if (out_kind == 1) { e.resid = dc; e.rldm = e.ldm; e.rldn = e.ldn; e.rb1 = e.ob1; }
+  if (out_kind == 3) {
+    e.mode = GEMM_HEADSPLIT; e.hs_S = hs_S; e.hs_H = N / 64; e.hs_slot_stride = (long)hs_S * N; e.hs_slots = dslots;
+  }
   try {
-    GemmOperand A = opnd(da, M, K, K, batch, (long)M * K), Bo = opnd(db, N, K, K, batch, (long)N * K);
+    GemmOperand A = opnd(da, M, K, K, batch, a_shared ? 0 : (long)M * K), Bo = opnd(db, N, K, K, batch, b_shared ? 0 : (long)N * K);
+    if (a_shared) A.n1 = 1;
+    if (b_shared) Bo.n1 = 1;
     if (use_simt) gemm_tn_simt(c->st, A, Bo, M, N, K, e);
-    else gemm_tn(c->st, A, Bo, M, N, K, e);
+    else gemm_tn(c->st, A, Bo, M, N, K, e, (GemmVariant)variant);
     WL_CUDA(cudaStreamSynchronize(c->st));
-    WL_CUDA(cudaMemcpy(cc, dc, nc * 4, cudaMemcpyDeviceToHost));
+    if (f16_out) {
+      std::vector<__half> h(nc);
+      WL_CUDA(cudaMemcpy(h.data(), dh, nc * 2, cudaMemcpyDeviceToHost));
+      for (size_t i = 0; i < nc; ++i) cc[i] = __half2float(h[i]);
+    } else {
+      WL_CUDA(cudaMemcpy(cc, dc, nc * 4, cudaMemcpyDeviceToHost));
+    }
   } catch (...) {
-    cudaFree(da); cudaFree(db); cudaFree(dc); if (dbias) cudaFree(dbias);
+    cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dh); if (dbias) cudaFree(dbias); if (dslots) cudaFree(dslots);
     throw;
   }
-  cudaFree(da); cudaFree(db); cudaFree(dc); if (dbias) cudaFree(dbias);
+  cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dh); if (dbias) cudaFree(dbias); if (dslots) cudaFree(dslots);
+  API_END(c)
+}
+
+extern "C" int wl_gemm_variant(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t* variant_out) {
+  API_BEGIN(c)
+  WL_CHECK(variant_out && M > 0 && N > 0 && K > 0 && batch > 0, WL_ERR_ARG, "wl_gemm_variant: bad arguments");
+  *variant_out = (int32_t)gemm_tn_variant(M, N, K, batch);
   API_END(c)
 }
 
@@ -1944,14 +1981,16 @@ extern "C" int wl_test_wgemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x
 
 extern "C" int wl_bench_gemm(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,
                              float* ms_out) {
-  // flags: 1 transposed (swap-AB) store, 2 bias, 4 GELU, 8 fp32 output with fp32 residual (in place)
+  // flags: 1 transposed (swap-AB) store, 2 bias, 4 GELU, 8 fp32 output with fp32 residual (in place), 16 bias on m,
+  // 32 A shared by the batch, 64 output rows padded to a multiple of 64 elements (V^T: S_PAD)
   API_BEGIN(c)
   WL_CHECK(ms_out && M > 0 && N > 0 && K > 0 && batch > 0 && iters > 0, WL_ERR_ARG, "wl_bench_gemm: bad arguments");
   __half *da = nullptr, *db = nullptr;
   void* dc = nullptr;
   float* dbias = nullptr;
-  const bool tr = flags & 1, f32 = flags & 8;
-  const size_t na = (size_t)batch * M * K, nb = (size_t)batch * N * K, nc = (size_t)batch * M * N;
+  const bool tr = flags & 1, f32 = flags & 8, a_shared = flags & 32;
+  const long ld = (flags & 64) ? (N + 63) / 64 * 64 : N;
+  const size_t na = (size_t)(a_shared ? 1 : batch) * M * K, nb = (size_t)batch * N * K, nc = (size_t)batch * M * ld;
   WL_CUDA(cudaMalloc((void**)&da, na * 2));
   WL_CUDA(cudaMalloc((void**)&db, nb * 2));
   WL_CUDA(cudaMalloc(&dc, nc * (f32 ? 4 : 2)));
@@ -1963,13 +2002,13 @@ extern "C" int wl_bench_gemm(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t
   WL_CUDA(cudaDeviceSynchronize());
   GemmEpilogue e;
   e.out = dc; e.out_f32 = f32 ? 1 : 0;
-  if (tr) { e.ldm = 1; e.ldn = M; } else { e.ldm = N; e.ldn = 1; }
-  e.ob1 = (long)M * N;
-  if (flags & 2) { e.bias = dbias; e.bias_on_m = tr ? 1 : 0; }
+  if (tr) { e.ldm = 1; e.ldn = M; } else { e.ldm = ld; e.ldn = 1; }
+  e.ob1 = (long)M * ld;
+  if (flags & 2) { e.bias = dbias; e.bias_on_m = (tr || (flags & 16)) ? 1 : 0; }
   if (flags & 4) e.gelu = 1;
   if (f32) { e.resid = (const float*)dc; e.rldm = e.ldm; e.rldn = e.ldn; e.rb1 = e.ob1; }
   try {
-    GemmOperand A = opnd(da, M, K, K, batch, (long)M * K), Bo = opnd(db, N, K, K, batch, (long)N * K);
+    GemmOperand A = opnd(da, M, K, K, a_shared ? 1 : batch, a_shared ? 0 : (long)M * K), Bo = opnd(db, N, K, K, batch, (long)N * K);
     for (int i = 0; i < 3; ++i) gemm_tn(c->st, A, Bo, M, N, K, e);
     WL_CUDA(cudaEventRecord(c->ev0, c->st));
     for (int i = 0; i < iters; ++i) gemm_tn(c->st, A, Bo, M, N, K, e);

@@ -58,22 +58,30 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
   if constexpr (KIND == EPI_HEADSPLIT && cnt >= 8) {
     // m = (b, s), n = (h, dd); one thread writes cnt (<=32) consecutive dd of one head row.  The 16-byte pieces of a
     // 128-byte key row are stored XOR-swizzled by (s & 7): the layout ldmatrix wants in the cross-attention kernel.
-    const int b = (int)(m / e.hs_S), s = (int)(m % e.hs_S);
+    // The slot index and the bias are all loaded before the first store: the compiler cannot rule out that a store
+    // changes them, so loads placed between the stores would each wait for a round trip to memory.
+    const int mi = (int)m;   // m < M, an int
+    const int b = mi / e.hs_S, s = mi % e.hs_S;
     const int h = n0 >> 6, dd = n0 & 63;
-    __half* dst = (__half*)e.out + (long)e.hs_slots[b] * e.hs_slot_stride + ((long)h * e.hs_S + s) * 64;
+    const long slot = e.hs_slots[b];
+    float x[cnt];
+#pragma unroll
+    for (int i = 0; i < cnt; ++i) x[i] = __uint_as_float(v[i]);
+    if (e.bias) {
+#pragma unroll
+      for (int i = 0; i < cnt; i += 8) {
+        if (n0 + i >= p.N) break;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) x[i + j] += e.bias[n0 + i + j];
+      }
+    }
+    __half* dst = (__half*)e.out + slot * e.hs_slot_stride + ((long)h * e.hs_S + s) * 64;
 #pragma unroll
     for (int i = 0; i < cnt; i += 8) {
       if (n0 + i >= p.N) break;
       __align__(16) __half2 h2[4];
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float a = __uint_as_float(v[i + 2 * j]), c = __uint_as_float(v[i + 2 * j + 1]);
-        if (e.bias) {
-          a += e.bias[n0 + i + 2 * j];
-          c += e.bias[n0 + i + 2 * j + 1];
-        }
-        h2[j] = __floats2half2_rn(a, c);
-      }
+      for (int j = 0; j < 4; ++j) h2[j] = __floats2half2_rn(x[i + 2 * j], x[i + 2 * j + 1]);
       *reinterpret_cast<uint4*>(dst + ((((dd + i) >> 3) ^ (s & 7)) << 3)) = *reinterpret_cast<const uint4*>(h2);
     }
     return;
@@ -82,6 +90,49 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
   const long rbase = (long)i1 * e.rb1 + (long)i2 * e.rb2 + m * e.rldm;
   const float bm = (e.bias && e.bias_on_m) ? e.bias[m] : 0.f;
   if constexpr (KIND == EPI_ROW && cnt >= 8) {
+    if (n0 + cnt <= p.N) {
+      // The whole piece is inside the tile: every load (bias, residual) is issued before the first store.  The output
+      // may be the residual itself (in place), so the compiler keeps a load that follows a store behind it, and loads
+      // interleaved with the stores would cost one round trip to memory per 8 columns.  Same arithmetic, same order.
+      float x[cnt];
+#pragma unroll
+      for (int i = 0; i < cnt; ++i) x[i] = __uint_as_float(v[i]) + bm;
+      if (e.bias && !e.bias_on_m) {
+#pragma unroll
+        for (int i = 0; i < cnt; i += 4) {
+          const float4 b4 = *reinterpret_cast<const float4*>(e.bias + n0 + i);
+          x[i] += b4.x; x[i + 1] += b4.y; x[i + 2] += b4.z; x[i + 3] += b4.w;
+        }
+      }
+      if (e.gelu) {
+#pragma unroll
+        for (int i = 0; i < cnt; ++i) x[i] = gelu_erf(x[i]);
+      }
+      if (e.resid) {
+        const float* r = e.resid + rbase + n0;
+        float4 r4[cnt / 4];
+#pragma unroll
+        for (int i = 0; i < cnt / 4; ++i) r4[i] = *reinterpret_cast<const float4*>(r + 4 * i);
+#pragma unroll
+        for (int i = 0; i < cnt / 4; ++i) {
+          x[4 * i] += r4[i].x; x[4 * i + 1] += r4[i].y; x[4 * i + 2] += r4[i].z; x[4 * i + 3] += r4[i].w;
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < cnt; i += 8) {
+        if (e.out_f32) {
+          float* o = (float*)e.out + obase + n0 + i;
+          *reinterpret_cast<float4*>(o) = make_float4(x[i], x[i + 1], x[i + 2], x[i + 3]);
+          *reinterpret_cast<float4*>(o + 4) = make_float4(x[i + 4], x[i + 5], x[i + 6], x[i + 7]);
+        } else {
+          __align__(16) __half2 h2[4];
+#pragma unroll
+          for (int j = 0; j < 4; ++j) h2[j] = __floats2half2_rn(x[i + 2 * j], x[i + 2 * j + 1]);
+          *reinterpret_cast<uint4*>((__half*)e.out + obase + n0 + i) = *reinterpret_cast<const uint4*>(h2);
+        }
+      }
+      return;
+    }
 #pragma unroll
     for (int i = 0; i < cnt; i += 8) {
       const int n = n0 + i;
@@ -295,6 +346,106 @@ struct EpiStage {
 template <int BN, int STAGES>
 __host__ __device__ constexpr int gemm_smem_bytes() { return STAGES * (A_STAGE_BYTES + BN * BK * 2) + EpiStage<BN>::BYTES + 1024 + 512; }
 
+// Where tile t's operands and output sit: batch entry (i1, i2), K range [kb0, kb0 + num_kb) in k-blocks.
+struct TileCoord {
+  int tile_m, tile_n, split, i1, i2, kb0, num_kb;
+};
+template <int KIND>
+__device__ __forceinline__ TileCoord tile_coord(const GemmKParams& p, int t, int tiles_m, int tiles_n, int total_kb) {
+  TileCoord c;
+  int zz;
+  tile_decode(p, t, tiles_m, tiles_n, c.tile_m, c.tile_n, zz);
+  const int z = KIND == EPI_PART ? 0 : zz;
+  c.split = KIND == EPI_PART ? zz : 0;
+  c.i1 = z % p.zn1;
+  c.i2 = z / p.zn1;
+  c.kb0 = KIND == EPI_PART ? c.split * p.kb_per_split : 0;
+  c.num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - c.kb0) : total_kb;
+  return c;
+}
+
+// TMA producer (one elected thread): fills the stage ring with the k-blocks of this CTA's tiles t = blockIdx.x,
+// blockIdx.x + gridDim.x, ... in that order, each stage once its consumers have handed it back.
+template <int BN, int STAGES, int KIND>
+__device__ __forceinline__ void gemm_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmKParams& p, uint8_t* sA,
+                                             uint8_t* sB, uint64_t* full, uint64_t* empty, int tiles_m, int tiles_n,
+                                             int total_tiles, int total_kb) {
+  constexpr int B_STAGE_BYTES = BN * BK * 2;
+  int stage = 0;
+  uint32_t phase = 0;
+  bool first = true;
+  // coordinate slot s (1..3) of a tensor map holds whichever of (row, i1, i2) was sorted there
+  auto slot = [](const int (&pos)[3], int s, int row, int j1, int j2) {
+    return pos[0] == s ? row : (pos[1] == s ? j1 : (pos[2] == s ? j2 : 0));
+  };
+  for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
+    const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
+    const int a1 = p.a_batched ? tc.i1 : 0, a2 = p.a_batched ? tc.i2 : 0;
+    const int b1 = p.b_batched ? tc.i1 : 0, b2 = p.b_batched ? tc.i2 : 0;
+    const int ca1 = slot(p.a_pos, 1, tc.tile_m * BM, a1, a2), ca2 = slot(p.a_pos, 2, tc.tile_m * BM, a1, a2),
+              ca3 = slot(p.a_pos, 3, tc.tile_m * BM, a1, a2);
+    const int cb1 = slot(p.b_pos, 1, tc.tile_n * BN, b1, b2), cb2 = slot(p.b_pos, 2, tc.tile_n * BN, b1, b2),
+              cb3 = slot(p.b_pos, 3, tc.tile_n * BN, b1, b2);
+    int pre = 0;
+    if (first) {
+      // First tile of this CTA.  When A is a weight matrix (decode: swap-AB, A = W) its k-blocks are requested
+      // BEFORE the dependency wait, so the weight stream overlaps the tail of the kernel that produces B.
+      if (p.e.a_static) {
+        pre = min(tc.num_kb, STAGES);
+        for (int kb = 0; kb < pre; ++kb) {
+          mbar_expect_tx(&full[kb], A_STAGE_BYTES + B_STAGE_BYTES);
+          tma_load_4d(sA + kb * A_STAGE_BYTES, tmA, &full[kb], (tc.kb0 + kb) * BK, ca1, ca2, ca3);
+        }
+      }
+      if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 0);
+      pdl_wait();
+      if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 1);
+      first = false;
+    }
+    for (int kb = 0; kb < tc.num_kb; ++kb) {
+      const int k0 = (tc.kb0 + kb) * BK;
+      if (kb < pre) {
+        tma_load_4d(sB + stage * B_STAGE_BYTES, tmB, &full[stage], k0, cb1, cb2, cb3);
+      } else {
+        mbar_wait(&empty[stage], phase ^ 1);
+        mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
+        tma_load_4d(sA + stage * A_STAGE_BYTES, tmA, &full[stage], k0, ca1, ca2, ca3);
+        tma_load_4d(sB + stage * B_STAGE_BYTES, tmB, &full[stage], k0, cb1, cb2, cb3);
+      }
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+  }
+}
+
+// Epilogue of 64 tile rows (m0 .. m0 + 63) held by one consumer warpgroup as a 64 x BN accumulator fragment: through the
+// warpgroup's staging buffer, ES::CH columns at a time, so that each thread stores whole 16-byte pieces of one output row.
+// bar_id: the warpgroup's own named barrier (128 threads).
+template <int BN, int KIND>
+__device__ __forceinline__ void epilogue_rows64(const GemmKParams& p, const float (&acc)[BN / 2], float* stg, int bar_id, long m0,
+                                                int n0, int i1, int i2, int split) {
+  using ES = EpiStage<BN>;
+  const int tw = threadIdx.x & 127;
+  const int row = tw & 63, half = tw >> 6;
+#pragma unroll
+  for (int ch = 0; ch < BN / ES::CH; ++ch) {
+    wgmma_acc_foreach(acc, [&](int r, int c, float v) {
+      if (c >= ch * ES::CH && c < (ch + 1) * ES::CH) stg[r * ES::LD + c - ch * ES::CH] = v;
+    });
+    named_bar_sync(bar_id, 128);
+    constexpr int CNT = ES::CH / 2;
+    uint32_t v[CNT];
+    const float4* src = reinterpret_cast<const float4*>(stg + row * ES::LD + half * CNT);
+#pragma unroll
+    for (int i = 0; i < CNT / 4; ++i) {
+      const float4 q = src[i];
+      v[4 * i] = __float_as_uint(q.x); v[4 * i + 1] = __float_as_uint(q.y);
+      v[4 * i + 2] = __float_as_uint(q.z); v[4 * i + 3] = __float_as_uint(q.w);
+    }
+    named_bar_sync(bar_id, 128);   // the next chunk reuses the staging buffer
+    epilogue_chunk<CNT, KIND>(p, m0 + row, n0 + ch * ES::CH + half * CNT, v, i1, i2, split);
+  }
+}
+
 // Persistent: each CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ...  (tile_m fastest, so CTAs
 // running side by side share the B (weight) tile in L2).
 // CTA = 384 threads: warp 0 TMA producer (warps 1-3 idle), warpgroups 1 and 2 the wgmma consumers of tile rows 0-63 and
@@ -334,76 +485,20 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
 
   if (warp == 0) {
-    if (elect_one()) {
-      int stage = 0;
-      uint32_t phase = 0;
-      bool first = true;
-      // coordinate slot s (1..3) of a tensor map holds whichever of (row, i1, i2) was sorted there
-      auto slot = [](const int (&pos)[3], int s, int row, int j1, int j2) {
-        return pos[0] == s ? row : (pos[1] == s ? j1 : (pos[2] == s ? j2 : 0));
-      };
-      for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-        int tile_m, tile_n, zz;
-        tile_decode(p, t, tiles_m, tiles_n, tile_m, tile_n, zz);
-        const int z = KIND == EPI_PART ? 0 : zz, split = KIND == EPI_PART ? zz : 0;
-        const int i1 = z % p.zn1, i2 = z / p.zn1;
-        const int kb0 = KIND == EPI_PART ? split * p.kb_per_split : 0;
-        const int num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - kb0) : total_kb;
-        const int a1 = p.a_batched ? i1 : 0, a2 = p.a_batched ? i2 : 0;
-        const int b1 = p.b_batched ? i1 : 0, b2 = p.b_batched ? i2 : 0;
-        const int ca1 = slot(p.a_pos, 1, tile_m * BM, a1, a2), ca2 = slot(p.a_pos, 2, tile_m * BM, a1, a2),
-                  ca3 = slot(p.a_pos, 3, tile_m * BM, a1, a2);
-        const int cb1 = slot(p.b_pos, 1, tile_n * BN, b1, b2), cb2 = slot(p.b_pos, 2, tile_n * BN, b1, b2),
-                  cb3 = slot(p.b_pos, 3, tile_n * BN, b1, b2);
-        int pre = 0;
-        if (first) {
-          // First tile of this CTA.  When A is a weight matrix (decode: swap-AB, A = W) its k-blocks are requested
-          // BEFORE the dependency wait, so the weight stream overlaps the tail of the kernel that produces B.
-          if (p.e.a_static) {
-            pre = min(num_kb, STAGES);
-            for (int kb = 0; kb < pre; ++kb) {
-              mbar_expect_tx(&full[kb], A_STAGE_BYTES + B_STAGE_BYTES);
-              tma_load_4d(sA + kb * A_STAGE_BYTES, &tmA, &full[kb], (kb0 + kb) * BK, ca1, ca2, ca3);
-            }
-          }
-          if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 0);
-          pdl_wait();
-          if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 1);
-          first = false;
-        }
-        for (int kb = 0; kb < num_kb; ++kb) {
-          const int k0 = (kb0 + kb) * BK;
-          if (kb < pre) {
-            tma_load_4d(sB + stage * B_STAGE_BYTES, &tmB, &full[stage], k0, cb1, cb2, cb3);
-          } else {
-            mbar_wait(&empty[stage], phase ^ 1);
-            mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
-            tma_load_4d(sA + stage * A_STAGE_BYTES, &tmA, &full[stage], k0, ca1, ca2, ca3);
-            tma_load_4d(sB + stage * B_STAGE_BYTES, &tmB, &full[stage], k0, cb1, cb2, cb3);
-          }
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
+    if (elect_one()) gemm_produce<BN, STAGES, KIND>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
   } else if (warp >= 4) {
     const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows 64 wg .. 64 wg + 63
-    const int tw = threadIdx.x & 127;
     float* stg = stg_all + wg * 64 * ES::LD;
     int stage = 0;
     uint32_t phase = 0;
     pdl_wait();   // the residual / output buffers belong to the preceding kernels
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      int tile_m, tile_n, zz;
-      tile_decode(p, t, tiles_m, tiles_n, tile_m, tile_n, zz);
-      const int z = KIND == EPI_PART ? 0 : zz, split = KIND == EPI_PART ? zz : 0;
-      const int i1 = z % p.zn1, i2 = z / p.zn1;
-      const int kb0 = KIND == EPI_PART ? split * p.kb_per_split : 0;
-      const int num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - kb0) : total_kb;
+      const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
+      for (int kb = 0; kb < tc.num_kb; ++kb) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
         wgmma_tile_k64<BN>(acc, sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, wg, kb > 0);
@@ -417,26 +512,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
-      const int row = tw & 63, half = tw >> 6;
-      const long m = (long)tile_m * BM + wg * 64 + row;
-#pragma unroll
-      for (int ch = 0; ch < BN / ES::CH; ++ch) {
-        wgmma_acc_foreach(acc, [&](int r, int c, float v) {
-          if (c >= ch * ES::CH && c < (ch + 1) * ES::CH) stg[r * ES::LD + c - ch * ES::CH] = v;
-        });
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");
-        constexpr int CNT = ES::CH / 2;
-        uint32_t v[CNT];
-        const float4* src = reinterpret_cast<const float4*>(stg + row * ES::LD + half * CNT);
-#pragma unroll
-        for (int i = 0; i < CNT / 4; ++i) {
-          const float4 q = src[i];
-          v[4 * i] = __float_as_uint(q.x); v[4 * i + 1] = __float_as_uint(q.y);
-          v[4 * i + 2] = __float_as_uint(q.z); v[4 * i + 3] = __float_as_uint(q.w);
-        }
-        asm volatile("bar.sync %0, 128;" ::"r"(1 + wg) : "memory");   // the next chunk reuses the staging buffer
-        epilogue_chunk<CNT, KIND>(p, m, tile_n * BN + ch * ES::CH + half * CNT, v, i1, i2, split);
-      }
+      epilogue_rows64<BN, KIND>(p, acc, stg, 1 + wg, (long)tc.tile_m * BM + wg * 64, tc.tile_n * BN, tc.i1, tc.i2, tc.split);
     }
     if constexpr (KIND == EPI_PART) {
       if (p.e.post != GEMM_POST_NONE) {
@@ -449,6 +525,99 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         post_op<NT>(p, te, post_red);
       }
     }
+  }
+}
+
+// Ping-pong variant for problems with at least two 128 x 128 tiles per CTA.  Each consumer warpgroup owns whole tiles:
+// warpgroup c takes tiles j = c, c + 2, c + 4, ... of the CTA's sequence t_j = blockIdx.x + j gridDim.x, so while one
+// runs its epilogue the other keeps the tensor cores busy.  An ordered pair of named barriers (PP_BAR + c) hands the
+// math phase from one warpgroup to the other: the producer fills the ring in tile order, and a warpgroup may only wait
+// on a stage's `full` barrier once every earlier use of that stage has been consumed.  Every output element sees the
+// same m64n128k16 sequence and the same epilogue arithmetic as in gemm_tn_kernel<128, ..>: the results are identical.
+// Registers: the producer warpgroup drops to PP_PRODUCER_REGS, the consumers (2 x 64 accumulators a thread) rise to
+// PP_CONSUMER_REGS; 128 x 40 + 256 x 232 <= 64 K.
+constexpr int PP_STAGES = 5;   // 5 x 32 KB ring + 2 x 17 KB staging: the most that fits 227 KB
+constexpr int PP_BAR = 4;      // named barriers 4, 5 (1, 2: per-warpgroup epilogue staging, 3: epi_sync)
+constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;
+
+template <int KIND>
+__global__ void __launch_bounds__(384, 1)
+gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                     const __grid_constant__ GemmKParams p) {
+  static_assert(KIND != EPI_PART, "split-K partials stay on gemm_tn_kernel");
+  constexpr int BN = 128, STAGES = PP_STAGES;
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  constexpr int B_STAGE_BYTES = BN * BK * 2;
+  using ES = EpiStage<BN>;
+  uint8_t* sA = base;
+  uint8_t* sB = base + STAGES * A_STAGE_BYTES;
+  float* stg_all = reinterpret_cast<float*>(sB + STAGES * B_STAGE_BYTES);
+  uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + ES::BYTES);
+  uint64_t* empty = full + STAGES;
+
+  const int warp = threadIdx.x >> 5;
+  const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
+  const int total_tiles = tiles_m * tiles_n * p.nz;
+  const int total_kb = (p.K + BK - 1) / BK;
+  pdl_trigger();
+
+  if (warp == 0 && elect_one()) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+  }
+  if (warp == 1 && elect_one()) {
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(&full[s], 1);
+      mbar_init(&empty[s], 4);   // one arrival per warp of the warpgroup that consumed the stage
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    setmaxnreg_dec<PP_PRODUCER_REGS>();
+    if (warp == 0 && elect_one())
+      gemm_produce<BN, STAGES, KIND>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
+    return;
+  }
+  setmaxnreg_inc<PP_CONSUMER_REGS>();
+  const int wg = (warp >> 2) - 1;
+  float* stg = stg_all + wg * 64 * ES::LD;
+  pdl_wait();   // the residual / output buffers belong to the preceding kernels
+  if (wg == 1) named_bar_arrive(PP_BAR, 256);   // warpgroup 0 takes the first tile (grid <= tiles: it exists)
+  for (int j = wg, t = blockIdx.x + wg * gridDim.x; t < total_tiles; j += 2, t += 2 * gridDim.x) {
+    const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
+    // every tile has total_kb k-blocks: tile j starts at ring position j * total_kb
+    const long it0 = (long)j * total_kb;
+    int stage = (int)(it0 % STAGES);
+    uint32_t phase = (uint32_t)((it0 / STAGES) & 1);
+    float acc[2][BN / 2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
+    named_bar_sync(PP_BAR + wg, 256);   // our turn: the other warpgroup has issued all MMAs of tile j - 1
+    int prev = -1;
+    for (int kb = 0; kb < tc.num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      wgmma_fence();
+      wgmma_tile_k64<BN>(acc[0], sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, 0, kb > 0);
+      wgmma_tile_k64<BN>(acc[1], sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, 1, kb > 0);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
+      prev = stage;
+      if (++stage == STAGES) { stage = 0; phase ^= 1; }
+    }
+    if (t + gridDim.x < total_tiles) named_bar_arrive(PP_BAR + (wg ^ 1), 256);   // tile j + 1 may start its MMAs
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc[0]);
+    wgmma_fence_regs(acc[1]);
+    if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      epilogue_rows64<BN, KIND>(p, acc[h], stg, 1 + wg, (long)tc.tile_m * BM + h * 64, tc.tile_n * BN, tc.i1, tc.i2, 0);
   }
 }
 
@@ -529,16 +698,31 @@ static TmapInfo get_tmap(const GemmOperand& op, int box_rows, int box_k) {
   return info;
 }
 
+static int num_sms() {
+  static int sms = 0;
+  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
+  return sms;
+}
+
 template <int BN, int STAGES, int MIN_CTAS, int KIND>
 static void launch_cfg(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, int Z) {
   constexpr int smem = gemm_smem_bytes<BN, STAGES>();
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
   GemmKParams q = p;
   q.nz = Z;
   const long tiles = (long)cdiv(p.N, BN) * cdiv(p.M, BM) * Z;
-  const int grid = (int)std::min<long>(tiles, (long)sms * MIN_CTAS);
+  const int grid = (int)std::min<long>(tiles, (long)num_sms() * MIN_CTAS);
   launch_kernel(gemm_tn_kernel<BN, STAGES, MIN_CTAS, KIND>, dim3(grid), dim3(384), (size_t)smem, stream, ta, tb, q);
+  g_gemm_launches++;
+}
+
+template <int KIND>
+static void launch_pingpong(cudaStream_t stream, const CUtensorMap& ta, const CUtensorMap& tb, const GemmKParams& p, int Z) {
+  constexpr int smem = gemm_smem_bytes<128, PP_STAGES>();
+  GemmKParams q = p;
+  q.nz = Z;
+  const long tiles = (long)cdiv(p.N, 128) * cdiv(p.M, BM) * Z;
+  const int grid = (int)std::min<long>(tiles, num_sms());
+  launch_kernel(gemm_pingpong_kernel<KIND>, dim3(grid), dim3(384), (size_t)smem, stream, ta, tb, q);
   g_gemm_launches++;
 }
 
@@ -557,11 +741,19 @@ static void prime_kind() {
   prime_cfg<128, 5, 1, KIND>();
 }
 void gemm_tl_bind(unsigned long long* p) { tl_bind_tu(p); }
+template <int KIND>
+static void prime_pingpong() {
+  constexpr int smem = gemm_smem_bytes<128, PP_STAGES>();
+  WL_CUDA(cudaFuncSetAttribute(gemm_pingpong_kernel<KIND>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+}
 void gemm_prime() {
   prime_kind<EPI_ROW>();
   prime_kind<EPI_COL>();
   prime_kind<EPI_PART>();
   prime_kind<EPI_HEADSPLIT>();
+  prime_pingpong<EPI_ROW>();
+  prime_pingpong<EPI_COL>();
+  prime_pingpong<EPI_HEADSPLIT>();
 }
 
 template <int KIND>
@@ -625,18 +817,31 @@ int gemm_split_plan(int M, int N, int K) {
   return cdiv(total_kb, kbs);
 }
 
-void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K, const GemmEpilogue& epi) {
+static int pick_bn(int N) {
+  static const int force_bn = env_int("WLB200_BN", 0);
+  if (force_bn) return force_bn;
+  if (N <= 16) return 16;
+  if (N <= 32) return 32;
+  if (N <= 64) return 64;
+  return 128;   // 64 x 128 fp32 accumulator per consumer warpgroup = 64 registers a thread
+}
+
+// Ping-pong only pays when each CTA has a second tile whose MMAs can hide the first one's epilogue.
+static bool pingpong_pays(int bn, long tiles) { return bn == 128 && tiles >= 2L * num_sms(); }
+
+GemmVariant gemm_tn_variant(int M, int N, int K, int Z) {
+  (void)K;
+  const int bn = pick_bn(N);
+  return pingpong_pays(bn, (long)cdiv(M, BM) * cdiv(N, bn) * Z) ? GEMM_PINGPONG : GEMM_CLASSIC;
+}
+
+void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K, const GemmEpilogue& epi,
+             GemmVariant variant) {
   static const int force_simt = env_int("WLB200_GEMM_SIMT", 0);
   if (force_simt) return gemm_tn_simt(stream, A, B, M, N, K, epi);
   int Z;
   GemmKParams p = make_params(A, B, M, N, K, epi, &Z);
-  static const int force_bn = env_int("WLB200_BN", 0);
-  int bn;
-  if (force_bn) bn = force_bn;
-  else if (N <= 16) bn = 16;
-  else if (N <= 32) bn = 32;
-  else if (N <= 64) bn = 64;
-  else bn = 128;   // 64 x 128 fp32 accumulator per consumer warpgroup = 64 registers a thread
+  int bn = pick_bn(N);
   if (epi.mode == GEMM_HEADSPLIT && bn < 64) bn = 64;
   if (epi.partials > 0) {
     WL_CHECK(Z == 1 && epi.out_f32 && !epi.gelu && !epi.resid && !epi.bias && epi.mode == GEMM_STORE, WL_ERR_ARG,
@@ -661,7 +866,17 @@ void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, in
   const CUtensorMap& ta = ia.tm;
   const CUtensorMap& tb = ib.tm;
   for (int i = 0; i < 3; ++i) { p.a_pos[i] = ia.pos[i]; p.b_pos[i] = ib.pos[i]; }
-  if (p.accum) launch_kind<EPI_PART>(bn, stream, ta, tb, p, Z);
+  bool pingpong = !p.accum && pingpong_pays(bn, (long)cdiv(M, BM) * cdiv(N, bn) * Z);
+  if (variant != GEMM_AUTO) {
+    WL_CHECK(variant == GEMM_CLASSIC || (!p.accum && bn == 128), WL_ERR_ARG,
+             "gemm_tn: the ping-pong kernel needs N tiles of 128 and no split-K");
+    pingpong = variant == GEMM_PINGPONG;
+  }
+  if (pingpong) {
+    if (epi.mode == GEMM_HEADSPLIT) launch_pingpong<EPI_HEADSPLIT>(stream, ta, tb, p, Z);
+    else if (p.vec_ok) launch_pingpong<EPI_ROW>(stream, ta, tb, p, Z);
+    else launch_pingpong<EPI_COL>(stream, ta, tb, p, Z);
+  } else if (p.accum) launch_kind<EPI_PART>(bn, stream, ta, tb, p, Z);
   else if (epi.mode == GEMM_HEADSPLIT) launch_kind<EPI_HEADSPLIT>(bn, stream, ta, tb, p, Z);
   else if (p.vec_ok) launch_kind<EPI_ROW>(bn, stream, ta, tb, p, Z);
   else launch_kind<EPI_COL>(bn, stream, ta, tb, p, Z);

@@ -57,9 +57,16 @@ struct GemmEpilogue {
   const int* hs_slots = nullptr;  // device: slot index per stream b
 };
 
+// Which persistent wgmma kernel runs a GEMM (gemm.cu).  CLASSIC: both consumer warpgroups share each 128 x BN tile.
+// PINGPONG: each warpgroup owns whole 128 x 128 tiles and its epilogue overlaps the other's MMAs; chosen when every CTA
+// gets at least two tiles and there is no split-K.  AUTO picks from the shape; the others force one (tests).
+enum GemmVariant : int { GEMM_AUTO = 0, GEMM_CLASSIC = 1, GEMM_PINGPONG = 2 };
+
 // Launch on `stream`. M/N/K are the logical sizes per batch entry. Throws wl::Error.
 void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K,
-             const GemmEpilogue& epi);
+             const GemmEpilogue& epi, GemmVariant variant = GEMM_AUTO);
+// The variant GEMM_AUTO selects for a non-split-K GEMM of this shape (Z batch entries).
+GemmVariant gemm_tn_variant(int M, int N, int K, int Z);
 
 // Plain CUDA-core reference of the same contract (debug/bisect aid on the GPU box, WLB200_GEMM=simt;
 // also what the GEMM unit test compares against on-device).

@@ -484,25 +484,53 @@ class B200Whisper:
             _lib.check(self.lib, self.ctx, rc, "wl_test_wgemm")
         return out
 
+    GEMM_OUT = {"f32": 0, "resid": 1, "f16": 2, "headsplit": 3}
+    GEMM_VARIANT = {"auto": 0, "classic": 1, "pingpong": 2}
+
     def test_gemm(self, a: np.ndarray, b: np.ndarray, bias: Optional[np.ndarray] = None, transposed_store: bool = False,
-                  gelu: bool = False, use_simt: bool = False) -> np.ndarray:
-        """C[z] = A[z] @ B[z]^T through the wgmma kernel (or the CUDA-core checker)."""
+                  gelu: bool = False, use_simt: bool = False, out: str = "f32", resid: Optional[np.ndarray] = None,
+                  batch: Optional[int] = None, hs_rows: int = 0, variant: str = "auto", bias_on_m: bool = False) -> np.ndarray:
+        """C[z] = A[z] @ B[z]^T through the wgmma kernel (or the CUDA-core checker).
+
+        out: "f32"; "resid" (C += the fp32 `resid`, in place); "f16"; "headsplit" (fp16 cross-KV layout of `hs_rows`
+        rows per stream, returned raw: [slot][N / 64][hs_rows][64], slots in reverse stream order, see wlb200.h).
+        batch: Z when one of a, b is a single 2-D matrix shared by the batch.  variant: "auto", "classic", "pingpong".
+        bias_on_m: bias indexed by m (implied by transposed_store)."""
         a16 = np.ascontiguousarray(a, dtype=np.float16)
         b16 = np.ascontiguousarray(b, dtype=np.float16)
-        if a16.ndim == 2:
-            a16, b16 = a16[None], b16[None]
-        Z, M, K = a16.shape
-        N = b16.shape[1]
-        c = np.zeros((Z, N, M) if transposed_store else (Z, M, N), dtype=np.float32)
+        if batch is None:
+            if a16.ndim == 2:
+                a16, b16 = a16[None], b16[None]
+            Z = a16.shape[0]
+        else:
+            Z = batch
+        a_shared, b_shared = a16.ndim == 2, b16.ndim == 2
+        M, K = a16.shape[-2:]
+        N = b16.shape[-2]
+        if resid is not None:
+            c = np.ascontiguousarray(resid, dtype=np.float32).reshape((Z, N, M) if transposed_store else (Z, M, N)).copy()
+        else:
+            c = np.zeros((Z, N, M) if transposed_store else (Z, M, N), dtype=np.float32)
+        opts = (self.GEMM_OUT[out] | (4 if a_shared else 0) | (8 if b_shared else 0) | (self.GEMM_VARIANT[variant] << 4)
+                | (64 if bias_on_m else 0) | (hs_rows << 8))
         bp = None
         if bias is not None:
             bias = np.ascontiguousarray(bias, dtype=np.float32)
             bp = _lib.ptr(bias, C.c_float)
         with self._lock:
             rc = self.lib.wl_test_gemm(self.ctx, _lib.ptr(a16.view(np.uint16), C.c_uint16), _lib.ptr(b16.view(np.uint16), C.c_uint16),
-                                       bp, _lib.ptr(c, C.c_float), M, N, K, Z, int(transposed_store), int(gelu), int(use_simt))
+                                       bp, _lib.ptr(c, C.c_float), M, N, K, Z, int(transposed_store), int(gelu), int(use_simt),
+                                       opts)
             _lib.check(self.lib, self.ctx, rc, "wl_test_gemm")
         return c
+
+    def gemm_variant(self, M: int, N: int, K: int, batch: int = 1) -> str:
+        """Which GEMM kernel the library picks for this shape on this device: "classic" or "pingpong"."""
+        v = C.c_int32()
+        with self._lock:
+            rc = self.lib.wl_gemm_variant(self.ctx, M, N, K, batch, C.byref(v))
+            _lib.check(self.lib, self.ctx, rc, "wl_gemm_variant")
+        return {1: "classic", 2: "pingpong"}[v.value]
 
 
 class DecodeSession:
