@@ -150,6 +150,39 @@ int wl_gemm_variant(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch,
  * with epilogue 0, 1, 2 */
 int wl_test_wgemm(wl_ctx* ctx, const uint16_t* w_f16, const uint16_t* x_f16, const float* bias, float* out, int32_t R,
                   int32_t n_out, int32_t K, int32_t mode);
+/* Test hooks of the decode-step kernels of the default path for more than 16 decoder rows.  Each launches the kernels
+ * exactly as the decode step does, but without programmatic dependent launch, on device copies of the host inputs.
+ *
+ * Split-K decode GEMM (csrc/dec_gemm.cu): out [nsplit][R][n_out] = the raw fp32 partial sum of W[n_out][K] X[R][K]^T
+ * over each K range (ranges of ceil(k-blocks / nsplit) 64-wide k-blocks, the last one shorter).  nsplit = 0 takes the
+ * engine's plan, dec_gemm_split_plan(n_out, R, K, 8).  The split used is written to nsplit_out; a split that cannot be
+ * formed (an empty K range) is an error.  out = NULL only resolves and reports the split. */
+int wl_test_dec_gemm(wl_ctx* ctx, const uint16_t* w_f16, const uint16_t* x_f16, float* out, int32_t R, int32_t n_out,
+                     int32_t K, int32_t nsplit, int32_t* nsplit_out);
+/* K11 cross attention + the combine kernel.  q = q_bias + the q_nsplit (1..4) fp32 partials q_part [q_nsplit][R][H*64],
+ * R = B * rows_per_stream; q_bias may be NULL.  k_pool / v_pool: fp16 [n_slots][H][1500][64] in the pool layout, i.e.
+ * the 16-byte piece p of key s stored at piece p ^ (s & 7) (wl_test_gemm opts 3).  Stream b reads slot[b] and is
+ * skipped when done[b] != 0.  nsplit: key ranges per (stream, head), one of 1, 2, 3, 4, 6, 12, or 0 for the engine's
+ * choice (cross_attn_pick_nsplit); the value used goes to nsplit_out.  out [R][H*64]: the fp16 output as float, the
+ * buffer filled with `sentinel` before the launch.  probs (nsplit 1 only, or NULL): [R][H][1500] attention
+ * probabilities, 0 for the rows of done streams. */
+int wl_test_cross_attn(wl_ctx* ctx, const float* q_part, const float* q_bias, int32_t q_nsplit, const uint16_t* k_pool,
+                       const uint16_t* v_pool, int32_t n_slots, const int32_t* slot, const int32_t* done, int32_t B,
+                       int32_t rows_per_stream, int32_t H, int32_t nsplit, int32_t* nsplit_out, float sentinel, float* out,
+                       float* probs);
+/* K10 self attention.  qkv = qkv_bias + the nsplit (1..8) partials qkv_part [nsplit][R][3*H*64]; nsplit 1 with
+ * qkv_bias NULL is the plain form.  Caches fp16 [n_rows][H][448][64], updated in place (the new k / v of row r at
+ * position pos[r] of cache row wrow[r], or of row r when wrow is NULL).  src [R][448]: cache row holding position p of
+ * row r.  Rows with active[r] == 0 are skipped.  out [R][H*64]: the fp16 output as float, filled with `sentinel`
+ * before the launch. */
+int wl_test_self_attn(wl_ctx* ctx, const float* qkv_part, const float* qkv_bias, int32_t nsplit, uint16_t* k_cache,
+                      uint16_t* v_cache, int32_t n_rows, const int16_t* src, const int32_t* pos, const int32_t* active,
+                      const int32_t* wrow, int32_t R, int32_t H, float sentinel, float* out);
+/* The consumers that fold split-K partials (part [nsplit][rows][cols], bias [cols] or NULL).  mode 0,
+ * layernorm_update_rows: x [rows][cols] += bias + the nsplit (0..8) partials in place, y = LayerNorm(x) * gamma + beta.
+ * mode 1, gelu_cast: y = gelu(bias + the nsplit (1..8) partials); x, gamma, beta unused.  y: the fp16 result as float. */
+int wl_test_fold(wl_ctx* ctx, int32_t mode, float* x, const float* part, int32_t nsplit, const float* bias,
+                 const float* gamma, const float* beta, float* y, int32_t rows, int32_t cols);
 /* device-resident timing of the GEMM kernel: C = A(MxK) * B(NxK)^T, `iters` launches between CUDA events;
  * bn = 0 picks the tile like the engine does. ms_out = average milliseconds per launch. */
 int wl_bench_gemm(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,

@@ -247,7 +247,7 @@ __global__ void __launch_bounds__(256) gelu_cast_kernel(PartialSrc in, __half* _
 #pragma unroll
   for (int s = 0; s < 4; ++s) { v.x += q[s].x; v.y += q[s].y; v.z += q[s].z; v.w += q[s].w; }
 #pragma unroll 1
-  for (int s = 4; s < in.nsplit; ++s) {   // more than 4 ranges never happens for the 4d-wide FC1 (tiles alone fill the SMs)
+  for (int s = 4; s < in.nsplit; ++s) {   // more than 4 ranges: narrow FC1s at few rows (tiny at 17..32 rows gets 6)
     const float4 p = __ldcg(p4 + s * st4);
     v.x += p.x; v.y += p.y; v.z += p.z; v.w += p.w;
   }

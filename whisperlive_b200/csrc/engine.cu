@@ -1979,6 +1979,176 @@ extern "C" int wl_test_wgemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x
   API_END(c)
 }
 
+// Device buffers of one decode-kernel test hook: freed when the hook returns, whether it returns normally or through an
+// exception (a failed check or launch).
+struct HookBufs {
+  std::vector<void*> p;
+  template <class T>
+  T* alloc(size_t n) {
+    void* q = nullptr;
+    WL_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)));
+    p.push_back(q);
+    return (T*)q;
+  }
+  template <class T>
+  T* upload(const T* h, size_t n) {
+    T* d = alloc<T>(n);
+    WL_CUDA(cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice));
+    return d;
+  }
+  ~HookBufs() {
+    for (void* q : p) cudaFree(q);
+  }
+};
+
+static void fill_f16(__half* d, size_t n, float v) {
+  std::vector<__half> h(n, __float2half_rn(v));
+  WL_CUDA(cudaMemcpy(d, h.data(), n * 2, cudaMemcpyHostToDevice));
+}
+static void download_f16(const __half* d, float* out, size_t n) {
+  std::vector<__half> h(n);
+  WL_CUDA(cudaMemcpy(h.data(), d, n * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < n; ++i) out[i] = __half2float(h[i]);
+}
+
+extern "C" int wl_test_dec_gemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x_f16, float* out, int32_t R, int32_t n_out,
+                                int32_t K, int32_t nsplit, int32_t* nsplit_out) {
+  API_BEGIN(c)
+  PdlScope pdl(false);
+  WL_CHECK(w_f16 && x_f16 && nsplit_out && R > 0 && n_out > 0 && K > 0 && K % 8 == 0 && nsplit >= 0, WL_ERR_ARG,
+           "wl_test_dec_gemm: bad arguments");
+  const int ns = nsplit == 0 ? dec_gemm_split_plan(n_out, R, K, 8) : nsplit;
+  const int kb = cdiv(K, 64);
+  WL_CHECK(cdiv(kb, cdiv(kb, ns)) == ns, WL_ERR_ARG, "wl_test_dec_gemm: %d K ranges cannot be formed from %d k-blocks", ns, kb);
+  *nsplit_out = ns;
+  if (!out) return WL_OK;   // split query only
+  HookBufs hb;
+  const long part = (long)R * n_out;
+  const __half* dw = hb.upload(reinterpret_cast<const __half*>(w_f16), (size_t)n_out * K);
+  const __half* dx = hb.upload(reinterpret_cast<const __half*>(x_f16), (size_t)R * K);
+  float* dout = hb.alloc<float>((size_t)ns * part);
+  WL_CUDA(cudaMemset(dout, 0xff, (size_t)ns * part * 4));   // NaN: an element no K range wrote cannot pass as a value
+  WL_CUDA(cudaDeviceSynchronize());
+  dec_gemm(c->st, dw, n_out, K, dx, R, dout, n_out, part, ns);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  WL_CUDA(cudaMemcpy(out, dout, (size_t)ns * part * 4, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+extern "C" int wl_test_cross_attn(wl_ctx* c, const float* q_part, const float* q_bias, int32_t q_nsplit, const uint16_t* k_pool,
+                                  const uint16_t* v_pool, int32_t n_slots, const int32_t* slot, const int32_t* done, int32_t B,
+                                  int32_t rows_per_stream, int32_t H, int32_t nsplit, int32_t* nsplit_out, float sentinel,
+                                  float* out, float* probs) {
+  API_BEGIN(c)
+  PdlScope pdl(false);
+  WL_CHECK(q_part && k_pool && v_pool && slot && done && out && nsplit_out && B > 0 && H > 0 && n_slots > 0 && nsplit >= 0 &&
+               rows_per_stream >= 1 && rows_per_stream <= MAX_ROWS_PER_STREAM,
+           WL_ERR_ARG, "wl_test_cross_attn: bad arguments");
+  for (int b = 0; b < B; ++b) WL_CHECK(slot[b] >= 0 && slot[b] < n_slots, WL_ERR_ARG, "wl_test_cross_attn: slot %d out of range", slot[b]);
+  const int nchunk = cdiv(S_ENC, 128);
+  const int ns = nsplit == 0 ? cross_attn_pick_nsplit(B, H, c->num_sms, rows_per_stream) : nsplit;
+  WL_CHECK(ns >= 1 && ns <= nchunk && cdiv(nchunk, cdiv(nchunk, ns)) == ns, WL_ERR_ARG,
+           "wl_test_cross_attn: %d key ranges cannot be formed from %d chunks", ns, nchunk);
+  WL_CHECK(!probs || ns == 1, WL_ERR_ARG, "wl_test_cross_attn: the probabilities need the whole key range (nsplit 1)");
+  *nsplit_out = ns;
+  const int d = H * 64, R = B * rows_per_stream;
+  const long slot_sz = (long)S_ENC * d;
+  HookBufs hb;
+  DecodeState s;
+  memset(&s, 0, sizeof(s));   // the two kernels read only slot and done
+  s.slot = hb.upload(slot, B);
+  s.done = hb.upload(done, B);
+  PartialSrc q;
+  q.nsplit = q_nsplit;
+  q.stride = (long)R * d;
+  q.ptr = hb.upload(q_part, (size_t)std::max(q_nsplit, 1) * R * d);
+  q.bias = q_bias ? hb.upload(q_bias, d) : nullptr;
+  const __half* kc = hb.upload(reinterpret_cast<const __half*>(k_pool), (size_t)n_slots * slot_sz);
+  const __half* vc = hb.upload(reinterpret_cast<const __half*>(v_pool), (size_t)n_slots * slot_sz);
+  CrossAttnWorkspace ws;
+  ws.part = hb.alloc<float>((size_t)B * H * ns * MAX_ROWS_PER_STREAM * 66);
+  ws.probs = probs ? hb.alloc<float>((size_t)R * H * S_ENC) : nullptr;
+  if (ws.probs) WL_CUDA(cudaMemset(ws.probs, 0, (size_t)R * H * S_ENC * 4));
+  __half* dout = hb.alloc<__half>((size_t)R * d);
+  fill_f16(dout, (size_t)R * d, sentinel);
+  WL_CUDA(cudaDeviceSynchronize());
+  decoder_cross_attn(c->st, s, q, kc, vc, slot_sz, ws, dout, B, rows_per_stream, H, d, ns);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  download_f16(dout, out, (size_t)R * d);
+  if (probs) WL_CUDA(cudaMemcpy(probs, ws.probs, (size_t)R * H * S_ENC * 4, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+extern "C" int wl_test_self_attn(wl_ctx* c, const float* qkv_part, const float* qkv_bias, int32_t nsplit, uint16_t* k_cache,
+                                 uint16_t* v_cache, int32_t n_rows, const int16_t* src, const int32_t* pos, const int32_t* active,
+                                 const int32_t* wrow, int32_t R, int32_t H, float sentinel, float* out) {
+  API_BEGIN(c)
+  PdlScope pdl(false);
+  WL_CHECK(qkv_part && k_cache && v_cache && src && pos && active && out && R > 0 && H > 0 && n_rows > 0 && nsplit >= 1 &&
+               nsplit <= 8,
+           WL_ERR_ARG, "wl_test_self_attn: bad arguments");
+  for (int r = 0; r < R; ++r) {
+    WL_CHECK(pos[r] >= 0 && pos[r] < T_MAX && (wrow ? wrow[r] : r) >= 0 && (wrow ? wrow[r] : r) < n_rows, WL_ERR_ARG,
+             "wl_test_self_attn: row %d: position or write row out of range", r);
+    for (int p = 0; active[r] && p < pos[r]; ++p)
+      WL_CHECK(src[(long)r * T_MAX + p] >= 0 && src[(long)r * T_MAX + p] < n_rows, WL_ERR_ARG, "wl_test_self_attn: src out of range");
+  }
+  const int d = H * 64;
+  const long row_stride = (long)H * T_MAX * 64;
+  HookBufs hb;
+  DecodeState s;
+  memset(&s, 0, sizeof(s));   // the kernel reads only src, pos, active and wrow
+  s.src = hb.upload(src, (size_t)R * T_MAX);
+  s.pos = hb.upload(pos, R);
+  s.active = hb.upload(active, R);
+  s.wrow = wrow ? hb.upload(wrow, R) : nullptr;
+  PartialSrc qkv;
+  qkv.nsplit = nsplit;
+  qkv.stride = (long)R * 3 * d;
+  qkv.ptr = hb.upload(qkv_part, (size_t)nsplit * R * 3 * d);
+  qkv.bias = qkv_bias ? hb.upload(qkv_bias, 3 * d) : nullptr;
+  __half* kc = hb.upload(reinterpret_cast<__half*>(k_cache), (size_t)n_rows * row_stride);
+  __half* vc = hb.upload(reinterpret_cast<__half*>(v_cache), (size_t)n_rows * row_stride);
+  __half* dout = hb.alloc<__half>((size_t)R * d);
+  fill_f16(dout, (size_t)R * d, sentinel);
+  WL_CUDA(cudaDeviceSynchronize());
+  decoder_self_attn(c->st, s, qkv, kc, vc, row_stride, dout, R, H, d);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  download_f16(dout, out, (size_t)R * d);
+  WL_CUDA(cudaMemcpy(k_cache, kc, (size_t)n_rows * row_stride * 2, cudaMemcpyDeviceToHost));
+  WL_CUDA(cudaMemcpy(v_cache, vc, (size_t)n_rows * row_stride * 2, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+extern "C" int wl_test_fold(wl_ctx* c, int32_t mode, float* x, const float* part, int32_t nsplit, const float* bias,
+                            const float* gamma, const float* beta, float* y, int32_t rows, int32_t cols) {
+  API_BEGIN(c)
+  PdlScope pdl(false);
+  WL_CHECK(y && rows > 0 && cols > 0 && (mode == 0 || mode == 1) && nsplit >= 0 && nsplit <= 8 && (nsplit == 0 || part),
+           WL_ERR_ARG, "wl_test_fold: bad arguments");
+  WL_CHECK(mode == 1 || (x && gamma && beta), WL_ERR_ARG, "wl_test_fold: layernorm_update needs x, gamma and beta");
+  WL_CHECK(mode == 0 || nsplit >= 1, WL_ERR_ARG, "wl_test_fold: gelu_cast needs at least one K range");
+  const size_t n = (size_t)rows * cols;
+  HookBufs hb;
+  PartialSrc upd;
+  upd.nsplit = nsplit;
+  upd.stride = (long)n;
+  upd.ptr = nsplit ? hb.upload(part, (size_t)nsplit * n) : nullptr;
+  upd.bias = bias ? hb.upload(bias, cols) : nullptr;
+  __half* dy = hb.alloc<__half>(n);
+  WL_CUDA(cudaMemset(dy, 0, n * 2));
+  float* dx = mode == 0 ? hb.upload(x, n) : nullptr;
+  const float* dg = mode == 0 ? hb.upload(gamma, cols) : nullptr;
+  const float* db = mode == 0 ? hb.upload(beta, cols) : nullptr;
+  WL_CUDA(cudaDeviceSynchronize());
+  if (mode == 0) layernorm_update_rows(c->st, dx, upd, dg, db, dy, rows, cols);
+  else gelu_cast(c->st, upd, dy, rows, cols);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  download_f16(dy, y, n);
+  if (mode == 0) WL_CUDA(cudaMemcpy(x, dx, n * 4, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
 extern "C" int wl_bench_gemm(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,
                              float* ms_out) {
   // flags: 1 transposed (swap-AB) store, 2 bias, 4 GELU, 8 fp32 output with fp32 residual (in place), 16 bias on m,

@@ -484,6 +484,108 @@ class B200Whisper:
             _lib.check(self.lib, self.ctx, rc, "wl_test_wgemm")
         return out
 
+    def test_dec_gemm(self, w: np.ndarray, x: np.ndarray, nsplit: int = 0) -> Tuple[np.ndarray, int]:
+        """Raw K-range partial sums [nsplit, R, n_out] of X[R, K] W[n_out, K]^T through the split-K decode GEMM
+        (wl_test_dec_gemm) and the split used; ``nsplit=0`` takes the engine's plan."""
+        w16 = np.ascontiguousarray(w, dtype=np.float16)
+        x16 = np.ascontiguousarray(x, dtype=np.float16)
+        n_out, K = w16.shape
+        R = x16.shape[0]
+        used = C.c_int32()
+        wp, xp = _lib.ptr(w16.view(np.uint16), C.c_uint16), _lib.ptr(x16.view(np.uint16), C.c_uint16)
+        with self._lock:
+            rc = self.lib.wl_test_dec_gemm(self.ctx, wp, xp, None, R, n_out, K, int(nsplit), C.byref(used))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_dec_gemm")
+            out = np.empty((used.value, R, n_out), dtype=np.float32)
+            rc = self.lib.wl_test_dec_gemm(self.ctx, wp, xp, _lib.ptr(out, C.c_float), R, n_out, K, used.value, C.byref(used))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_dec_gemm")
+        return out, used.value
+
+    def test_cross_attn(self, q_part: np.ndarray, q_bias: Optional[np.ndarray], k_pool: np.ndarray, v_pool: np.ndarray,
+                        slot: Sequence[int], done: Sequence[int], rows_per_stream: int, nsplit: int = 0,
+                        sentinel: float = 0.0, probs: bool = False) -> Tuple[np.ndarray, Optional[np.ndarray], int]:
+        """K11 cross attention (wl_test_cross_attn).  q_part [q_nsplit, R, H*64] fp32; k_pool / v_pool fp16
+        [n_slots, H, 1500, 64] already in the swizzled pool layout.  Returns (out [R, H*64], probs [R, H, 1500] or None,
+        key split used)."""
+        qp = np.ascontiguousarray(q_part, dtype=np.float32)
+        kp = np.ascontiguousarray(k_pool, dtype=np.float16)
+        vp = np.ascontiguousarray(v_pool, dtype=np.float16)
+        n_slots, H = kp.shape[:2]
+        sl = np.ascontiguousarray(slot, dtype=np.int32)
+        dn = np.ascontiguousarray(done, dtype=np.int32)
+        B = len(sl)
+        R = B * rows_per_stream
+        out = np.empty((R, H * 64), dtype=np.float32)
+        pr = np.empty((R, H, 1500), dtype=np.float32) if probs else None
+        bp = None
+        if q_bias is not None:
+            q_bias = np.ascontiguousarray(q_bias, dtype=np.float32)
+            bp = _lib.ptr(q_bias, C.c_float)
+        used = C.c_int32()
+        with self._lock:
+            rc = self.lib.wl_test_cross_attn(self.ctx, _lib.ptr(qp, C.c_float), bp, qp.shape[0],
+                                             _lib.ptr(kp.view(np.uint16), C.c_uint16), _lib.ptr(vp.view(np.uint16), C.c_uint16),
+                                             n_slots, _lib.ptr(sl, C.c_int32), _lib.ptr(dn, C.c_int32), B, rows_per_stream, H,
+                                             int(nsplit), C.byref(used), float(sentinel), _lib.ptr(out, C.c_float),
+                                             None if pr is None else _lib.ptr(pr, C.c_float))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_cross_attn")
+        return out, pr, used.value
+
+    def test_self_attn(self, qkv_part: np.ndarray, qkv_bias: Optional[np.ndarray], k_cache: np.ndarray, v_cache: np.ndarray,
+                       src: np.ndarray, pos: Sequence[int], active: Sequence[int], wrow: Optional[Sequence[int]] = None,
+                       sentinel: float = 0.0) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """K10 self attention (wl_test_self_attn).  qkv_part [nsplit, R, 3*H*64] fp32 (nsplit 1 without a bias: the plain
+        form); caches fp16 [n_rows, H, 448, 64]; src [R, 448].  Returns (out [R, H*64], k cache, v cache) after the call."""
+        qp = np.ascontiguousarray(qkv_part, dtype=np.float32)
+        kc = np.ascontiguousarray(k_cache, dtype=np.float16).copy()
+        vc = np.ascontiguousarray(v_cache, dtype=np.float16).copy()
+        n_rows, H = kc.shape[:2]
+        R = qp.shape[1]
+        sr = np.ascontiguousarray(src, dtype=np.int16)
+        ps = np.ascontiguousarray(pos, dtype=np.int32)
+        ac = np.ascontiguousarray(active, dtype=np.int32)
+        wr = None if wrow is None else np.ascontiguousarray(wrow, dtype=np.int32)
+        out = np.empty((R, H * 64), dtype=np.float32)
+        bp = None
+        if qkv_bias is not None:
+            qkv_bias = np.ascontiguousarray(qkv_bias, dtype=np.float32)
+            bp = _lib.ptr(qkv_bias, C.c_float)
+        with self._lock:
+            rc = self.lib.wl_test_self_attn(self.ctx, _lib.ptr(qp, C.c_float), bp, qp.shape[0],
+                                            _lib.ptr(kc.view(np.uint16), C.c_uint16), _lib.ptr(vc.view(np.uint16), C.c_uint16),
+                                            n_rows, _lib.ptr(sr, C.c_int16), _lib.ptr(ps, C.c_int32), _lib.ptr(ac, C.c_int32),
+                                            None if wr is None else _lib.ptr(wr, C.c_int32), R, H, float(sentinel),
+                                            _lib.ptr(out, C.c_float))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_self_attn")
+        return out, kc, vc
+
+    def test_layernorm_update(self, x: np.ndarray, part: Optional[np.ndarray], bias: Optional[np.ndarray], gamma: np.ndarray,
+                              beta: np.ndarray) -> Tuple[np.ndarray, np.ndarray]:
+        """x += bias + the partials [nsplit, rows, d] (none when ``part`` is None), y = LayerNorm(x) as fp16
+        (wl_test_fold mode 0).  Returns (updated x, y)."""
+        x = np.ascontiguousarray(x, dtype=np.float32).copy()
+        rows, d = x.shape
+        y = np.empty_like(x)
+        self._fold(0, x, part, bias, np.ascontiguousarray(gamma, dtype=np.float32), np.ascontiguousarray(beta, dtype=np.float32),
+                   y, rows, d)
+        return x, y
+
+    def test_gelu_cast(self, part: np.ndarray, bias: Optional[np.ndarray]) -> np.ndarray:
+        """fp16(gelu(bias + the partials [nsplit, rows, cols])) (wl_test_fold mode 1)."""
+        _, rows, cols = part.shape
+        y = np.empty((rows, cols), dtype=np.float32)
+        self._fold(1, None, part, bias, None, None, y, rows, cols)
+        return y
+
+    def _fold(self, mode, x, part, bias, gamma, beta, y, rows, cols):
+        fp = lambda a: None if a is None else _lib.ptr(a, C.c_float)
+        part = None if part is None else np.ascontiguousarray(part, dtype=np.float32)
+        bias = None if bias is None else np.ascontiguousarray(bias, dtype=np.float32)
+        with self._lock:
+            rc = self.lib.wl_test_fold(self.ctx, mode, fp(x), fp(part), 0 if part is None else part.shape[0], fp(bias), fp(gamma),
+                                       fp(beta), fp(y), rows, cols)
+            _lib.check(self.lib, self.ctx, rc, "wl_test_fold")
+
     GEMM_OUT = {"f32": 0, "resid": 1, "f16": 2, "headsplit": 3}
     GEMM_VARIANT = {"auto": 0, "classic": 1, "pingpong": 2}
 
