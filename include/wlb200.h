@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 3
+#define WL_ABI_VERSION 4
 
 typedef struct wl_ctx wl_ctx;
 
@@ -99,14 +99,25 @@ int wl_generate(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* pro
 
 /* N2. Decode session: step-level continuous batching -- replaces the run-to-completion batches of the reference's
  * BatchInferenceWorker._process_multi (whisper_live/batch_inference.py:155-187; its gaps :259, :334-339).
- *   wl_session_open    fixes the search options (wl_generate's, sampling excluded) and the number of stream indices
- *                      (<= max_streams); every index starts idle.  Re-opening is allowed once nothing is decoding.
+ *   wl_session_open    fixes the search options (wl_generate's beam or greedy search; sampling is chosen per stream at
+ *                      admission) and the number of stream indices (<= max_streams); every index starts idle.
+ *                      Re-opening is allowed once nothing is decoding.
  *   wl_session_admit   puts n streams into idle indices: prompts prefilled in one batched pass (K8), search state
  *                      initialised; the streams already decoding are untouched.  max_length[n] like wl_generate's.
+ *   wl_session_admit_ex the same with a search per stream (search[n], or NULL = wl_session_admit): sample = 1 decodes
+ *                      the stream by Gumbel-max sampling over the full distribution, num_hypotheses independent rows
+ *                      (1 .. the session's rows per stream: beam_size, or num_hypotheses when beam_size = 1), with the
+ *                      draws of wl_generate(seed) for the stream at batch position noise_key.  The result does not
+ *                      depend on which other streams share the loop, and admitting it captures no new graph.  A bad
+ *                      spec (num_hypotheses out of range, temperature <= 0 or not finite, negative key) fails the
+ *                      whole call before anything is staged: every index stays free.  sample = 0 is the session's own
+ *                      search (the other fields are ignored).
  *   wl_session_run     runs the device-side token loop over every admitted stream for at most max_steps steps; with
  *                      break_on_finish it also returns as soon as some stream has finished.  done_out[capacity]: 1 for
  *                      indices whose stream is finished and not yet collected.  steps_ran: token steps executed.
  *   wl_session_collect hypotheses of one finished index (outputs like one stream of wl_generate); the index goes idle.
+ *                      out_ids / out_len / out_score hold the index's own hypothesis count: the sampled stream's
+ *                      num_hypotheses, else the session's.
  *   wl_session_close   drops whatever is still in flight.
  * The session has its own decode state and self-attention cache: wl_generate / wl_align / wl_detect_language /
  * wl_encode may be called between two wl_session_run calls (temperature-fallback retries, word alignment of a finished
@@ -114,6 +125,15 @@ int wl_generate(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* pro
 int wl_session_open(wl_ctx* ctx, const wl_gen_opts* opts, int32_t capacity);
 int wl_session_admit(wl_ctx* ctx, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
                      const int32_t* prompt_off, const int32_t* max_length);
+typedef struct wl_stream_search {
+  int32_t sample;            /* 0: the session's search options; 1: Gumbel-max sampling over the full distribution */
+  int32_t num_hypotheses;    /* sampling: 1 .. the session's rows per stream */
+  float temperature;         /* sampling: > 0, finite */
+  uint32_t seed;             /* sampling noise = that of wl_generate(seed) ... */
+  int32_t noise_key;         /* ... for the stream at batch position noise_key (>= 0) */
+} wl_stream_search;
+int wl_session_admit_ex(wl_ctx* ctx, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
+                        const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search);
 int wl_session_run(wl_ctx* ctx, int32_t max_steps, int32_t break_on_finish, int32_t* done_out, int32_t* steps_ran);
 int wl_session_collect(wl_ctx* ctx, int32_t index, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
                        int32_t* out_steps);

@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -40,6 +40,13 @@ class WlGenOpts(C.Structure):
     ]
 
 
+class WlStreamSearch(C.Structure):
+    _fields_ = [
+        ("sample", C.c_int32), ("num_hypotheses", C.c_int32), ("temperature", C.c_float), ("seed", C.c_uint32),
+        ("noise_key", C.c_int32),
+    ]
+
+
 # name -> (restype, argtypes); every symbol include/wlb200.h declares
 SIGNATURES = {
     "wl_init": (C.c_int, [C.POINTER(WlConfig), C.POINTER(C.c_void_p)]),
@@ -56,6 +63,8 @@ SIGNATURES = {
                               c_f32p, c_i32p]),
     "wl_session_open": (C.c_int, [C.c_void_p, C.POINTER(WlGenOpts), C.c_int32]),
     "wl_session_admit": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p]),
+    "wl_session_admit_ex": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
+                                      C.POINTER(WlStreamSearch)]),
     "wl_session_run": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, c_i32p, c_i32p]),
     "wl_session_collect": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_f32p, c_f32p, c_i32p]),
     "wl_session_close": (C.c_int, [C.c_void_p]),

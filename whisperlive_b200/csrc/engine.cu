@@ -44,6 +44,11 @@ struct GraphEntry {
   long kernels = 0;  // kernel nodes per replay
 };
 
+// Rows of the per-stream metadata table of a decode call (stream_meta / search_meta -> upload_state_tables):
+// slot, len, sot_index, use_ts, n_new, force_len, pre_n, pre_last, pre_penult, pre_lts, then the stream's search:
+// smode, temperature (float bits), noise seed, noise key, rows
+constexpr int META_ROWS = 15;
+
 struct wl_ctx {
   wl_config cfg;
   std::vector<int32_t> align_heads;
@@ -146,8 +151,9 @@ struct wl_ctx {
     __half *kcache = nullptr, *vcache = nullptr;
     unsigned* mask = nullptr;
     int* idx_dev = nullptr;
-    std::vector<int> hp, meta;          // host shadows: prompts [cap][T_MAX], per-stream metadata [10][cap]
+    std::vector<int> hp, meta;          // host shadows: prompts [cap][T_MAX], per-stream metadata [META_ROWS][cap]
     std::vector<char> used, finished;   // index holds an admitted stream / that stream has finished decoding
+    std::vector<int> nh;                // hypotheses the index's stream returns: N when it samples, else NH
     int live = 0;                       // admitted and still decoding
     long steps = 0, runs = 0, admitted = 0;
   } sess;
@@ -210,7 +216,9 @@ static void alloc_decode_state(wl_ctx* c, DecodeState& s) {
   s.hyp_count = dalloc<int>(c, B); s.hyp_cum = dalloc<float>(c, B * MAX_HYPS); s.hyp_len = dalloc<int>(c, B * MAX_HYPS);
   s.hyp_tok = dalloc<int>(c, B * MAX_HYPS * T_MAX); s.steps_run = dalloc<int>(c, B); s.n_done = dalloc<int>(c, 1);
   s.force_len = dalloc<int>(c, B); s.force_prob = dalloc<float>(c, B * T_MAX);
-  s.seed = dalloc<unsigned>(c, 1); s.steps_left = dalloc<int>(c, 1);
+  s.steps_left = dalloc<int>(c, 1);
+  s.smode = dalloc<int>(c, B); s.temp = dalloc<float>(c, B); s.nseed = dalloc<unsigned>(c, B); s.nkey = dalloc<int>(c, B);
+  s.nrows = dalloc<int>(c, B);
   s.pre_n = dalloc<int>(c, B); s.pre_last = dalloc<int>(c, B); s.pre_penult = dalloc<int>(c, B); s.pre_lts = dalloc<int>(c, B);
   s.brk = dalloc<int>(c, 2);
 }
@@ -1205,7 +1213,8 @@ static VocabIds vocab_ids(wl_ctx* c) {
   return v;
 }
 
-// Per-stream metadata of a decode call (column b of the [10][B] table `meta`; tokens into hp_row[T_MAX]).  Returns the
+// Per-stream metadata of a decode call (rows 0-9 of column b of the [META_ROWS][B] table `meta`; tokens into
+// hp_row[T_MAX]; search_meta writes the other rows).  Returns the
 // decode steps the stream may need without prefill; *n_new_out = the new tokens it may emit.
 static int stream_meta(wl_ctx* c, int b, int slot, const int32_t* prompt, int P, int ml, bool forced, int* hp_row, int* meta, int col,
                        int ncol, int* n_new_out) {
@@ -1250,26 +1259,42 @@ static int stream_meta(wl_ctx* c, int b, int slot, const int32_t* prompt, int P,
   return steps;
 }
 
-// prompts [B][T_MAX] + the [10][B] metadata table (pinned host) -> the device state
+// The search of the stream in column `col` (rows 10-14 of the metadata table): sample = 0 takes the call's / session's
+// SearchOpts over `rows` rows; sample = 1 is Gumbel-max sampling at `temperature` over `rows` independent rows, its noise
+// that of wl_generate(seed) for the stream at batch position `key`.
+static void search_meta(int* meta, int col, int ncol, int sample, float temperature, uint32_t seed, int key, int rows) {
+  int tbits;
+  memcpy(&tbits, &temperature, 4);
+  meta[10 * ncol + col] = sample;
+  meta[11 * ncol + col] = tbits;
+  meta[12 * ncol + col] = (int)seed;
+  meta[13 * ncol + col] = key;
+  meta[14 * ncol + col] = rows;
+}
+
+// prompts [B][T_MAX] + the [META_ROWS][B] metadata table (pinned host) -> the device state
 static void upload_state_tables(wl_ctx* c, const int* hp, const int* meta, int B) {
   const DecodeState& s = c->ds;
   cudaStream_t st = c->st;
   WL_CUDA(cudaMemcpyAsync(s.prompt, hp, (size_t)B * T_MAX * 4, cudaMemcpyHostToDevice, st));
-  int* dst[10] = {s.slot, s.prompt_len, s.sot_index, s.use_ts, s.n_new, s.force_len, s.pre_n, s.pre_last, s.pre_penult, s.pre_lts};
-  for (int k = 0; k < 10; ++k) WL_CUDA(cudaMemcpyAsync(dst[k], meta + (size_t)k * B, B * 4, cudaMemcpyHostToDevice, st));
+  void* dst[META_ROWS] = {s.slot, s.prompt_len, s.sot_index, s.use_ts, s.n_new, s.force_len, s.pre_n, s.pre_last, s.pre_penult,
+                          s.pre_lts, s.smode, s.temp, s.nseed, s.nkey, s.nrows};
+  for (int k = 0; k < META_ROWS; ++k) WL_CUDA(cudaMemcpyAsync(dst[k], meta + (size_t)k * B, B * 4, cudaMemcpyHostToDevice, st));
 }
 
-// upload prompts & per-stream metadata; returns max steps
+// upload prompts & per-stream metadata, every stream with the same search (key = batch position); returns max steps
 static int upload_streams(wl_ctx* c, const int32_t* slots, int B, const int32_t* prompts, const int32_t* off, int max_length,
-                          bool forced, const int32_t* max_len_ps = nullptr, int* max_new_out = nullptr) {
+                          bool forced, int sample, float temperature, uint32_t seed, int rows, const int32_t* max_len_ps = nullptr,
+                          int* max_new_out = nullptr) {
   ensure_host(c, (size_t)B * (T_MAX + 16), 16);
   int* hp = c->h_int;                      // [B][T_MAX]
-  int* meta = c->h_int + (size_t)B * T_MAX;  // slot, len, sot_index, use_ts, n_new, force_len, pre_n, pre_last, pre_penult, pre_lts
+  int* meta = c->h_int + (size_t)B * T_MAX;  // [META_ROWS][B]
   int max_steps = 0, max_new = 0;
   for (int b = 0; b < B; ++b) {
     int n_new = 0;
     const int steps = stream_meta(c, b, slots[b], prompts + off[b], off[b + 1] - off[b], max_len_ps ? max_len_ps[b] : max_length,
                                   forced, hp + (size_t)b * T_MAX, meta, b, B, &n_new);
+    search_meta(meta, b, B, sample, temperature, seed, b, rows);
     max_steps = std::max(max_steps, steps);
     max_new = std::max(max_new, n_new);
   }
@@ -1310,8 +1335,8 @@ static cudaGraphExec_t decode_graph(wl_ctx* c, const char* tag, int B, int Kr, i
                                     int nsplit, bool loop_graph, long* kernels) {
   cudaStream_t st = c->st;
   char key[160];
-  snprintf(key, sizeof(key), "%s/%d/%d/%d/%d/%d/%d/%d/%08x/%d/%d", tag, B, Kr, K, so.max_cand, so.suppress_blank, so.max_initial_ts,
-           so.sampling, *(const unsigned*)&so.temperature, loop_graph ? 1 : 0, xa_prefetch_streams() * 2 + (cgemm_enabled() ? 1 : 0));
+  snprintf(key, sizeof(key), "%s/%d/%d/%d/%d/%d/%d/%d/%d", tag, B, Kr, K, so.max_cand, so.suppress_blank, so.max_initial_ts,
+           loop_graph ? 1 : 0, xa_prefetch_streams() * 2 + (cgemm_enabled() ? 1 : 0));
   GraphEntry& ge = c->graphs[key];
   if (!ge.exec) {
     const long before = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + cgemm_launch_count() + other_launch_count();
@@ -1375,8 +1400,8 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
   so.beam = K; so.rows_per_stream = Kr;
   so.max_cand = std::max(1, std::min(MAX_HYPS, (int)lroundf(K * o->patience)));
   so.suppress_blank = o->suppress_blank; so.max_initial_ts = o->max_initial_timestamp_index;
-  so.sampling = (K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f) ? 1 : 0;
-  so.temperature = o->sampling_temperature; so.seed = o->seed; so.suppress_mask = c->suppress_mask;
+  so.suppress_mask = c->suppress_mask;
+  const int sample = (K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f) ? 1 : 0;
   const VocabIds vi = vocab_ids(c);
   cudaStream_t st = c->st;
   // suppress bitmask
@@ -1387,15 +1412,14 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
     if (t >= 0 && t < c->V) mask[t >> 5] |= 1u << (t & 31);
   }
   int max_new = 0;
-  int max_steps = upload_streams(c, slots, B, prompts, prompt_off, o->max_length, false, o->max_length_per_stream, &max_new);
+  int max_steps = upload_streams(c, slots, B, prompts, prompt_off, o->max_length, false, sample, o->sampling_temperature, o->seed, Kr,
+                                 o->max_length_per_stream, &max_new);
   // K8: every prompt position but the last goes through the decoder in ONE batched pass (WLB200_PREFILL=0: one decode
   // step per prompt token, the round-1 behaviour)
   static const bool prefill_env = [] { const char* e = getenv("WLB200_PREFILL"); return e ? atoi(e) != 0 : true; }();
   const bool prefilled = o->prefill == 1 || (o->prefill == 0 && prefill_env);
   if (prefilled) max_steps = max_new;
   WL_CUDA(cudaMemcpyAsync(c->suppress_mask, mask.data(), nwords * 4, cudaMemcpyHostToDevice, st));
-  const unsigned seed_host = o->seed;
-  WL_CUDA(cudaMemcpyAsync(c->ds.seed, &seed_host, sizeof(unsigned), cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaEventRecord(c->ev0, st));
   if (prefilled) {
     // upload_streams staged the prompts in pinned host memory: h_int = [B][T_MAX] tokens, then the per-stream metadata
@@ -1511,9 +1535,10 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   const int K = o->beam_size, Kr = K > 1 ? K : o->num_hypotheses;
   WL_CHECK(Kr <= c->Km, WL_ERR_ARG, "wl_session_open: %d rows per stream exceed max_beam=%d", Kr, c->Km);
   WL_CHECK(K == 1 || o->num_hypotheses <= MAX_HYPS, WL_ERR_ARG, "too many hypotheses");
-  // sampling draws are keyed by (call seed, batch position): a session has neither, so the temperature-fallback rungs stay
-  // on wl_generate (the transcriber routes them there)
-  WL_CHECK(!(K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f), WL_ERR_ARG, "wl_session_open: sampling is not supported in a decode session");
+  // the session's own search is beam or greedy: sampling is chosen per stream at admission (wl_session_admit_ex), where
+  // each sampled stream brings the seed and noise key its draws are keyed by
+  WL_CHECK(!(K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f), WL_ERR_ARG,
+           "wl_session_open: sampling is chosen per stream at admission (wl_session_admit_ex), not for the session");
   if (!ss.allocated) {
     alloc_decode_state(c, ss.ds);
     ss.kcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
@@ -1528,7 +1553,7 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   so.beam = K; so.rows_per_stream = Kr;
   so.max_cand = std::max(1, std::min(MAX_HYPS, (int)lroundf(K * o->patience)));
   so.suppress_blank = o->suppress_blank; so.max_initial_ts = o->max_initial_timestamp_index;
-  so.sampling = 0; so.temperature = o->sampling_temperature; so.seed = o->seed; so.suppress_mask = ss.mask;
+  so.suppress_mask = ss.mask;
   ss.nsplit = cross_attn_pick_nsplit(capacity, c->H, c->num_sms, Kr);
   const int nwords = (c->V + 31) / 32 + 1;
   std::vector<unsigned> mask(nwords, 0u);
@@ -1538,23 +1563,25 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   }
   const int cap = capacity, R = cap * Kr;
   ss.hp.assign((size_t)cap * T_MAX, 0);
-  ss.meta.assign((size_t)10 * cap, 0);
-  for (int b = 0; b < cap; ++b) { ss.meta[1 * cap + b] = 1; ss.meta[2 * cap + b] = -1; ss.meta[4 * cap + b] = 1; }   // harmless idle values
+  ss.meta.assign((size_t)META_ROWS * cap, 0);
+  for (int b = 0; b < cap; ++b) {   // harmless idle values
+    ss.meta[1 * cap + b] = 1; ss.meta[2 * cap + b] = -1; ss.meta[4 * cap + b] = 1;
+    search_meta(ss.meta.data(), b, cap, 0, 0.f, 0u, b, Kr);
+  }
   ss.used.assign(cap, 0);
   ss.finished.assign(cap, 0);
+  ss.nh.assign(cap, ss.NH);
   ss.live = 0;
   cudaStream_t st = c->st;
   const DecodeState& s = ss.ds;
   std::vector<int> ones(cap, 1);
   const int nd = cap, brk0[2] = {0, 0};
-  const unsigned seed_host = o->seed;
   WL_CUDA(cudaMemcpyAsync(ss.mask, mask.data(), nwords * 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaMemcpyAsync(s.done, ones.data(), cap * 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaMemsetAsync(s.active, 0, (size_t)R * 4, st));
   WL_CUDA(cudaMemsetAsync(s.hyp_count, 0, (size_t)cap * 4, st));
   WL_CUDA(cudaMemcpyAsync(s.n_done, &nd, 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaMemcpyAsync(s.brk, brk0, 8, cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaMemcpyAsync(s.seed, &seed_host, 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaStreamSynchronize(st));   // the host vectors above go out of scope
   ss.open = true;
   API_END(c)
@@ -1562,6 +1589,11 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
 
 extern "C" int wl_session_admit(wl_ctx* c, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
                                 const int32_t* prompt_off, const int32_t* max_length) {
+  return wl_session_admit_ex(c, n, index, slots, prompts, prompt_off, max_length, nullptr);
+}
+
+extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
+                                   const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search) {
   API_BEGIN(c)
   wl_ctx::Session& ss = c->sess;
   WL_CHECK(ss.open, WL_ERR_STATE, "wl_session_admit: no open session");
@@ -1571,18 +1603,32 @@ extern "C" int wl_session_admit(wl_ctx* c, int32_t n, const int32_t* index, cons
     WL_CHECK(index[i] >= 0 && index[i] < cap, WL_ERR_ARG, "wl_session_admit: index %d outside the session capacity %d", index[i], cap);
     WL_CHECK(!ss.used[index[i]], WL_ERR_STATE, "wl_session_admit: index %d still holds a stream", index[i]);
     for (int j = 0; j < i; ++j) WL_CHECK(index[j] != index[i], WL_ERR_ARG, "wl_session_admit: index %d listed twice", index[i]);
+    if (search && search[i].sample) {
+      const wl_stream_search& q = search[i];
+      WL_CHECK(q.sample == 1, WL_ERR_ARG, "wl_session_admit: stream %d: sample must be 0 or 1, got %d", i, q.sample);
+      WL_CHECK(q.num_hypotheses >= 1 && q.num_hypotheses <= ss.Kr, WL_ERR_ARG,
+               "wl_session_admit: stream %d: %d sampled hypotheses outside 1 .. %d rows per stream", i, q.num_hypotheses, ss.Kr);
+      WL_CHECK(std::isfinite(q.temperature) && q.temperature > 0.f, WL_ERR_ARG,
+               "wl_session_admit: stream %d: sampling temperature %g must be finite and > 0", i, (double)q.temperature);
+      WL_CHECK(q.noise_key >= 0, WL_ERR_ARG, "wl_session_admit: stream %d: negative noise key %d", i, q.noise_key);
+    }
   }
   // validate + stage everything before touching the session (a bad prompt must not leave a half-admitted stream)
   std::vector<int> hp = ss.hp, meta = ss.meta;
-  for (int i = 0; i < n; ++i)
+  for (int i = 0; i < n; ++i) {
     stream_meta(c, i, slots[i], prompts + prompt_off[i], prompt_off[i + 1] - prompt_off[i], max_length[i], false,
                 hp.data() + (size_t)index[i] * T_MAX, meta.data(), index[i], cap, nullptr);
+    const bool sample = search && search[i].sample;
+    search_meta(meta.data(), index[i], cap, sample ? 1 : 0, sample ? search[i].temperature : 0.f, sample ? search[i].seed : 0u,
+                sample ? search[i].noise_key : index[i], sample ? search[i].num_hypotheses : ss.Kr);
+  }
   ss.hp.swap(hp);
   ss.meta.swap(meta);
+  for (int i = 0; i < n; ++i) ss.nh[index[i]] = (search && search[i].sample) ? search[i].num_hypotheses : ss.NH;
   ensure_host(c, (size_t)cap * (T_MAX + 16) + n, 16);
   int* php = c->h_int;
   int* pmeta = php + (size_t)cap * T_MAX;
-  int* pidx = pmeta + (size_t)10 * cap;
+  int* pidx = pmeta + (size_t)META_ROWS * cap;
   memcpy(php, ss.hp.data(), ss.hp.size() * 4);
   memcpy(pmeta, ss.meta.data(), ss.meta.size() * 4);
   memcpy(pidx, index, (size_t)n * 4);
@@ -1678,7 +1724,7 @@ extern "C" int wl_session_collect(wl_ctx* c, int32_t index, int32_t* out_ids, in
   WL_CUDA(cudaMemcpyAsync(h_cum, s.hyp_cum + (size_t)index * MAX_HYPS, MAX_HYPS * 4, cudaMemcpyDeviceToHost, st));
   WL_CUDA(cudaMemcpyAsync(h_ns, s.no_speech + index, 4, cudaMemcpyDeviceToHost, st));
   WL_CUDA(cudaStreamSynchronize(st));
-  emit_hyps(ss.NH, ss.length_penalty, h_cnt[0], h_len, h_cum, h_tok, out_ids, out_len, out_score);
+  emit_hyps(ss.nh[index], ss.length_penalty, h_cnt[0], h_len, h_cum, h_tok, out_ids, out_len, out_score);
   if (out_no_speech) *out_no_speech = h_ns[0];
   if (out_steps) *out_steps = h_steps[0];
   ss.used[index] = 0;
@@ -1712,7 +1758,7 @@ static void forced_run(wl_ctx* c, const int32_t* slots, int B, const int32_t* to
   so.beam = 1; so.rows_per_stream = 1; so.max_cand = 1; so.suppress_mask = c->suppress_mask;
   const VocabIds vi = vocab_ids(c);
   cudaStream_t st = c->st;
-  const int max_steps = upload_streams(c, slots, B, tokens, off, T_MAX, true);
+  const int max_steps = upload_streams(c, slots, B, tokens, off, T_MAX, true, 0, 0.f, 0u, 1);
   decode_init(st, c->ds, so, vi, B, B);
   const int nsplit = align_mode ? 1 : cross_attn_pick_nsplit(B, c->H, c->num_sms, 1);
   for (int i = 0; i < max_steps; ++i) {

@@ -102,23 +102,27 @@ struct DecodeState {
   int* steps_run;    // [B] decoder steps executed for the stream (diagnostics)
   int* n_done;       // [1] number of finished streams
   int* steps_left;   // [1] decode steps the device-side loop may still run (conditional WHILE graph)
-  unsigned* seed;    // [1] sampling seed of this generate call (device scalar: the captured graph does not depend on it)
-  int* brk;          // [2] decode sessions (step-level admission): [0] != 0 -> the device-side loop also ends as soon as a
+  // per-stream search (device tables: the captured graph does not depend on which streams sample)
+  int* smode;        // [B] 0: the call's / session's search (SearchOpts); 1: Gumbel-max sampling, independent rows
+  float* temp;       // [B] sampling temperature
+  unsigned* nseed;   // [B] sampling noise seed
+  int* nkey;         // [B] noise key: the stream index that goes into the noise hash
+  int* nrows;        // [B] rows the stream uses (<= rows_per_stream); rows nrows .. rows_per_stream-1 stay inactive
+  int* brk;         // [2] decode sessions (step-level admission): [0] != 0 -> the device-side loop also ends as soon as a
                      //   stream finishes (so the host can hand its result out and refill the index); [1] = n_done at launch
   // teacher-forced mode (detect_language / align / logits test hook)
   int* force_len;    // [B] 0 = normal search; >0 = feed prompt only, then stop
   float* force_prob; // [B][T_MAX] P(prompt[i+1] | prompt[..i]) in teacher-forced mode
 };
 
+// Options shared by every stream of a call / session.  Whether a stream samples, at what temperature and with which
+// noise is per stream: DecodeState::smode / temp / nseed / nkey / nrows.
 struct SearchOpts {
-  int beam;            // K (1 = greedy / sampling)
+  int beam;            // K (1 = greedy, or sampling when the stream's smode says so)
   int rows_per_stream; // Kr
   int max_cand;        // round(K * patience)
   int suppress_blank;
   int max_initial_ts;
-  int sampling;        // 1: Gumbel-max sampling over the full distribution
-  float temperature;
-  unsigned seed;
   const unsigned* suppress_mask;  // device bitmask over the vocabulary
 };
 

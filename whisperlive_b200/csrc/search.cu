@@ -193,10 +193,14 @@ __global__ void __launch_bounds__(SR_THREADS) search_rows_kernel(DecodeState s, 
     lse = hi + log1pf(expf(lo - hi));
   }
 
-  // selection keys in place: log-prob (beam / greedy) or log-prob / T + Gumbel noise (sampling); rule e drops text
-  const int NC = o.beam > 1 ? 2 * o.beam : 1;
+  // selection keys in place: log-prob (beam / greedy) or log-prob / T + Gumbel noise (sampling); rule e drops text.
+  // The noise of row j of a sampling stream is keyed by (seed, noise key, j, step) -- wl_generate: key = batch position.
+  const bool sampling = s.smode[b] != 0;
+  const int NC = (!sampling && o.beam > 1) ? 2 * o.beam : 1;
+  const float temperature = s.temp[b];
   uint32_t gkey = 0;
-  if (o.sampling) gkey = hash_u32((*s.seed * 0x9E3779B1u) ^ hash_u32((uint32_t)((b * 64 + (r - b * o.rows_per_stream)) * 65537 + s.step[b])));
+  if (sampling)
+    gkey = hash_u32((s.nseed[b] * 0x9E3779B1u) ^ hash_u32((uint32_t)((s.nkey[b] * 64 + (r - b * o.rows_per_stream)) * 65537 + s.step[b])));
   float bk = -INFINITY;        // this thread's best remaining entry
   int bt = 0x7fffffff;
   for (int i4 = tid; i4 < n4; i4 += SR_THREADS) {
@@ -209,9 +213,9 @@ __global__ void __launch_bounds__(SR_THREADS) search_rows_kernel(DecodeState s, 
       if (x[e] > -INFINITY && !(text_off && t + e < v.ts_begin)) {
         const float lp = x[e] - lse;
         key = lp;
-        if (o.sampling) {
+        if (sampling) {
           const double u = ((double)hash_u32((uint32_t)(t + e) ^ gkey) + 0.5) / 4294967296.0;
-          key = __fdiv_rn(lp, o.temperature) + (float)(-log(-log(u)));
+          key = __fdiv_rn(lp, temperature) + (float)(-log(-log(u)));
         }
         if (key > bk) { bk = key; bt = t + e; }   // ascending token order: strict > keeps the lowest id among equals
       }
@@ -292,6 +296,10 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
   if (s.done[b]) return;
   const int Kr = o.rows_per_stream, row0 = b * Kr;
   const int P = s.prompt_len[b], fed = s.fed[b];
+  // greedy / sampling: every row is an independent hypothesis, over the stream's own N <= Kr rows (a sampling stream
+  // of a beam session included)
+  const bool independent = o.beam == 1 || s.smode[b] != 0;
+  const int N = s.nrows[b];
   __shared__ int sh_hist[MAX_ROWS_PER_STREAM][T_MAX];
   __shared__ short sh_src[MAX_ROWS_PER_STREAM][T_MAX];
   __shared__ int new_parent[MAX_ROWS_PER_STREAM], new_tok[MAX_ROWS_PER_STREAM];
@@ -324,9 +332,9 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
       s.pos[row0] = nf;
       s.fed[b] = nf;
     }
-    if (nf == P - 1 && o.beam == 1 && Kr > 1) {
+    if (nf == P - 1 && independent && N > 1) {
       // independent sampling rows all start from the prompt cache of row 0
-      for (int j = 1; j < Kr; ++j) {
+      for (int j = 1; j < N; ++j) {
         for (int p = tid; p < nf; p += 128) s.src[(long)(row0 + j) * T_MAX + p] = s.src[(long)row0 * T_MAX + p];
         if (tid == 0) {
           s.tok_in[row0 + j] = s.prompt[(long)b * T_MAX + nf];
@@ -341,8 +349,8 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
   const bool last_step = step + 1 >= s.n_new[b];
 
   // ---- greedy / sampling: every row is an independent hypothesis
-  if (o.beam == 1) {
-    if (tid < Kr && !s.row_done[row0 + tid]) {
+  if (independent) {
+    if (tid < N && !s.row_done[row0 + tid]) {
       const int r = row0 + tid;
       const int tok = s.cand_tok[(long)r * MAX_CAND];
       const float val = s.cand_val[(long)r * MAX_CAND];
@@ -366,11 +374,11 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
     if (tid == 0) {
       s.step[b] = step + 1;
       bool all = true;
-      for (int j = 0; j < Kr; ++j) all = all && s.row_done[row0 + j];
+      for (int j = 0; j < N; ++j) all = all && s.row_done[row0 + j];
       finished = all ? 1 : 0;
       if (all) {
-        s.hyp_count[b] = Kr;
-        for (int j = 0; j < Kr; ++j) {
+        s.hyp_count[b] = N;
+        for (int j = 0; j < N; ++j) {
           s.hyp_cum[b * MAX_HYPS + j] = s.cum[row0 + j];
           s.hyp_len[b * MAX_HYPS + j] = s.gen_len[row0 + j];
         }
@@ -379,7 +387,7 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
     }
     __syncthreads();
     if (finished) {
-      for (int j = 0; j < Kr; ++j)
+      for (int j = 0; j < N; ++j)
         for (int p = tid; p < s.gen_len[row0 + j]; p += 128)
           s.hyp_tok[((long)b * MAX_HYPS + j) * T_MAX + p] = s.hist[(long)(row0 + j) * T_MAX + p];
     }
@@ -532,11 +540,12 @@ __global__ void decode_init_kernel(DecodeState s, SearchOpts o, VocabIds v, int 
   // stream's first row) the first decode step feeds the LAST prompt token
   const int fed0 = (prefilled && s.force_len[b] == 0) ? P - 1 : 0;
   // independent sampling rows all continue from the prompt cache of row 0 (what search_streams does when the feeding
-  // reaches the last prompt token)
-  const bool fan_out = o.beam == 1 && s.force_len[b] == 0 && fed0 == P - 1;
+  // reaches the last prompt token); a stream that uses N < Kr rows leaves rows N .. Kr-1 inactive for its whole life
+  const bool fan_out = (o.beam == 1 || s.smode[b] != 0) && s.force_len[b] == 0 && fed0 == P - 1;
+  const int N = fan_out ? s.nrows[b] : 1;
   if (tid < Kr) {
     const int r = row0 + tid;
-    const bool on = tid == 0 || fan_out;
+    const bool on = tid < N;
     s.tok_in[r] = s.prompt[(long)b * T_MAX + fed0];
     s.pos[r] = fed0;
     s.active[r] = on ? 1 : 0;
@@ -546,10 +555,8 @@ __global__ void decode_init_kernel(DecodeState s, SearchOpts o, VocabIds v, int 
     s.row_done[r] = 0;
     s.nospeech_row[r] = 0.f;
   }
-  for (int j = 0; j < Kr; ++j) {
-    if (j > 0 && !fan_out) break;
+  for (int j = 0; j < N; ++j)
     for (int p = tid; p < fed0; p += blockDim.x) s.src[(long)(row0 + j) * T_MAX + p] = (short)row0;
-  }
   if (tid == 0) {
     s.fed[b] = fed0;
     s.step[b] = 0;

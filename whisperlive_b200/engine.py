@@ -391,7 +391,8 @@ class B200Whisper:
     # ------------------------------------------------------------------ N2: decode session (step-level admission)
     def open_decode_session(self, capacity: Optional[int] = None, **generate_kwargs) -> "DecodeSession":
         """A decode loop whose streams come and go independently (``wl_session_*``): same keyword arguments as
-        ``generate`` (``max_length`` is given per stream at admission; sampling options are not accepted)."""
+        ``generate`` (``max_length`` is given per stream at admission; the session's own search does not sample, a
+        stream samples when ``DecodeSession.admit`` is given a ``sampling`` spec for it)."""
         # one session per engine context: whatever an earlier owner left behind (a scheduler stopped mid-decode) is dropped
         with self._lock:
             rc = self.lib.wl_session_close(self.ctx)
@@ -649,8 +650,13 @@ class DecodeSession:
                 result = sess.collect(i)            # WhisperGenerationResult, the index is free again
             ... admit whoever arrived meanwhile ...
 
-    One-shot engine calls (``encode``, ``generate`` for a temperature-fallback retry, ``align``, ``detect_language``)
-    may be interleaved between two ``run`` calls: the session owns its decode state and self-attention cache."""
+    One-shot engine calls (``encode``, ``generate``, ``align``, ``detect_language``) may be interleaved between two
+    ``run`` calls: the session owns its decode state and self-attention cache.
+
+    The session's own search is beam or greedy.  A stream may instead be admitted for Gumbel-max sampling (a
+    temperature-fallback rung): ``admit(..., sampling=[(temperature, num_hypotheses, seed, noise_key), ...])`` decodes it
+    over ``num_hypotheses <= rows_per_stream`` independent rows with exactly the draws ``generate(seed=seed)`` gives the
+    stream at batch position ``noise_key``, whoever else is in the loop."""
 
     def __init__(self, engine: B200Whisper, capacity: int, *, beam_size: int = 5, patience: float = 1, num_hypotheses: int = 1,
                  length_penalty: float = 1, repetition_penalty: float = 1, no_repeat_ngram_size: int = 0,
@@ -660,10 +666,13 @@ class DecodeSession:
         if repetition_penalty != 1 or no_repeat_ngram_size != 0:
             raise NotImplementedError("repetition_penalty / no_repeat_ngram_size other than the reference's 1 / 0")
         if int(beam_size) == 1 and sampling_topk != 1 and sampling_temperature > 0:
-            raise ValueError("a decode session does not sample: run temperature-fallback retries through generate()")
+            raise ValueError("a decode session's own search does not sample: pass sampling= per stream to admit()")
         self.engine = engine
         self.capacity = int(capacity)
         self.num_hypotheses = int(num_hypotheses)
+        # decoder rows per stream: the most hypotheses a sampled stream may ask for
+        self.rows_per_stream = int(beam_size) if int(beam_size) > 1 else self.num_hypotheses
+        self._nh: Dict[int, int] = {}                 # index -> hypotheses its stream returns
         self._sup = np.asarray(sorted({int(t) for t in (suppress_tokens or ()) if t >= 0}), dtype=np.int32)
         self._opts = _lib.WlGenOpts(
             beam_size=int(beam_size), patience=float(patience), num_hypotheses=self.num_hypotheses,
@@ -691,13 +700,15 @@ class DecodeSession:
 
     # -- admission ---------------------------------------------------------------------------------
     def admit(self, features: Sequence[EncoderOutput], prompts: Sequence[Sequence[int]], max_lengths: Sequence[int],
-              indices: Optional[Sequence[int]] = None) -> List[int]:
-        """Admit one stream per (single-stream encoder view, prompt, max_length); returns the indices they decode in."""
+              indices: Optional[Sequence[int]] = None,
+              sampling: Optional[Sequence[Optional[Tuple[float, int, int, int]]]] = None) -> List[int]:
+        """Admit one stream per (single-stream encoder view, prompt, max_length); returns the indices they decode in.
+        ``sampling``: per stream None (the session's search) or ``(temperature, num_hypotheses, seed, noise_key)``."""
         n = len(prompts)
         if n == 0:
             return []
-        if len(features) != n or len(max_lengths) != n:
-            raise ValueError("admit: features / prompts / max_lengths differ in length")
+        if len(features) != n or len(max_lengths) != n or (sampling is not None and len(sampling) != n):
+            raise ValueError("admit: features / prompts / max_lengths / sampling differ in length")
         free = self.free_indices()
         if indices is None:
             if n > len(free):
@@ -715,13 +726,22 @@ class DecodeSession:
         idx = np.asarray(list(indices), dtype=np.int32)
         sl = np.asarray(slots, dtype=np.int32)
         ml = np.asarray(list(max_lengths), dtype=np.int32)
+        specs = list(sampling) if sampling is not None else [None] * n
+        search = (_lib.WlStreamSearch * n)()
+        for q, sp in zip(search, specs):
+            if sp is not None:
+                t, nh, seed, key = sp
+                q.sample, q.num_hypotheses, q.temperature = 1, int(nh), float(t)
+                q.seed, q.noise_key = int(seed) & 0xFFFFFFFF, int(key)
         eng = self.engine
         with eng._lock:
-            rc = eng.lib.wl_session_admit(eng.ctx, n, _lib.ptr(idx, C.c_int32), _lib.ptr(sl, C.c_int32), _lib.ptr(flat, C.c_int32),
-                                          _lib.ptr(off, C.c_int32), _lib.ptr(ml, C.c_int32))
+            rc = eng.lib.wl_session_admit_ex(eng.ctx, n, _lib.ptr(idx, C.c_int32), _lib.ptr(sl, C.c_int32),
+                                             _lib.ptr(flat, C.c_int32), _lib.ptr(off, C.c_int32), _lib.ptr(ml, C.c_int32),
+                                             search if sampling is not None else None)
             _lib.check(eng.lib, eng.ctx, rc, "wl_session_admit")
-        for i, f in zip(idx.tolist(), features):
+        for i, f, sp in zip(idx.tolist(), features, specs):
             self._held[i] = f
+            self._nh[i] = self.num_hypotheses if sp is None else int(sp[1])
         return idx.tolist()
 
     # -- the token loop ----------------------------------------------------------------------------
@@ -742,7 +762,7 @@ class DecodeSession:
 
     def collect(self, index: int) -> WhisperGenerationResult:
         eng = self.engine
-        NH = self.num_hypotheses
+        NH = self._nh.get(int(index), self.num_hypotheses)
         ids = np.zeros((NH, T_MAX), dtype=np.int32)
         lens = np.zeros(NH, dtype=np.int32)
         score = np.zeros(NH, dtype=np.float32)
@@ -753,6 +773,7 @@ class DecodeSession:
                                             _lib.ptr(score, C.c_float), C.byref(nsp), C.byref(steps))
             _lib.check(eng.lib, eng.ctx, rc, "wl_session_collect")
         self._held.pop(int(index), None)
+        self._nh.pop(int(index), None)
         seqs, scs = [], []
         for h in range(NH):
             if lens[h] >= 0:

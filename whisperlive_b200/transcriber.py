@@ -295,16 +295,28 @@ class _StreamJob:
                 f"The length of the prompt is {len(self.prompt)}, and the `max_new_tokens` "
                 f"{max_length - len(self.prompt)}. Thus, the combined length of the prompt and `max_new_tokens` is: "
                 f"{max_length}. This exceeds the `max_length` of the Whisper model: {self.m.max_length}.")
-        kw = dict(length_penalty=o.length_penalty, repetition_penalty=o.repetition_penalty,
-                  no_repeat_ngram_size=o.no_repeat_ngram_size, max_length=max_length, return_scores=True,
-                  return_no_speech_prob=True, suppress_blank=o.suppress_blank, suppress_tokens=o.suppress_tokens,
-                  max_initial_timestamp_index=int(round(o.max_initial_timestamp / self.m.time_precision)))
+        kw = dict(self._shared_kwargs(), max_length=max_length)
         t = self.temperature
         if t > 0:
             kw.update(beam_size=1, num_hypotheses=o.best_of, sampling_topk=0, sampling_temperature=t)
         else:
             kw.update(beam_size=o.beam_size, patience=o.patience)
         return kw
+
+    def _shared_kwargs(self) -> dict:
+        """The generate options every rung of the ladder shares."""
+        o = self.opt
+        return dict(length_penalty=o.length_penalty, repetition_penalty=o.repetition_penalty,
+                    no_repeat_ngram_size=o.no_repeat_ngram_size, return_scores=True, return_no_speech_prob=True,
+                    suppress_blank=o.suppress_blank, suppress_tokens=o.suppress_tokens,
+                    max_initial_timestamp_index=int(round(o.max_initial_timestamp / self.m.time_precision)))
+
+    def session_kwargs(self) -> dict:
+        """Options of the decode session this stream's windows decode in, whatever rung they are on: rung 0's beam
+        search and the shared options (``max_length`` is given per stream at admission, a sampling rung joins with a
+        per-stream sampling spec)."""
+        o = self.opt
+        return dict(self._shared_kwargs(), beam_size=o.beam_size, patience=o.patience, num_hypotheses=1)
 
     def accept(self, result) -> bool:
         """Record one decode; True when the window is settled (else retry at the next temperature)."""
@@ -605,8 +617,11 @@ class TranscribeSession:
         others are in the middle of a 100-token decode starts decoding a few token steps later, and is answered when ITS
         last window settles.  Falls back to ``round()`` on engines without decode sessions.
 
-        What stays on the one-shot path: sampling retries of the temperature ladder (their noise is keyed per call),
-        streams whose search options differ from the open session's while it is busy wait for it to drain."""
+        A session is keyed by its streams' rung-0 options (``_StreamJob.session_kwargs``), so every rung of a stream
+        decodes in it: a sampling rung of the temperature ladder joins the running loop with a per-stream sampling spec
+        when ``best_of`` fits the session's rows per stream, its noise seeded by ``session_noise_seed`` (noise key 0).
+        What stays on the one-shot path: sampling rungs whose ``best_of`` does not fit, or whose rung-0 options differ
+        from the open session's while it is busy (beam rungs in that case wait for the session to drain)."""
         m = self.m
         if not hasattr(m.model, "open_decode_session"):
             return self.round()
@@ -614,37 +629,45 @@ class TranscribeSession:
         self.rounds += 1
         self._encode_pending()
         one_shot: List[_Entry] = []
-        joining: List[Tuple[_Entry, int]] = []
+        joining: List[Tuple[_Entry, int, Optional[tuple]]] = []
         waiting = [e for e in self.entries if e.state == "decode"]
         for e in waiting:
             try:
                 kw = e.job.generate_kwargs()
+                skw = e.job.session_kwargs()
             except Exception as ex:
                 self._fail(e, ex)
                 continue
-            if kw.get("beam_size", 1) == 1 and kw.get("sampling_topk", 1) != 1 and kw.get("sampling_temperature", 0) > 0:
-                one_shot.append(e)
-                continue
-            key = json.dumps({a: v for a, v in kw.items() if a != "max_length"}, sort_keys=True, default=list)
+            key = json.dumps(skw, sort_keys=True, default=list)
             ds = self._dsess
             if ds is None or (key != self._dsess_key and ds.live == 0 and not joining):
                 if ds is not None:
                     ds.close()
-                skw = {a: v for a, v in kw.items() if a != "max_length"}
                 ds = self._dsess = m.model.open_decode_session(**skw)
                 self._dsess_key = key
+            spec = None
+            if kw.get("beam_size", 1) == 1 and kw.get("sampling_topk", 1) != 1 and kw.get("sampling_temperature", 0) > 0:
+                # a session model without per-stream sampling has no rows_per_stream: its rungs stay one-shot
+                if key != self._dsess_key or kw["num_hypotheses"] > getattr(ds, "rows_per_stream", 0):
+                    one_shot.append(e)
+                    continue
+                spec = (kw["sampling_temperature"], kw["num_hypotheses"],
+                        session_noise_seed(e.handle, e.job.seek, e.job.temp_idx), 0)
             if key != self._dsess_key or len(joining) >= len(ds.free_indices()):
                 continue                                   # next step_round: the loop has to drain / free an index first
-            joining.append((e, kw["max_length"]))
+            joining.append((e, kw["max_length"], spec))
         if joining:                                        # ONE admission = one batched prefill pass for all of them
             ds = self._dsess
+            specs = [sp for _, _, sp in joining]
             try:
-                idxs = ds.admit([e.job.enc for e, _ in joining], [e.job.prompt for e, _ in joining], [ml for _, ml in joining])
+                idxs = ds.admit([e.job.enc for e, _, _ in joining], [e.job.prompt for e, _, _ in joining],
+                                [ml for _, ml, _ in joining],
+                                **({"sampling": specs} if any(sp is not None for sp in specs) else {}))
             except Exception as ex:
-                for e, _ in joining:
+                for e, _, _ in joining:
                     self._fail(e, ex)
                 idxs = []
-            for idx, (e, _) in zip(idxs, joining):
+            for idx, (e, _, _) in zip(idxs, joining):
                 e.state = "running"
                 self._running[idx] = e
                 self.admitted_steps.append(getattr(ds, "steps", 0))
@@ -790,6 +813,23 @@ class TranscribeSession:
         if e.parent is not None:
             e.parent.done_one()
             e.parent = None
+
+
+def _lowbias32(x: int) -> int:
+    x &= 0xFFFFFFFF
+    x ^= x >> 16
+    x = (x * 0x7FEB352D) & 0xFFFFFFFF
+    x ^= x >> 15
+    x = (x * 0x846CA68B) & 0xFFFFFFFF
+    return x ^ (x >> 16)
+
+
+def session_noise_seed(handle: int, seek: int, rung: int) -> int:
+    """32-bit noise seed of a sampling rung decoded in a step-round decode session (noise key 0):
+    ``lowbias32(lowbias32(lowbias32(handle) ^ seek) ^ rung)`` over the stream's handle in its ``TranscribeSession``, the
+    window's ``seek`` (frames) and the rung's index in the temperature ladder.  A stream's draws therefore depend only
+    on the stream itself -- not on which streams share its rounds or when it arrived."""
+    return _lowbias32(_lowbias32(_lowbias32(handle) ^ (seek & 0xFFFFFFFF)) ^ (rung & 0xFFFFFFFF))
 
 
 def _join_encoded(views: List[Any]):
