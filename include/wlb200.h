@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 4
+#define WL_ABI_VERSION 5
 
 typedef struct wl_ctx wl_ctx;
 
@@ -118,6 +118,20 @@ int wl_generate(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* pro
  *   wl_session_collect hypotheses of one finished index (outputs like one stream of wl_generate); the index goes idle.
  *                      out_ids / out_len / out_score hold the index's own hypothesis count: the sampled stream's
  *                      num_hypotheses, else the session's.
+ *   wl_session_peek    the interim hypothesis of n indices (index[n]), for text before a stream finishes: out_ids
+ *                      [n][448], out_len / out_score / out_no_speech / out_step / out_final [n] (the last three may be
+ *                      NULL).  A stream still decoding reports its leading row -- row 0 for the session's own search
+ *                      (beam search keeps its best live beam there), the alive row with the highest cum_logprob (lowest
+ *                      row on ties) for a sampled stream -- as the tokens generated so far (the layout of
+ *                      wl_session_collect), score cum_logprob / len^length_penalty, step = generation steps done, final = 0.
+ *                      A finished, uncollected index reports the hypothesis wl_session_collect returns first, final = 1,
+ *                      and stays collectable (ranked with collect's own arithmetic).  One kernel, one device-to-host copy,
+ *                      one stream synchronise -- plus one small copy in the rare case of a finished index whose last-bit
+ *                      near-tie the device ranked the other way (length_penalty other than 0 or 1); legal between
+ *                      two wl_session_run calls.  A beam stream's interim hypothesis need not be a prefix of its final one.
+ *   wl_session_cancel  n distinct indices go idle at once: a running stream stops decoding, a finished one's result is
+ *                      discarded; each index can be admitted again right away.  The streams in flight are untouched.
+ *   Both fail before anything is launched, with no index changed, when an index is idle or out of range.
  *   wl_session_close   drops whatever is still in flight.
  * The session has its own decode state and self-attention cache: wl_generate / wl_align / wl_detect_language /
  * wl_encode may be called between two wl_session_run calls (temperature-fallback retries, word alignment of a finished
@@ -137,6 +151,9 @@ int wl_session_admit_ex(wl_ctx* ctx, int32_t n, const int32_t* index, const int3
 int wl_session_run(wl_ctx* ctx, int32_t max_steps, int32_t break_on_finish, int32_t* done_out, int32_t* steps_ran);
 int wl_session_collect(wl_ctx* ctx, int32_t index, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
                        int32_t* out_steps);
+int wl_session_peek(wl_ctx* ctx, int32_t n, const int32_t* index, int32_t* out_ids, int32_t* out_len, float* out_score,
+                    float* out_no_speech, int32_t* out_step, int32_t* out_final);
+int wl_session_cancel(wl_ctx* ctx, int32_t n, const int32_t* index);
 int wl_session_close(wl_ctx* ctx);
 
 /* K13. probs [B, n_lang] softmax over the language tokens after feeding <|startoftranscript|>. */

@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 4
+ABI_VERSION = 5
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -67,6 +67,8 @@ SIGNATURES = {
                                       C.POINTER(WlStreamSearch)]),
     "wl_session_run": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, c_i32p, c_i32p]),
     "wl_session_collect": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_f32p, c_f32p, c_i32p]),
+    "wl_session_peek": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i32p, c_i32p]),
+    "wl_session_cancel": (C.c_int, [C.c_void_p, C.c_int32, c_i32p]),
     "wl_session_close": (C.c_int, [C.c_void_p]),
     "wl_detect_language": (C.c_int, [C.c_void_p, c_i32p, C.c_int32, c_f32p]),
     "wl_align": (C.c_int, [C.c_void_p, c_i32p, C.c_int32, c_i32p, C.c_int32, c_i32p, c_i32p, c_i32p, C.c_int32, c_i32p,

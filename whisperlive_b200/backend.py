@@ -17,7 +17,9 @@ from __future__ import annotations
 
 import json
 import logging
+import os
 import threading
+import time
 
 try:  # the reference package must be importable: this module is a plugin for it
     from whisper_live.backend.base import ServeClientBase
@@ -36,6 +38,9 @@ if ServeClientBase is not None:
         MAX_STREAMS = 8          # streams batched per decode step on this GPU
         BATCH_WINDOW_MS = 20
         MODEL_FACTORY = None     # tests inject a callable(model_name) -> transcriber
+        PARTIALS = os.environ.get("WLB200_PARTIALS", "0") == "1"   # interim text of the chunk in flight
+        REQUEST_TIMEOUT_S = 30
+        WAIT_SLICE_S = 0.05      # how often a waiting client thread looks at exit / new interim text
 
         def __init__(self, websocket, task="transcribe", device=None, language=None, client_uid=None, model="small.en",
                      initial_prompt=None, vad_parameters=None, use_vad=True, single_model=True, send_last_n_segments=10,
@@ -94,18 +99,51 @@ if ServeClientBase is not None:
                                                 "language_prob": info.language_probability}))
 
         def transcribe_audio(self, input_sample):
+            """Submit the chunk and wait for it in short slices: interim text goes out while it decodes (``PARTIALS``),
+            and a timeout or a disconnect (``self.exit``) cancels the request so it stops using the engine."""
             request = BatchRequest(audio=input_sample, language=self.language, task=self.task,
                                    initial_prompt=self.initial_prompt, use_vad=self.use_vad,
                                    vad_parameters=self.vad_parameters if self.use_vad else None,
-                                   word_timestamps=self.word_timestamps, client_uid=self.client_uid, hotwords=self.hotwords)
+                                   word_timestamps=self.word_timestamps, client_uid=self.client_uid, hotwords=self.hotwords,
+                                   want_partials=self.PARTIALS)
             ServeClientB200.BATCH_WORKER.submit(request)
-            if not request.future.wait(timeout=30):
-                raise TimeoutError("transcription request timed out after 30 s")
+            duration = input_sample.shape[0] / self.RATE
+            deadline = time.monotonic() + self.REQUEST_TIMEOUT_S
+            sent = 0
+            while not request.future.is_set():
+                if self.exit:
+                    request.cancel()
+                    return None
+                left = deadline - time.monotonic()
+                if left <= 0:
+                    request.cancel()
+                    raise TimeoutError(f"transcription request timed out after {self.REQUEST_TIMEOUT_S} s")
+                request.partial.event.wait(timeout=min(self.WAIT_SLICE_S, left))
+                request.partial.event.clear()
+                version, segs = request.partial.latest()
+                if version != sent and not request.future.is_set():
+                    sent = version
+                    self.send_interim(segs, duration)
             if request.error:
                 raise request.error
             if self.language is None and request.info is not None:
                 self.set_language(request.info)
             return request.result
+
+        def send_interim(self, segments, duration):
+            """The unfinished text of the chunk in flight as the reference's incomplete line: the recent transcript plus
+            one ``completed: False`` segment (``prepare_segments(last)``).  Segments over ``no_speech_thresh`` are left
+            out as ``update_segments`` does; the transcript, ``timestamp_offset`` and the rest of the commit state stay
+            as they are."""
+            kept = [s for s in segments if self.get_segment_no_speech_prob(s) <= self.no_speech_thresh]
+            if not kept:
+                return
+            with self.lock:
+                offset = self.timestamp_offset
+            last = self.format_segment(offset + self.get_segment_start(kept[0]),
+                                       offset + min(duration, self.get_segment_end(kept[-1])),
+                                       "".join(s.text for s in kept), completed=False)
+            self.send_transcription_to_client(self.prepare_segments(last))
 
         def handle_transcription_output(self, result, duration):
             segments = []

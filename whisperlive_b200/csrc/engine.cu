@@ -151,6 +151,7 @@ struct wl_ctx {
     __half *kcache = nullptr, *vcache = nullptr;
     unsigned* mask = nullptr;
     int* idx_dev = nullptr;
+    int* peek_dev = nullptr;            // wl_session_peek staging [max_streams][PEEK_STRIDE]
     std::vector<int> hp, meta;          // host shadows: prompts [cap][T_MAX], per-stream metadata [META_ROWS][cap]
     std::vector<char> used, finished;   // index holds an admitted stream / that stream has finished decoding
     std::vector<int> nh;                // hypotheses the index's stream returns: N when it samples, else NH
@@ -1303,6 +1304,11 @@ static int upload_streams(wl_ctx* c, const int32_t* slots, int B, const int32_t*
   return max_steps;
 }
 
+// the score CT2 ranks a hypothesis by: cum_logprob / len^length_penalty
+static float hyp_score(float cum, int len, float length_penalty) {
+  return length_penalty == 0.f ? cum : cum / powf((float)std::max(len, 1), length_penalty);
+}
+
 // finished hypotheses of one stream (device order) -> the NH best by cum_logprob / len^length_penalty, like CT2
 static void emit_hyps(int NH, float length_penalty, int count, const int* h_len, const float* h_cum, const int* h_tok, int32_t* out_ids,
                       int32_t* out_len, float* out_score) {
@@ -1311,7 +1317,7 @@ static void emit_hyps(int NH, float length_penalty, int count, const int* h_len,
   std::vector<float> score(cnt);
   for (int i = 0; i < cnt; ++i) {
     order[i] = i;
-    score[i] = length_penalty == 0.f ? h_cum[i] : h_cum[i] / powf((float)std::max(h_len[i], 1), length_penalty);
+    score[i] = hyp_score(h_cum[i], h_len[i], length_penalty);
   }
   std::stable_sort(order.begin(), order.end(), [&](int a, int bb) { return score[a] > score[bb]; });
   for (int hh = 0; hh < NH; ++hh) {
@@ -1545,6 +1551,7 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
     ss.vcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
     ss.mask = dalloc<unsigned>(c, (c->V + 31) / 32 + 1);
     ss.idx_dev = dalloc<int>(c, c->Bm);
+    ss.peek_dev = dalloc<int>(c, (size_t)c->Bm * PEEK_STRIDE);
     ss.allocated = true;
   }
   ss.cap = capacity; ss.K = K; ss.Kr = Kr; ss.NH = o->num_hypotheses; ss.length_penalty = o->length_penalty;
@@ -1729,6 +1736,86 @@ extern "C" int wl_session_collect(wl_ctx* c, int32_t index, int32_t* out_ids, in
   if (out_steps) *out_steps = h_steps[0];
   ss.used[index] = 0;
   ss.finished[index] = 0;
+  API_END(c)
+}
+
+// every listed index must hold a stream (running, or finished and not yet collected); checked before anything launches
+static void check_session_indices(const wl_ctx::Session& ss, int n, const int32_t* index, bool distinct, const char* what) {
+  WL_CHECK(ss.open, WL_ERR_STATE, "%s: no open session", what);
+  WL_CHECK(n >= 1 && n <= ss.cap && index, WL_ERR_ARG, "%s: bad arguments (%d indices, capacity %d)", what, n, ss.cap);
+  for (int i = 0; i < n; ++i) {
+    WL_CHECK(index[i] >= 0 && index[i] < ss.cap, WL_ERR_ARG, "%s: index %d outside the session capacity %d", what, index[i], ss.cap);
+    WL_CHECK(ss.used[index[i]], WL_ERR_STATE, "%s: index %d is idle", what, index[i]);
+    if (distinct)
+      for (int j = 0; j < i; ++j) WL_CHECK(index[j] != index[i], WL_ERR_ARG, "%s: index %d listed twice", what, index[i]);
+  }
+}
+
+extern "C" int wl_session_peek(wl_ctx* c, int32_t n, const int32_t* index, int32_t* out_ids, int32_t* out_len, float* out_score,
+                               float* out_no_speech, int32_t* out_step, int32_t* out_final) {
+  API_BEGIN(c)
+  wl_ctx::Session& ss = c->sess;
+  check_session_indices(ss, n, index, false, "wl_session_peek");
+  WL_CHECK(out_ids && out_len && out_score, WL_ERR_ARG, "wl_session_peek: bad arguments");
+  cudaStream_t st = c->st;
+  ensure_host(c, (size_t)n * PEEK_STRIDE + n, 16);
+  int* h = c->h_int;
+  int* hidx = h + (size_t)n * PEEK_STRIDE;
+  memcpy(hidx, index, (size_t)n * 4);
+  WL_CUDA(cudaMemcpyAsync(ss.idx_dev, hidx, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  session_peek(st, ss.ds, ss.so, ss.length_penalty, ss.idx_dev, ss.peek_dev, n);
+  WL_CUDA(cudaMemcpyAsync(h, ss.peek_dev, (size_t)n * PEEK_STRIDE * 4, cudaMemcpyDeviceToHost, st));
+  WL_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) {
+    const int* e = h + (size_t)i * PEEK_STRIDE;
+    int len = e[0];
+    float cum, ns;
+    memcpy(&cum, e + 1, 4);
+    memcpy(&ns, e + 2, 4);
+    int best = e[5];
+    if (e[4]) {   // finished: rank its hypotheses with emit_hyps' arithmetic (first of the best scores)
+      float bs = 0.f;
+      for (int k = 0; k < e[6]; ++k) {
+        float ck;
+        memcpy(&ck, e + PEEK_TAB + MAX_HYPS + k, 4);
+        const float sc = hyp_score(ck, e[PEEK_TAB + k], ss.length_penalty);
+        if (k == 0 || sc > bs) { best = k; bs = sc; }
+      }
+    }
+    if (e[4] && best != e[5]) {   // a last-bit near-tie the device's powf ranked the other way: fetch the host's pick
+      len = e[PEEK_TAB + best];
+      memcpy(&cum, e + PEEK_TAB + MAX_HYPS + best, 4);
+      if (len > 0)
+        WL_CUDA(cudaMemcpy(out_ids + (size_t)i * T_MAX, ss.ds.hyp_tok + ((size_t)index[i] * MAX_HYPS + best) * T_MAX,
+                           (size_t)len * 4, cudaMemcpyDeviceToHost));
+    } else if (len > 0) {
+      memcpy(out_ids + (size_t)i * T_MAX, e + PEEK_HDR, (size_t)len * 4);
+    }
+    out_len[i] = len;
+    out_score[i] = len < 0 ? 0.f : hyp_score(cum, len, ss.length_penalty);
+    if (out_no_speech) out_no_speech[i] = ns;
+    if (out_step) out_step[i] = e[3];
+    if (out_final) out_final[i] = e[4];
+  }
+  API_END(c)
+}
+
+extern "C" int wl_session_cancel(wl_ctx* c, int32_t n, const int32_t* index) {
+  API_BEGIN(c)
+  wl_ctx::Session& ss = c->sess;
+  check_session_indices(ss, n, index, true, "wl_session_cancel");
+  cudaStream_t st = c->st;
+  ensure_host(c, (size_t)n, 16);
+  memcpy(c->h_int, index, (size_t)n * 4);
+  WL_CUDA(cudaMemcpyAsync(ss.idx_dev, c->h_int, (size_t)n * 4, cudaMemcpyHostToDevice, st));
+  session_cancel(st, ss.ds, ss.Kr, ss.idx_dev, n);
+  WL_CUDA(cudaStreamSynchronize(st));
+  for (int i = 0; i < n; ++i) {
+    const int b = index[i];
+    if (!ss.finished[b]) ss.live -= 1;
+    ss.used[b] = 0;
+    ss.finished[b] = 0;
+  }
   API_END(c)
 }
 

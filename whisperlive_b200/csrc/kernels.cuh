@@ -164,6 +164,19 @@ void loop_condition(cudaStream_t st, const DecodeState& s, cudaGraphConditionalH
 void decode_init(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, int B, int R, int prefilled = 0,
                  const int* index = nullptr);
 
+// Decode sessions, between two runs (never while the loop graph is in flight).  session_peek: the interim hypothesis of
+// the n stream indices index[n] -> out [n][PEEK_STRIDE] ints: [0] token count (-1: finished without a hypothesis),
+// [1] cum_logprob and [2] no-speech probability (float bits), [3] generation steps, [4] 1 = finished, [PEEK_HDR ..] the
+// tokens; a finished stream also gives [5] the hypothesis slot reported, [6] its hypothesis count and at [PEEK_TAB ..]
+// the lengths, then the cum_logprobs (float bits), of its MAX_HYPS hypothesis slots.
+// session_cancel: the n listed indices go idle (done, rows inactive, n_done counts them).
+constexpr int PEEK_TAB = 8;
+constexpr int PEEK_HDR = PEEK_TAB + 2 * MAX_HYPS;
+constexpr int PEEK_STRIDE = PEEK_HDR + T_MAX;
+void session_peek(cudaStream_t st, const DecodeState& s, const SearchOpts& o, float length_penalty, const int* index, int* out,
+                  int n);
+void session_cancel(cudaStream_t st, const DecodeState& s, int Kr, const int* index, int n);
+
 // ---------------------------------------------------------------------------- K8 batched prefill helpers (prefill.cu)
 void prefill_embed(cudaStream_t st, const int* tok, const int* pos, const int* active, const int* wrow, const __half* emb,
                    const __half* pos_emb, float* x, short* src, int M, int d);

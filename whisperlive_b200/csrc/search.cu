@@ -577,4 +577,88 @@ void decode_init(cudaStream_t st, const DecodeState& s, const SearchOpts& o, con
   note_launch(1);
 }
 
+// ============================================================================ decode sessions between two runs
+// One block per listed stream index.  A stream still decoding reports its leading row: row 0 (beam search keeps the best
+// live beam there; greedy), or for a sampling stream the alive row with the highest cum (lowest row on ties).  A finished
+// stream reports the hypothesis wl_session_collect would put first: the best cum / len^length_penalty, lowest slot on
+// ties (emit_hyps' stable sort), and its whole hypothesis table, so the host can rank it with the host's own powf (the
+// device's may differ in the last bit for a penalty other than 0 or 1).  Reads the decode state only.
+__global__ void __launch_bounds__(128) session_peek_kernel(DecodeState s, SearchOpts o, float length_penalty,
+                                                           const int* __restrict__ index, int* __restrict__ out) {
+  const int b = index[blockIdx.x], tid = threadIdx.x;
+  const int Kr = o.rows_per_stream, row0 = b * Kr;
+  int* dst = out + (long)blockIdx.x * PEEK_STRIDE;
+  __shared__ const int* sh_tok;
+  __shared__ int sh_len;
+  if (tid == 0) {
+    const int fin = s.done[b];
+    int len;
+    float cum;
+    const int* tok;
+    if (fin) {
+      const int cnt = min(s.hyp_count[b], MAX_HYPS);
+      int best = -1;
+      float bs = 0.f;
+      for (int i = 0; i < cnt; ++i) {
+        const float c = s.hyp_cum[b * MAX_HYPS + i];
+        const int hl = s.hyp_len[b * MAX_HYPS + i];
+        const float l = (float)max(hl, 1);
+        // the host's powf(l, 1) is exactly l: divide directly so the default penalty ranks exactly like emit_hyps
+        const float sc = length_penalty == 0.f ? c : (length_penalty == 1.f ? c / l : c / powf(l, length_penalty));
+        if (best < 0 || sc > bs) { best = i; bs = sc; }
+        dst[PEEK_TAB + i] = hl;
+        dst[PEEK_TAB + MAX_HYPS + i] = __float_as_int(c);
+      }
+      dst[5] = best;
+      dst[6] = cnt;
+      len = best < 0 ? -1 : s.hyp_len[b * MAX_HYPS + best];
+      cum = best < 0 ? 0.f : s.hyp_cum[b * MAX_HYPS + best];
+      tok = s.hyp_tok + ((long)b * MAX_HYPS + max(best, 0)) * T_MAX;
+    } else {
+      int r = row0;
+      if (s.smode[b] != 0)
+        for (int j = 1; j < s.nrows[b]; ++j) {
+          const int q = row0 + j;
+          if (!s.row_done[q] && (s.row_done[r] || s.cum[q] > s.cum[r])) r = q;
+        }
+      len = s.gen_len[r];
+      cum = s.cum[r];
+      tok = s.hist + (long)r * T_MAX;
+    }
+    dst[0] = len;
+    dst[1] = __float_as_int(cum);
+    dst[2] = __float_as_int(s.no_speech[b]);
+    dst[3] = s.step[b];
+    dst[4] = fin;
+    sh_tok = tok;
+    sh_len = len;
+  }
+  __syncthreads();
+  for (int p = tid; p < sh_len; p += blockDim.x) dst[PEEK_HDR + p] = sh_tok[p];
+}
+
+void session_peek(cudaStream_t st, const DecodeState& s, const SearchOpts& o, float length_penalty, const int* index, int* out,
+                  int n) {
+  session_peek_kernel<<<n, 128, 0, st>>>(s, o, length_penalty, index, out);
+  WL_CUDA(cudaGetLastError());
+  note_launch(1);
+}
+
+// The listed indices go idle: done, rows inactive.  A stream still decoding is counted into n_done here, the way
+// finish_stream counts a stream that ends (decode_init's admission takes it out again); a finished one already is.
+__global__ void session_cancel_kernel(DecodeState s, int Kr, const int* __restrict__ index) {
+  const int b = index[blockIdx.x], j = threadIdx.x;
+  if (j < Kr) s.active[b * Kr + j] = 0;
+  if (j == 0 && !s.done[b]) {
+    s.done[b] = 1;
+    atomicAdd(s.n_done, 1);
+  }
+}
+
+void session_cancel(cudaStream_t st, const DecodeState& s, int Kr, const int* index, int n) {
+  session_cancel_kernel<<<n, 32, 0, st>>>(s, Kr, index);
+  WL_CUDA(cudaGetLastError());
+  note_launch(1);
+}
+
 }  // namespace wl

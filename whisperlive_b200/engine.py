@@ -781,6 +781,43 @@ class DecodeSession:
                 scs.append(float(score[h]))
         return WhisperGenerationResult(seqs, scs, float(nsp.value), int(steps.value))
 
+    def peek(self, indices: Sequence[int]) -> List[Tuple[List[int], float, float, int, bool]]:
+        """Interim hypothesis of each index between two ``run`` calls: ``(tokens, score, no_speech_prob, step, final)``.
+        A running stream reports its leading row (a beam stream's need not be a prefix of its final hypothesis), a
+        finished one the hypothesis ``collect`` returns first, and stays collectable.  One kernel and one copy for all."""
+        n = len(indices)
+        if n == 0:
+            return []
+        idx = np.asarray(list(indices), dtype=np.int32)
+        ids = np.zeros((n, T_MAX), dtype=np.int32)
+        lens = np.zeros(n, dtype=np.int32)
+        score = np.zeros(n, dtype=np.float32)
+        nsp = np.zeros(n, dtype=np.float32)
+        step = np.zeros(n, dtype=np.int32)
+        final = np.zeros(n, dtype=np.int32)
+        eng = self.engine
+        with eng._lock:
+            rc = eng.lib.wl_session_peek(eng.ctx, n, _lib.ptr(idx, C.c_int32), _lib.ptr(ids, C.c_int32), _lib.ptr(lens, C.c_int32),
+                                         _lib.ptr(score, C.c_float), _lib.ptr(nsp, C.c_float), _lib.ptr(step, C.c_int32),
+                                         _lib.ptr(final, C.c_int32))
+            _lib.check(eng.lib, eng.ctx, rc, "wl_session_peek")
+        return [(ids[i, :max(0, int(lens[i]))].tolist(), float(score[i]), float(nsp[i]), int(step[i]), bool(final[i]))
+                for i in range(n)]
+
+    def cancel(self, indices: Sequence[int]) -> None:
+        """Take running or finished-but-uncollected streams out of the session; their indices are free at once."""
+        idx = np.asarray(list(indices), dtype=np.int32)
+        if len(idx) == 0:
+            return
+        eng = self.engine
+        with eng._lock:
+            rc = eng.lib.wl_session_cancel(eng.ctx, len(idx), _lib.ptr(idx, C.c_int32))
+            _lib.check(eng.lib, eng.ctx, rc, "wl_session_cancel")
+        for i in idx.tolist():
+            self._held.pop(i, None)
+            self._nh.pop(i, None)
+        self._finished = [i for i in self._finished if i not in set(idx.tolist())]
+
     def close(self) -> None:
         if self.closed:
             return

@@ -159,6 +159,26 @@ class MultiDeviceSession:
     def result_of(self, entry: _PlacedEntry):
         return self.sessions[entry.device].result_of(entry.inner)
 
+    def _locate(self, handles: Sequence[int]) -> List[dict]:
+        """per device: local handle -> global handle of those of ``handles`` it holds"""
+        want = set(handles)
+        return [{lo: h for lo, h in hs.items() if h in want} for hs in self._handles]
+
+    def partials(self, handles: Sequence[int]) -> dict:
+        """``TranscribeSession.partials`` on the device that owns each handle (one peek per device)."""
+        out = {}
+        for g, loc in enumerate(self._locate(handles)):
+            if loc:
+                for lo, segs in self.sessions[g].partials(list(loc)).items():
+                    out[loc[lo]] = segs
+        return out
+
+    def cancel(self, handle: int) -> None:
+        for g, loc in enumerate(self._locate([handle])):
+            for lo in loc:
+                self.sessions[g].cancel(lo)
+                del self._handles[g][lo]
+
     def close(self) -> None:
         for s in self.sessions:
             if hasattr(s, "close"):

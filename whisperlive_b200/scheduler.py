@@ -14,7 +14,9 @@ the drop-in schema a client thread fills in and waits on); the control flow is d
   (``TranscribeSession.step_round`` over the engine's decode session, ``wl_session_*``): a late chunk is encoded,
   prefilled and joins the loop of the chunks that are already decoding a few token steps after it arrived, and the index
   of a finished stream is refilled immediately;
-* an engine error fails the streams it touched, never the scheduler (``TranscribeSession`` isolates them).
+* an engine error fails the streams it touched, never the scheduler (``TranscribeSession`` isolates them);
+* between step rounds the owner thread publishes interim segments for the requests that want them (one batched peek of
+  the decode session) and drops cancelled requests, freeing their decode index and encoder slots.
 
 ``linger_ms`` (default 0) optionally waits for more requests when the engine is idle and a single request arrived --
 the latency / batching trade the reference hard-codes as its 50 ms window.
@@ -33,10 +35,42 @@ import numpy as np
 log = logging.getLogger("whisperlive_b200.scheduler")
 
 
+class RequestCancelled(RuntimeError):
+    """The error a request's future carries after ``BatchRequest.cancel``."""
+
+
+class Partial:
+    """The latest interim segments of a request that wants them: ``version`` counts publications, ``event`` is set on
+    each one and when the request finishes (so a client can wait on it alone)."""
+
+    def __init__(self):
+        self._lock = threading.Lock()
+        self.segments: List[Any] = []
+        self.version = 0
+        self.ntok = 0
+        self.event = threading.Event()
+
+    def publish(self, segments: List[Any]) -> bool:
+        """Store ``segments`` as a new version when their token count differs from the last one's."""
+        ntok = sum(len(s.tokens) for s in segments)
+        with self._lock:
+            if ntok == self.ntok:
+                return False
+            self.segments, self.ntok, self.version = list(segments), ntok, self.version + 1
+        self.event.set()
+        return True
+
+    def latest(self):
+        """``(version, segments)``"""
+        with self._lock:
+            return self.version, list(self.segments)
+
+
 @dataclass
 class BatchRequest:
     """What a client thread submits and waits on (same fields as the reference's request record,
-    whisper_live/batch_inference.py:51-84, so ``ServeClient*`` code can fill either)."""
+    whisper_live/batch_inference.py:51-84, so ``ServeClient*`` code can fill either).  ``want_partials``: publish interim
+    segments in ``partial`` after each step round; ``cancel()``: nobody waits for the result any more."""
     audio: np.ndarray
     language: Optional[str] = None
     task: str = "transcribe"
@@ -52,6 +86,14 @@ class BatchRequest:
     error: Optional[Exception] = None
     submitted_at: float = 0.0
     finished_at: float = 0.0
+    want_partials: bool = False
+    partial: Partial = field(default_factory=Partial)
+    cancelled: bool = False
+
+    def cancel(self) -> None:
+        """The scheduler drops this request at its next round boundary (its decode index and encoder slots go back) and
+        sets its future with ``RequestCancelled``; a request that already finished keeps its result."""
+        self.cancelled = True
 
     def kwargs(self) -> dict:
         return dict(language=self.language, task=self.task, initial_prompt=self.initial_prompt, vad_filter=self.use_vad,
@@ -129,6 +171,9 @@ class RoundScheduler:
                     return
             room = self.capacity - len(in_flight)
             new = self._take(room, block=not in_flight) if room > 0 else []
+            for r in [r for r in new if r.cancelled]:
+                new.remove(r)
+                self._finish(r, None, None, RequestCancelled("request cancelled before admission"))
             if new:
                 if in_flight:
                     self.admitted_mid_flight += len(new)
@@ -141,10 +186,12 @@ class RoundScheduler:
                     for r in new:
                         self._finish(r, None, None, e)
             self.max_in_flight = max(self.max_in_flight, len(in_flight))
+            self._drop_cancelled(session, in_flight)
             if not in_flight:
                 continue
+            step = self.step_tokens > 0 and hasattr(session, "step_round")
             try:
-                if self.step_tokens > 0 and hasattr(session, "step_round"):
+                if step:
                     session.step_round(self.step_tokens)
                 else:
                     session.round()
@@ -165,6 +212,31 @@ class RoundScheduler:
                     self._finish(r, segments, info, None)
                 except Exception as e:
                     self._finish(r, None, None, e)
+            if step:
+                self._publish_partials(session, in_flight)
+
+    def _drop_cancelled(self, session, in_flight: Dict[int, BatchRequest]) -> None:
+        """Take the cancelled requests out of the session (index and encoder slots back) and answer them."""
+        for h, r in [(h, r) for h, r in in_flight.items() if r.cancelled]:
+            del in_flight[h]
+            try:
+                session.cancel(h)
+            except Exception as e:          # the stream stays in the session; its result is dropped when it finishes
+                log.error("cancel failed: %s", e)
+            self._finish(r, None, None, RequestCancelled("request cancelled"))
+
+    def _publish_partials(self, session, in_flight: Dict[int, BatchRequest]) -> None:
+        """One batched ``partials`` call for the in-flight requests that want interim text (none: no peek at all)."""
+        want = [h for h, r in in_flight.items() if r.want_partials and not r.cancelled]
+        if not want or not hasattr(session, "partials"):
+            return
+        try:
+            got = session.partials(want)
+        except Exception as e:              # interim text is best effort: the final result is unaffected
+            log.error("partials failed: %s", e)
+            return
+        for h, segs in got.items():
+            in_flight[h].partial.publish(segs)
 
     def _finish(self, r: BatchRequest, segments, info, error) -> None:
         r.result = list(segments) if segments is not None else None
@@ -173,6 +245,7 @@ class RoundScheduler:
         r.finished_at = time.monotonic()
         self.streams_done += 1
         r.future.set()
+        r.partial.event.set()
 
 
 class _OneShotSession:
@@ -201,6 +274,10 @@ class _OneShotSession:
         except Exception as e:
             for h, _, _ in batch:
                 self._done.append(_Done(h, None, e))
+
+    def cancel(self, handle):
+        self._pending = [p for p in self._pending if p[0] != handle]
+        self._done = [d for d in self._done if d.handle != handle]
 
     def pop_finished(self):
         d, self._done = self._done, []

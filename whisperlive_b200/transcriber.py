@@ -27,7 +27,7 @@ import time
 import logging
 import os
 import zlib
-from dataclasses import asdict, dataclass, field
+from dataclasses import asdict, dataclass, field, replace
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
@@ -704,6 +704,64 @@ class TranscribeSession:
         if self._dsess is not None:
             self._dsess.close()
             self._dsess = None
+
+    # -- between two rounds: interim text, cancellation --------------------------------------------
+    def partials(self, handles: Sequence[int]) -> Dict[int, List[Segment]]:
+        """Interim segments of the streams ``handles`` (live entries only): the segments of the windows that already
+        settled, then the running window's tokens so far cut by ``_split_segments_by_timestamps`` -- ONE ``peek`` of the
+        decode session for all of them.  Only a rung-0 decode gives interim text: a window on a fallback rung shows
+        nothing more until it settles.  Interim segments carry no words (alignment runs once, at settle); VAD-clipped
+        streams get the mapping of their final result."""
+        m = self.m
+        want = set(handles)
+        live = [e for e in self.entries if e.handle in want and e.job is not None]
+        running = {id(e): idx for idx, e in self._running.items()}
+        ds = self._dsess
+        peek_on = [e for e in live if id(e) in running and e.job.temp_idx == 0] if ds is not None and hasattr(ds, "peek") else []
+        peeked = dict(zip((id(e) for e in peek_on), ds.peek([running[id(e)] for e in peek_on]))) if peek_on else {}
+        out: Dict[int, List[Segment]] = {}
+        for e in live:
+            j = e.job
+            # copies down to the words: restore_speech_timestamps below maps them in place, and result_of maps the
+            # stream's own segments and words once, when it finishes
+            segs = [replace(s, words=None if s.words is None else [replace(w) for w in s.words]) for s in j.segments]
+            if id(e) in peeked:
+                tokens, score, no_speech, _step, _final = peeked[id(e)]
+                n = len(tokens)
+                avg_logprob = score * (n ** j.opt.length_penalty) / (n + 1)
+                pieces, _seek, _single = m._split_segments_by_timestamps(
+                    tokenizer=j.tok, tokens=tokens, time_offset=j.time_offset, segment_size=j.segment_size,
+                    segment_duration=j.segment_duration, seek=j.seek)
+                cr = get_compression_ratio(j.tok.decode(tokens).strip()) if n else 0.0
+                for piece in pieces:
+                    text = j.tok.decode(piece["tokens"])
+                    if piece["start"] == piece["end"] or not text.strip():
+                        continue
+                    segs.append(Segment(id=len(segs) + 1, seek=j.seek, start=piece["start"], end=piece["end"], text=text,
+                                        tokens=piece["tokens"], avg_logprob=avg_logprob, compression_ratio=cr,
+                                        no_speech_prob=no_speech, words=None, temperature=j.temperature))
+            p = e.prepared
+            if p is not None and p.get("speech_chunks"):
+                segs = restore_speech_timestamps(segs, p["speech_chunks"], m.feature_extractor.sampling_rate, m._vad)
+            out[e.handle] = segs
+        return out
+
+    def cancel(self, handle: int) -> None:
+        """Drop a stream in any state: its decode-session index (if it is running) and its encoder slots are free when
+        this returns, and the session forgets it.  A handle it does not hold is ignored."""
+        e = next((x for x in self.entries if x.handle == handle), None)
+        if e is None:
+            return
+        idx = next((i for i, x in self._running.items() if x is e), None)
+        if idx is not None:
+            self._dsess.cancel([idx])
+            del self._running[idx]
+        if e.job is not None:
+            e.job.enc = None
+        if e.parent is not None:
+            e.parent.done_one()
+            e.parent = None
+        self.entries.remove(e)
 
     # -- the three parts of a round -----------------------------------------------------------------
     def _encode_pending(self) -> None:
