@@ -28,7 +28,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 5
+#define WL_ABI_VERSION 6
 
 typedef struct wl_ctx wl_ctx;
 
@@ -68,9 +68,24 @@ typedef struct wl_gen_opts {
                                         step per prompt token; the parity tests compare the two) */
 } wl_gen_opts;
 
+/* With WLB200_FUSE_POST=1 (a diagnostic switch, default off) wl_init refuses a second live context on a device: the
+ * fused kernels' grid barrier is not safe with two contexts decoding at once.
+ * A wl_init that fails frees whatever it had created; so does a wl_finalize_weights that fails (the tensors
+ * wl_load_tensor uploaded stay until wl_destroy).  A failed load leaves no device memory behind but the context's. */
 int wl_init(const wl_config* cfg, wl_ctx** out);
 void wl_destroy(wl_ctx* ctx);
-const char* wl_last_error(wl_ctx* ctx);   /* ctx may be NULL: last wl_init failure */
+const char* wl_last_error(wl_ctx* ctx);   /* ctx may be NULL: last wl_init / wl_mem_info failure */
+
+/* Device memory the context holds right now, in bytes, counted where the library allocates it: weights (the uploaded
+ * tensors and their fused copies), the encoder workspaces and slot pool, the self-attention caches, both decode
+ * states, an open session, the log-mel / prefill / align workspaces at their current grown size, and the weight-load
+ * staging buffer while a load runs.  Not counted: buffers a call frees before it returns, CUDA graph executables and
+ * the CUDA context of the process. */
+int wl_device_bytes(wl_ctx* ctx, int64_t* out);
+/* Free and total device memory of CUDA ordinal `device` (cudaMemGetInfo); needs no context, so a load can be checked
+ * before it starts.  The query runs on its own thread: the calling thread's current device is untouched, and no
+ * device other than `device` gets a CUDA context. */
+int wl_mem_info(int32_t device, int64_t* free_bytes, int64_t* total_bytes);
 
 /* Weights: float32 host tensors under HF WhisperForConditionalGeneration names
  * ("model.encoder.conv1.weight", ...), plus "mel_filters" [n_mels, 201]. */

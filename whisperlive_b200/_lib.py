@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 5
+ABI_VERSION = 6
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -52,6 +52,8 @@ SIGNATURES = {
     "wl_init": (C.c_int, [C.POINTER(WlConfig), C.POINTER(C.c_void_p)]),
     "wl_destroy": (None, [C.c_void_p]),
     "wl_last_error": (C.c_char_p, [C.c_void_p]),
+    "wl_device_bytes": (C.c_int, [C.c_void_p, c_i64p]),
+    "wl_mem_info": (C.c_int, [C.c_int32, c_i64p, c_i64p]),
     "wl_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
     "wl_finalize_weights": (C.c_int, [C.c_void_p]),
     "wl_mel": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p, c_i64p]),

@@ -8,10 +8,15 @@ signature :19-40, ``SINGLE_MODEL`` / ``BATCH_WORKER`` class attributes :15-17, `
 ``"backend": "faster_whisper"`` :123-131 (the stock client only collects transcripts for that backend
 name: whisper_live/client.py:182).
 
-Differences that are the point of the port: one engine per process shared by all clients, driven by a
+Differences that are the point of the port: one engine per model shared by all clients, driven by a
 single scheduler thread that batches the chunks of all live connections per decode step
 (whisperlive_b200.scheduler.StreamScheduler); no CPU device / compute-type probing -- construction
 fails loudly without the CUDA engine.
+
+``single_model=True`` (the constructor default): the first connection's model serves every connection, as the
+reference's ``SINGLE_MODEL``.  ``single_model=False`` (the reference server's default): each connection is served by the
+model it asked for, from a ``models.ModelRegistry`` shared by the process -- loaded once, kept resident while idle,
+evicted least recently used first when a new model needs the memory.
 """
 from __future__ import annotations
 
@@ -27,6 +32,7 @@ except Exception as _e:  # pragma: no cover
     ServeClientBase = None
     _IMPORT_ERROR = _e
 
+from .models import ModelRegistry, engine_footprint
 from .scheduler import BatchRequest, StreamScheduler
 
 if ServeClientBase is not None:
@@ -35,11 +41,13 @@ if ServeClientBase is not None:
         SINGLE_MODEL = None
         SINGLE_MODEL_LOCK = threading.Lock()
         BATCH_WORKER = None
+        REGISTRY = None          # models.ModelRegistry of the single_model=False connections (built on first use)
         MAX_STREAMS = 8          # streams batched per decode step on this GPU
         BATCH_WINDOW_MS = 20
         MODEL_FACTORY = None     # tests inject a callable(model_name) -> transcriber
         PARTIALS = os.environ.get("WLB200_PARTIALS", "0") == "1"   # interim text of the chunk in flight
         REQUEST_TIMEOUT_S = 30
+        MEMORY_RESERVE_BYTES = 1 << 30   # kept free beyond a new model's footprint (CUDA graphs, allocator rounding)
         WAIT_SLICE_S = 0.05      # how often a waiting client thread looks at exit / new interim text
 
         def __init__(self, websocket, task="transcribe", device=None, language=None, client_uid=None, model="small.en",
@@ -56,17 +64,26 @@ if ServeClientBase is not None:
             self.vad_parameters = vad_parameters or {"threshold": 0.5}
             self.hotwords = hotwords
             self.compute_type = "float16"
+            self.model_entry = None
+            self.registry = None
+            self.scheduler = None    # the registry entry's scheduler; kept after cleanup() so a chunk in flight finds it
             if self.model_size_or_path is None:
                 return
             try:
                 cls = ServeClientB200
-                with cls.SINGLE_MODEL_LOCK:
-                    if cls.SINGLE_MODEL is None:
-                        cls.SINGLE_MODEL = self.create_model()
-                        cls.BATCH_WORKER = StreamScheduler(cls.SINGLE_MODEL, max_batch_size=cls.MAX_STREAMS,
-                                                           batch_window_ms=cls.BATCH_WINDOW_MS)
-                        cls.BATCH_WORKER.start()
-                self.transcriber = cls.SINGLE_MODEL
+                if single_model:
+                    with cls.SINGLE_MODEL_LOCK:
+                        if cls.SINGLE_MODEL is None:
+                            cls.SINGLE_MODEL = self.create_model()
+                            cls.BATCH_WORKER = StreamScheduler(cls.SINGLE_MODEL, max_batch_size=cls.MAX_STREAMS,
+                                                               batch_window_ms=cls.BATCH_WINDOW_MS)
+                            cls.BATCH_WORKER.start()
+                    self.transcriber = cls.SINGLE_MODEL
+                else:
+                    self.registry = cls.model_registry()
+                    self.model_entry = self.registry.acquire(self.model_size_or_path)
+                    self.transcriber = self.model_entry.transcriber
+                    self.scheduler = self.model_entry.scheduler
             except Exception as e:
                 logging.error(f"Failed to load model: {e}")
                 self.websocket.send(json.dumps({"uid": self.client_uid, "status": "ERROR",
@@ -80,16 +97,48 @@ if ServeClientBase is not None:
 
         def create_model(self):
             """Build the shared transcriber (CUDA engine). Raises when no H100 / library is available."""
+            return ServeClientB200.build_model(self.model_size_or_path, self.compute_type)
+
+        @staticmethod
+        def build_model(model_size_or_path, compute_type="float16"):
             if ServeClientB200.MODEL_FACTORY is not None:
-                return ServeClientB200.MODEL_FACTORY(self.model_size_or_path)
+                return ServeClientB200.MODEL_FACTORY(model_size_or_path)
             from .parallel import MultiDeviceWhisperModel, devices_from_env
             from .transcriber import B200WhisperModel
             devices = devices_from_env()     # WLB200_DEVICES=0,1,...: one engine context per GPU, streams placed i mod G
             if len(devices) > 1:
-                return MultiDeviceWhisperModel(self.model_size_or_path, device_index=devices, device="cuda",
-                                               compute_type=self.compute_type, max_streams=ServeClientB200.MAX_STREAMS)
-            return B200WhisperModel(self.model_size_or_path, device="cuda", device_index=devices[0],
-                                    compute_type=self.compute_type, max_streams=ServeClientB200.MAX_STREAMS)
+                return MultiDeviceWhisperModel(model_size_or_path, device_index=devices, device="cuda",
+                                               compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS)
+            return B200WhisperModel(model_size_or_path, device="cuda", device_index=devices[0],
+                                    compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS)
+
+        @classmethod
+        def model_registry(cls) -> ModelRegistry:
+            """The process's registry of per-connection models.  With the CUDA engine an entry is keyed by the checkpoint
+            directory a name resolves to (``weights.resolve_model_dir``, local snapshots only, as ``B200WhisperModel``
+            loads them) and a load is checked against the free memory of every configured device; a ``MODEL_FACTORY``
+            model is keyed by its name and loaded without a check."""
+            with cls.SINGLE_MODEL_LOCK:
+                if cls.REGISTRY is None:
+                    kw = {}
+                    if cls.MODEL_FACTORY is None:
+                        from .parallel import devices_from_env
+                        from .weights import resolve_model_dir
+                        resolve = lambda name: resolve_model_dir(name, local_files_only=True)
+                        kw = dict(resolve=resolve, devices=devices_from_env(), reserve_bytes=cls.MEMORY_RESERVE_BYTES,
+                                  footprint=lambda name: engine_footprint(name, cls.MAX_STREAMS, resolve=resolve))
+                    cls.REGISTRY = ModelRegistry(cls.build_model, max_streams=cls.MAX_STREAMS,
+                                                 batch_window_ms=cls.BATCH_WINDOW_MS, **kw)
+                return cls.REGISTRY
+
+        def cleanup(self):
+            """The connection ended (the server calls this on disconnect): its model loses a connection, then the
+            reference's cleanup stops the transcription thread.  A chunk the thread submits in between still goes to
+            this model's scheduler (``self.scheduler`` stays set) and is cancelled once ``exit`` is set."""
+            entry, self.model_entry = getattr(self, "model_entry", None), None
+            if entry is not None:
+                self.registry.release(entry)
+            super().cleanup()
 
         def set_language(self, info):
             if info.language_probability > 0.5:
@@ -106,7 +155,8 @@ if ServeClientBase is not None:
                                    vad_parameters=self.vad_parameters if self.use_vad else None,
                                    word_timestamps=self.word_timestamps, client_uid=self.client_uid, hotwords=self.hotwords,
                                    want_partials=self.PARTIALS)
-            ServeClientB200.BATCH_WORKER.submit(request)
+            worker = self.scheduler if self.registry is not None else ServeClientB200.BATCH_WORKER
+            worker.submit(request)
             duration = input_sample.shape[0] / self.RATE
             deadline = time.monotonic() + self.REQUEST_TIMEOUT_S
             sent = 0
@@ -160,6 +210,9 @@ if ServeClientBase is not None:
                 cls.BATCH_WORKER.stop()
             cls.BATCH_WORKER = None
             cls.SINGLE_MODEL = None
+            if cls.REGISTRY is not None:
+                cls.REGISTRY.shutdown()
+            cls.REGISTRY = None
 
 else:
 

@@ -60,6 +60,11 @@ _TABLE = {
     "large-v3": (1280, 20, 32, 32, 128, 51866),
     "large-v3-turbo": (1280, 20, 32, 4, 128, 51866),
     "turbo": (1280, 20, 32, 4, 128, 51866),
+    # distilled checkpoints: the teacher's encoder, two decoder layers
+    "distil-small.en": (768, 12, 12, 2, 80, 51864),
+    "distil-medium.en": (1024, 16, 24, 2, 80, 51864),
+    "distil-large-v2": (1280, 20, 32, 2, 80, 51865),
+    "distil-large-v3": (1280, 20, 32, 2, 128, 51866),
 }
 
 

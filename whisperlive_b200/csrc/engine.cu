@@ -5,7 +5,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
+#include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "../../include/wlb200.h"
@@ -28,6 +30,17 @@ void search_tl_bind(unsigned long long* p);
 }  // namespace wl
 
 static std::string g_init_error;
+
+// WLB200_FUSE_POST=1 (default off) fuses the split-K consumers into the producing GEMM behind a grid barrier that
+// needs every CTA of the grid resident at once.  Two contexts decoding at the same time on one device (two models of
+// one process) could each be partly resident and wait on each other, so with it on wl_init refuses a second context
+// on a device: g_live counts the contexts alive per device.
+static bool fuse_post_env() {
+  static const bool on = [] { const char* e = getenv("WLB200_FUSE_POST"); return e ? atoi(e) != 0 : false; }();
+  return on;
+}
+static std::mutex g_live_mu;
+static std::map<int, int> g_live;
 
 struct EncLayer {
   __half *w_qk, *w_v, *w_o, *w_fc1, *w_fc2;
@@ -65,7 +78,11 @@ struct wl_ctx {
   int num_sms = 132;
   int d, H, Le, Ld, n_mels, V, Vld, Bm, Km, Rm, NS;
   bool finalized = false;
-  std::vector<void*> allocs;
+  bool counted_live = false;   // counted in g_live (a wl_init that succeeded)
+  // every device buffer the context holds and its size in bytes (dalloc); dev_bytes is their sum plus the weight-load
+  // staging buffer while it exists -- what wl_device_bytes reports
+  std::vector<std::pair<void*, size_t>> allocs;
+  int64_t dev_bytes = 0;
   std::map<std::string, void*> dev;                 // raw uploaded tensors (fp16 for ndim>=2, f32 for 1-D)
   std::map<std::string, std::vector<int64_t>> shape;
   long graph_launched = 0;   // kernels executed through graph replays
@@ -179,15 +196,57 @@ struct wl_ctx {
 template <class T>
 static T* dalloc(wl_ctx* c, size_t n, bool zero = true) {
   void* p = nullptr;
-  cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
+  const size_t bytes = std::max<size_t>(n, 1) * sizeof(T);
+  cudaError_t e = cudaMalloc(&p, bytes);
   if (e != cudaSuccess) {
+    cudaGetLastError();   // an out-of-memory cudaMalloc is not sticky: leave no error behind for the next call
     char b[256];
     snprintf(b, sizeof(b), "cudaMalloc of %.1f MB failed: %s", n * sizeof(T) / 1048576.0, cudaGetErrorString(e));
     throw wl::Error{WL_ERR_NOMEM, b};
   }
-  c->allocs.push_back(p);
-  if (zero) WL_CUDA(cudaMemset(p, 0, std::max<size_t>(n, 1) * sizeof(T)));
+  c->allocs.push_back({p, bytes});
+  c->dev_bytes += (int64_t)bytes;
+  if (zero) WL_CUDA(cudaMemset(p, 0, bytes));
   return (T*)p;
+}
+
+// Frees the buffers dalloc made after the first `mark` ones (a wl_finalize_weights that failed part-way) and the
+// weight-load staging buffer.
+static void free_allocs_from(wl_ctx* c, size_t mark) {
+  if (c->allocs.size() > mark || c->stage_f32) cudaDeviceSynchronize();
+  while (c->allocs.size() > mark) {
+    cudaFree(c->allocs.back().first);
+    c->dev_bytes -= (int64_t)c->allocs.back().second;
+    c->allocs.pop_back();
+  }
+  if (c->stage_f32) {
+    cudaFree(c->stage_f32);
+    c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
+    c->stage_f32 = nullptr;
+    c->stage_cap = 0;
+  }
+}
+
+// Everything a context owns on the device and the host, and the context itself: wl_destroy, and wl_init when it
+// fails part-way.
+static void free_ctx(wl_ctx* c) {
+  if (c->st || !c->allocs.empty()) cudaSetDevice(c->cfg.device);
+  if (c->st) cudaStreamSynchronize(c->st);
+  for (auto& g : c->graphs)
+    if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
+  free_allocs_from(c, 0);
+  if (c->h_int) cudaFreeHost(c->h_int);
+  if (c->h_flt) cudaFreeHost(c->h_flt);
+  if (c->ev0) cudaEventDestroy(c->ev0);
+  if (c->ev1) cudaEventDestroy(c->ev1);
+  if (c->pev0) cudaEventDestroy(c->pev0);
+  if (c->pev1) cudaEventDestroy(c->pev1);
+  if (c->st) cudaStreamDestroy(c->st);
+  if (c->counted_live) {
+    std::lock_guard<std::mutex> g(g_live_mu);
+    --g_live[c->cfg.device];
+  }
+  delete c;
 }
 
 static void ensure_host(wl_ctx* c, size_t n_int, size_t n_flt) {
@@ -264,17 +323,28 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     if (const char* tl = getenv("WLB200_TIMELINE")) {
       c->tl_path = tl;
       WL_CUDA(cudaMalloc((void**)&c->tl_dev, (size_t)(TL_CAP + 1) * 8));
+      c->allocs.push_back({c->tl_dev, (size_t)(TL_CAP + 1) * 8});
+      c->dev_bytes += (int64_t)(TL_CAP + 1) * 8;
       WL_CUDA(cudaMemset(c->tl_dev, 0, (size_t)(TL_CAP + 1) * 8));
-      c->allocs.push_back(c->tl_dev);
       gemm_tl_bind(c->tl_dev); dec_gemm_tl_bind(c->tl_dev); wgemm_tl_bind(c->tl_dev); attention_tl_bind(c->tl_dev); elementwise_tl_bind(c->tl_dev); search_tl_bind(c->tl_dev);
     }
     c->enc.resize(c->Le);
     c->dec.resize(c->Ld);
     for (int i = c->NS - 1; i >= 0; --i) c->slot_free.push_back(i);
     c->slot_used.assign(c->NS, 0);
+    {
+      std::lock_guard<std::mutex> g(g_live_mu);
+      int& live = g_live[cfg->device];
+      WL_CHECK(!(fuse_post_env() && live > 0), WL_ERR_STATE,
+               "WLB200_FUSE_POST=1 allows one engine context per device (its grid barrier needs every CTA resident, "
+               "which two contexts decoding at once on device %d cannot guarantee); %d already exist", cfg->device, live);
+      ++live;
+      c->counted_live = true;
+    }
   } catch (const wl::Error& e) {
+    // a failed init frees the stream, the events and the timeline buffer it had made: nothing stays on the device
     g_init_error = e.msg;
-    delete c;
+    free_ctx(c);
     return e.code;
   }
   *out = c;
@@ -283,20 +353,35 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
 
 extern "C" void wl_destroy(wl_ctx* c) {
   if (!c) return;
-  cudaSetDevice(c->cfg.device);
-  cudaStreamSynchronize(c->st);
-  for (auto& g : c->graphs)
-    if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
-  for (void* p : c->allocs) cudaFree(p);
-  if (c->stage_f32) cudaFree(c->stage_f32);
-  if (c->h_int) cudaFreeHost(c->h_int);
-  if (c->h_flt) cudaFreeHost(c->h_flt);
-  if (c->ev0) cudaEventDestroy(c->ev0);
-  if (c->ev1) cudaEventDestroy(c->ev1);
-  if (c->pev0) cudaEventDestroy(c->pev0);
-  if (c->pev1) cudaEventDestroy(c->pev1);
-  if (c->st) cudaStreamDestroy(c->st);
-  delete c;
+  free_ctx(c);
+}
+
+extern "C" int wl_device_bytes(wl_ctx* c, int64_t* out) {
+  if (!c || !out) return WL_ERR_ARG;
+  *out = c->dev_bytes;
+  return WL_OK;
+}
+
+// The query runs on a thread of its own, so the caller's current device is never touched: restoring it with
+// cudaSetDevice would create a context on a device the caller never used (cudaGetDevice reports 0 on a fresh thread).
+// Only the queried device's primary context is initialised -- the device a model is about to be loaded on.
+extern "C" int wl_mem_info(int32_t device, int64_t* free_out, int64_t* total_out) {
+  if (!free_out || !total_out) return WL_ERR_ARG;
+  size_t fr = 0, tot = 0;
+  cudaError_t e = cudaSuccess;
+  std::thread q([&] {
+    e = cudaSetDevice(device);
+    if (e == cudaSuccess) e = cudaMemGetInfo(&fr, &tot);
+    if (e != cudaSuccess) cudaGetLastError();
+  });
+  q.join();
+  if (e != cudaSuccess) {
+    g_init_error = std::string("wl_mem_info(") + std::to_string(device) + "): " + cudaGetErrorString(e);
+    return WL_ERR_CUDA;
+  }
+  *free_out = (int64_t)fr;
+  *total_out = (int64_t)tot;
+  return WL_OK;
 }
 
 extern "C" const char* wl_last_error(wl_ctx* c) { return c ? c->err.c_str() : g_init_error.c_str(); }
@@ -342,10 +427,12 @@ extern "C" int wl_load_tensor(wl_ctx* c, const char* name, const float* data, co
     // is 1.5 G values; converting them on one host thread took longer than everything else in wl_init together.
     if (n > c->stage_cap) {
       if (c->stage_f32) cudaFree(c->stage_f32);
+      c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
       c->stage_f32 = nullptr;
       c->stage_cap = 0;
       WL_CUDA(cudaMalloc((void**)&c->stage_f32, n * sizeof(float)));
       c->stage_cap = n;
+      c->dev_bytes += (int64_t)(n * sizeof(float));
     }
     WL_CUDA(cudaMemcpyAsync(c->stage_f32, data, n * sizeof(float), cudaMemcpyHostToDevice, c->st));
     __half* p = dalloc<__half>(c, n, false);
@@ -423,9 +510,24 @@ static void build_mel_tables(wl_ctx* c) {
   c->mel_ooff = dalloc<long>(c, c->Bm + 1);
 }
 
+static void finalize_impl(wl_ctx* c);
+
+// A finalize that fails part-way (a missing tensor, an out-of-memory workspace) frees every buffer it had allocated and
+// the staging buffer before it returns: only the tensors wl_load_tensor uploaded remain, until wl_destroy.
 extern "C" int wl_finalize_weights(wl_ctx* c) {
   API_BEGIN(c)
   WL_CHECK(!c->finalized, WL_ERR_STATE, "weights already finalized");
+  const size_t mark = c->allocs.size();
+  try {
+    finalize_impl(c);
+  } catch (...) {
+    free_allocs_from(c, mark);
+    throw;
+  }
+  API_END(c)
+}
+
+static void finalize_impl(wl_ctx* c) {
   const int64_t d = c->d, ff = 4 * c->d, nm = c->n_mels, V = c->V;
   const size_t dd = (size_t)d * d;
   const std::string E = "model.encoder.", D = "model.decoder.";
@@ -489,7 +591,12 @@ extern "C" int wl_finalize_weights(wl_ctx* c) {
     L.ln3_b = (float*)need(c, p + "final_layer_norm.bias", {d});
   }
   build_mel_tables(c);
-  if (c->stage_f32) { cudaFree(c->stage_f32); c->stage_f32 = nullptr; c->stage_cap = 0; }
+  if (c->stage_f32) {
+    cudaFree(c->stage_f32);
+    c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
+    c->stage_f32 = nullptr;
+    c->stage_cap = 0;
+  }
 
   // ---- encoder workspaces (EB streams per pass, AB streams per attention sub-pass)
   const int H = c->H;
@@ -539,7 +646,6 @@ extern "C" int wl_finalize_weights(wl_ctx* c) {
   alloc_decode_state(c, c->ds);
   WL_CUDA(cudaDeviceSynchronize());
   c->finalized = true;
-  API_END(c)
 }
 
 // ------------------------------------------------------------------------------------------ K1 mel
@@ -869,7 +975,7 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
   // the producing split-K GEMM behind a grid barrier (13 -> 9 launches per layer).  The barrier gates every CTA on the
   // slowest one and the row work then runs on fewer CTAs than the separate kernels chained by programmatic dependent
   // launch get.
-  static const bool fuse_env = [] { const char* e = getenv("WLB200_FUSE_POST"); return e ? atoi(e) != 0 : false; }();
+  static const bool fuse_env = fuse_post_env();
   static const bool simt_env = [] { const char* e = getenv("WLB200_GEMM_SIMT"); return e && atoi(e) != 0; }();
   const bool fuse = fuse_env && splitk && !simt_env;
   struct Post { int kind = GEMM_POST_NONE; const float* g = nullptr; const float* b = nullptr; };

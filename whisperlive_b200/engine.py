@@ -9,6 +9,7 @@ libwlb200.so through the C ABI (include/wlb200.h); numpy arrays are only the hos
 from __future__ import annotations
 
 import ctypes as C
+import os
 import threading
 import weakref
 from dataclasses import dataclass, field
@@ -97,6 +98,67 @@ class EncoderOutput:
         return out.astype(dtype) if dtype is not None else out
 
 
+def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
+                       n_align_heads: Optional[int] = None) -> int:
+    """Device bytes a context of these shapes allocates through ``wl_init``, the weight load and one open decode session
+    (csrc/engine.cu: ``wl_load_tensor``, ``finalize_impl``, ``alloc_decode_state``, ``wl_session_open``), plus the
+    workspaces its first step round grows: the log-mel of ``max_streams`` 30-second chunks (``wl_mel``) and the batched
+    prefill at its first size of 1024 rows (``prefill_reserve``).  What a model registry compares with the free memory
+    before a load.  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
+    chunks, more prompt rows, the word-alignment buffers) and the allocator's rounding."""
+    B, K = int(max_streams), int(max_beam)
+    NS = int(enc_slots) if enc_slots is not None else 2 * B
+    d, H, Le, Ld, nm, V = dims.d_model, dims.n_heads, dims.enc_layers, dims.dec_layers, dims.n_mels, dims.vocab
+    ff, dd, S, S_PAD, T = 4 * d, d * d, 1500, 1536, T_MAX
+    MAX_HYPS, MAX_CAND, MAX_ROWS, PEEK_STRIDE = 16, 16, 8, 8 + 2 * 16 + T_MAX
+    if n_align_heads is None:
+        n_align_heads = len(dims.default_alignment_heads())
+    f32 = i32 = 4
+    f16 = 2
+    # weights as uploaded: fp16 for matrices, fp32 for vectors, the encoder position table and the mel filters
+    enc_layer = 4 * dd * f16 + 3 * d * f32 + 2 * d * f32 + 2 * ff * d * f16 + (ff + d) * f32 + 2 * d * f32
+    dec_layer = 8 * dd * f16 + 6 * d * f32 + 3 * 2 * d * f32 + 2 * ff * d * f16 + (ff + d) * f32
+    weights = (d * nm * 3 * f16 + d * f32 + d * d * 3 * f16 + d * f32 + S * d * f32 + Le * enc_layer + 2 * d * f32
+               + V * d * f16 + T * d * f16 + Ld * dec_layer + 2 * d * f32 + nm * 201 * f32)
+    # fused copies finalize makes: encoder Q|K, decoder Q|K|V (weights and biases)
+    fused = Le * (2 * dd * f16 + 2 * d * f32) + Ld * (3 * dd * f16 + 3 * d * f32)
+    mel_tables = (400 + 800) * f32 + 2 * nm * i32 + B * 4 + 4 * (B + 1) * 8 + B * i32 + 3 * B * i32
+    EB = min(B, max(1, int(os.environ.get("WLB200_ENC_BATCH") or 16)))
+    AB = min(EB, 2 if d >= 1024 else 4)
+    M = EB * S
+    encoder = (B * nm * 3000 * f32 + (EB * 3002 * nm + 4096) * f16 + (EB * 3002 * d + 4096) * f16 + M * d * f32
+               + M * d * f16 + M * 2 * d * f16 + EB * d * S_PAD * f16 + AB * H * S * S_PAD * (f32 + f16) + M * d * f16
+               + M * ff * f16 + B * i32)
+    pool = NS * S * d * f16 + Ld * 2 * NS * S * d * f16
+    R = B * K
+    Rp = (R + 15) // 16 * 16
+    mask = ((V + 31) // 32 + 1) * 4
+    caches = 2 * Ld * R * H * T * 64 * f16
+    decoder = (R * d * f32 + (R * 16 * d + R * 4 * ff) * f32 + R * 16 * d * f32 + R * ((V + 3) // 4 * 4) * f32
+               + 2 * Rp * d * f16 + Rp * ff * f16 + caches + B * H * 12 * MAX_ROWS * 66 * f32 + 2 * 4 + mask
+               + (2 * n_align_heads * i32 if n_align_heads else 0))
+    state = (8 * R * 4 + R * T * i32 + R * T * 2 + 2 * R * MAX_CAND * 4 + 22 * B * 4 + B * T * i32
+             + 2 * B * MAX_HYPS * 4 + B * MAX_HYPS * T * i32 + B * T * f32 + 4 * 4)
+    session = state + caches + mask + B * i32 + B * PEEK_STRIDE * i32
+    pcm = B * 30 * 16000
+    frames = B * (30 * 16000 // 160 + 1) * nm
+    mel = (pcm + pcm // 4) * f32 + (frames + frames // 4) * f32
+    cap = 1024
+    prefill = (4 * cap * i32 + 2 * (cap // 8 + 128) * i32 + (3 * R + 16) * i32 + cap * T * 2 + 5 * cap * d * f32
+               + 2 * cap * d * f16 + cap * ff * f16 + 128 * H * 12 * MAX_ROWS * 66 * f32)
+    return int(weights + fused + mel_tables + encoder + pool + decoder + state + session + mel + prefill)
+
+
+def mem_info(device: int = 0) -> Tuple[int, int]:
+    """``(free, total)`` device memory of CUDA ordinal ``device`` in bytes (``wl_mem_info``; no context needed)."""
+    lib = _lib.load()
+    free, total = C.c_int64(0), C.c_int64(0)
+    rc = lib.wl_mem_info(int(device), C.byref(free), C.byref(total))
+    if rc != 0:
+        raise _lib.WlError(f"wl_mem_info failed ({rc}): {lib.wl_last_error(None).decode()}")
+    return int(free.value), int(total.value)
+
+
 class B200Whisper:
     def __init__(self, dims: WhisperDims, weights: Dict[str, "np.ndarray"], device_index: Union[int, List[int]] = 0,
                  compute_type: str = "float16", max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
@@ -136,7 +198,11 @@ class B200Whisper:
             raise _lib.WlError(f"wl_init failed ({rc}): {self.lib.wl_last_error(None).decode()}")
         self.ctx = ctx
         self._fin = weakref.finalize(self, self.lib.wl_destroy, ctx)
-        self._load_weights(weights)
+        try:
+            self._load_weights(weights)
+        except BaseException:
+            self._fin()      # a failed load gives its device memory back now, not when the traceback is collected
+            raise
 
     # ------------------------------------------------------------------ construction
     @classmethod
@@ -207,6 +273,22 @@ class B200Whisper:
 
     def kernel_launches(self) -> int:
         return int(self.lib.wl_kernel_launches(self.ctx))
+
+    @property
+    def device_bytes(self) -> int:
+        """Device memory this context holds right now (``wl_device_bytes``): weights, workspaces, slot pool, caches,
+        decode states and the workspaces grown so far; 0 once the context is destroyed."""
+        out = C.c_int64(0)
+        with self._lock:     # destroy() frees the context under the same lock
+            if not self._fin.alive:
+                return 0
+            _lib.check(self.lib, self.ctx, self.lib.wl_device_bytes(self.ctx, C.byref(out)), "wl_device_bytes")
+        return int(out.value)
+
+    def destroy(self) -> None:
+        """Free the context and all its device memory now (idempotent); the engine is unusable afterwards."""
+        with self._lock:
+            self._fin()
 
     def last_device_ms(self, which: int) -> float:
         return float(self.lib.wl_last_device_ms(self.ctx, which))

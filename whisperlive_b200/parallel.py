@@ -27,7 +27,7 @@ from __future__ import annotations
 
 import concurrent.futures as cf
 import os
-from typing import Any, List, Optional, Sequence, Tuple
+from typing import Any, Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -86,6 +86,20 @@ class MultiDeviceWhisperModel:
 
     def close(self):
         self._pool.shutdown(wait=True)
+
+    @property
+    def device_bytes(self) -> Dict[int, int]:
+        """Device memory the engine contexts hold right now, summed per CUDA ordinal."""
+        out: Dict[int, int] = {}
+        for d, m in zip(self.device_index, self.models):
+            out[int(d)] = out.get(int(d), 0) + int(m.device_bytes)
+        return out
+
+    def destroy(self) -> None:
+        """Stop the worker threads and free every device's engine context now."""
+        self.close()
+        for m in self.models:
+            m.destroy()
 
 
 class _PlacedEntry:

@@ -975,6 +975,15 @@ class B200WhisperModel:
     def supported_languages(self) -> List[str]:
         return list(LANGUAGE_CODES) if self.model.is_multilingual else ["en"]
 
+    @property
+    def device_bytes(self) -> int:
+        """Device memory the engine context holds right now (``B200Whisper.device_bytes``)."""
+        return int(self.model.device_bytes)
+
+    def destroy(self) -> None:
+        """Free the engine context and its device memory now (a model registry evicting this model)."""
+        self.model.destroy()
+
     # -- Boundary B ---------------------------------------------------------------------------
     def transcribe(self, audio: np.ndarray, language: Optional[str] = None, task: str = "transcribe",
                    log_progress: bool = False, beam_size: int = 5, best_of: int = 5, patience: float = 1,

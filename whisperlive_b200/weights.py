@@ -124,15 +124,37 @@ def load_model_dir(path: str) -> Dict[str, torch.Tensor]:
     raise FileNotFoundError(f"{path}: neither model.safetensors nor model.bin")
 
 
+# Size name -> hub repository of its CTranslate2 conversion, for the sizes whose repository is not
+# ``Systran/faster-whisper-<size>``.  Like faster-whisper's ``utils._MODELS``, which this table is recalled from:
+# faster-whisper is not a dependency of this project, so the table was not read from it.
+HUB_REPOS = {
+    "distil-small.en": "Systran/faster-distil-whisper-small.en",
+    "distil-medium.en": "Systran/faster-distil-whisper-medium.en",
+    "distil-large-v2": "Systran/faster-distil-whisper-large-v2",
+    "distil-large-v3": "Systran/faster-distil-whisper-large-v3",
+    "large-v3-turbo": "mobiuslabsgmbh/faster-whisper-large-v3-turbo",
+    "turbo": "mobiuslabsgmbh/faster-whisper-large-v3-turbo",
+}
+
+
+def hub_repo(name: str) -> str:
+    """Hub repository a size name or hub id resolves to: a hub id (``owner/repo``) as given, a size in ``HUB_REPOS``
+    through the table, any other size as ``Systran/faster-whisper-<size>``."""
+    name = str(name)
+    if "/" in name:
+        return name
+    return HUB_REPOS.get(name, f"Systran/faster-whisper-{name}")
+
+
 def resolve_model_dir(model_size_or_path: str, download_root=None, local_files_only: bool = False) -> str:
     """Directory holding the checkpoint + tokenizer.json for a path, a size name or a hub id.
     Mirrors the reference's resolution order (faster_whisper_backend.py:133-178): local directory first,
-    then the hub snapshot of ``Systran/faster-whisper-<size>`` (CT2 format, what ``download_model`` fetches).
+    then the hub snapshot of ``hub_repo(size)`` (CT2 format, what ``download_model`` fetches).
     Raises FileNotFoundError with the reason instead of falling back to anything."""
     if isinstance(model_size_or_path, str) and os.path.isdir(model_size_or_path):
         return model_size_or_path
     name = str(model_size_or_path)
-    repo = name if "/" in name else f"Systran/faster-whisper-{name}"
+    repo = hub_repo(name)
     try:
         import huggingface_hub
     except Exception as e:
