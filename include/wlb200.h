@@ -235,6 +235,23 @@ int wl_test_self_attn(wl_ctx* ctx, const float* qkv_part, const float* qkv_bias,
  * mode 1, gelu_cast: y = gelu(bias + the nsplit (1..8) partials); x, gamma, beta unused.  y: the fp16 result as float. */
 int wl_test_fold(wl_ctx* ctx, int32_t mode, float* x, const float* part, int32_t nsplit, const float* bias,
                  const float* gamma, const float* beta, float* y, int32_t rows, int32_t cols);
+/* Test hooks of the encoder-pass kernels.  Each runs the code the encoder pass runs, on device copies of the inputs.
+ *
+ * Encoder self-attention of nb streams, H heads (d = 64 H).  qk: fp16 [nb][1500][2d], Q | K as the QK GEMM writes it;
+ * vt: fp16 [nb][d][1536], V transposed per head, the 36 pad columns taken as given.  out: fp16 [nb * 1500 + 128][d],
+ * uploaded as the caller filled it and copied back whole (128 guard rows after the last stream).  path 0: the fused
+ * flash-attention kernel; path 1: the unfused scores GEMM + softmax_rows + P V GEMM in sub-passes of ab streams
+ * (ab = 0: the engine's rule, 2 streams for d >= 1024, else 4). */
+int wl_test_enc_attn(wl_ctx* ctx, const uint16_t* qk_f16, const uint16_t* vt_f16, uint16_t* out_f16, int32_t nb, int32_t H,
+                     int32_t path, int32_t ab);
+/* The conv stem with the loaded conv weights, biases and positional table: feats [nb][n_mels][3000] f32 -> x_out
+ * [nb][1500][d] f32, the residual stream after conv2 + GELU + positions. */
+int wl_test_enc_stem(wl_ctx* ctx, const float* feats_f32, float* x_out_f32, int32_t nb);
+/* layernorm_rows over x [rows][d] (d a multiple of 4, at most 1280).  y16_as_f32 (the fp16 output as float) and y32
+ * (the fp32 output), either may be NULL: [rows + 8][d], uploaded as the caller filled them (y16 rounded to fp16) and
+ * copied back whole, so the 8 guard rows after the last one show what the kernel wrote past it. */
+int wl_test_layernorm(wl_ctx* ctx, const float* x_f32, const float* gamma, const float* beta, float* y16_as_f32, float* y32,
+                      int32_t rows, int32_t d);
 /* device-resident timing of the GEMM kernel: C = A(MxK) * B(NxK)^T, `iters` launches between CUDA events;
  * bn = 0 picks the tile like the engine does. ms_out = average milliseconds per launch. */
 int wl_bench_gemm(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,

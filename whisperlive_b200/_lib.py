@@ -87,6 +87,9 @@ SIGNATURES = {
                                     c_i32p, c_i32p, c_i32p, C.c_int32, C.c_int32, C.c_float, c_f32p]),
     "wl_test_fold": (C.c_int, [C.c_void_p, C.c_int32, c_f32p, c_f32p, C.c_int32, c_f32p, c_f32p, c_f32p, c_f32p,
                                C.c_int32, C.c_int32]),
+    "wl_test_enc_attn": (C.c_int, [C.c_void_p, c_u16p, c_u16p, c_u16p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "wl_test_enc_stem": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int32]),
+    "wl_test_layernorm": (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_int32, C.c_int32]),
     "wl_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_f32p]),
     "wl_kernel_launches": (C.c_int64, [C.c_void_p]),
     "wl_last_device_ms": (C.c_float, [C.c_void_p, C.c_int32]),

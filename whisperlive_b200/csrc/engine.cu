@@ -512,6 +512,9 @@ static void build_mel_tables(wl_ctx* c) {
 
 static void finalize_impl(wl_ctx* c);
 
+// streams per sub-pass of the unfused encoder attention: the fp32 scores of one stream are H x 1500 x 1536 floats
+static int enc_attn_streams(int d) { return d >= 1024 ? 2 : 4; }
+
 // A finalize that fails part-way (a missing tensor, an out-of-memory workspace) frees every buffer it had allocated and
 // the staging buffer before it returns: only the tensors wl_load_tensor uploaded remain, until wl_destroy.
 extern "C" int wl_finalize_weights(wl_ctx* c) {
@@ -604,7 +607,7 @@ static void finalize_impl(wl_ctx* c) {
   // ~1 GB at large-v3, small next to 80 GB
   static const int enc_batch = [] { const char* e = getenv("WLB200_ENC_BATCH"); return e ? std::max(1, atoi(e)) : 16; }();
   c->EB = std::min(c->Bm, enc_batch);
-  c->AB = std::min(c->EB, d >= 1024 ? 2 : 4);
+  c->AB = std::min(c->EB, enc_attn_streams(d));
   const size_t M = (size_t)c->EB * S_ENC;
   c->feat32 = dalloc<float>(c, (size_t)c->Bm * nm * 3000);  // all streams of a call stay resident (wl_encode_resident)
   c->feat16 = dalloc<__half>(c, (size_t)c->EB * 3002 * nm + 4096);
@@ -785,22 +788,55 @@ static GemmOperand opnd(const __half* p, long rows, long k, long ld, int n1 = 1,
   return o;
 }
 
-static void encoder_pass(wl_ctx* c, int nb, const int* slots_host, const float* feat_dev) {
-  const int d = c->d, H = c->H, nm = c->n_mels, ff = 4 * c->d;
-  const long M = (long)nb * S_ENC;
-  cudaStream_t st = c->st;
-  prep_features(st, feat_dev, c->feat16, nb, nm);
+// The conv stem: features [nb][n_mels][3000] f32 -> x [nb][1500][d] f32 (conv1 + GELU, conv2 (stride 2) + GELU + the
+// positional table).  feat16 [nb][3002][n_mels] and conv1o [nb][3002][d] are workspaces whose rows 0 and 3001 of every
+// stream must be zero (the conv padding): nothing here writes them.
+static void encoder_stem(wl_ctx* c, cudaStream_t st, int nb, const float* feat_dev, __half* feat16, __half* conv1o, float* x) {
+  const int d = c->d, nm = c->n_mels;
+  prep_features(st, feat_dev, feat16, nb, nm);
   {  // conv1 + GELU -> conv1o rows 1..3000 (rows 0 / 3001 stay zero)
     GemmEpilogue e;
-    e.out = c->conv1o + d; e.out_f32 = 0; e.ldm = d; e.ldn = 1; e.ob1 = 3002L * d; e.bias = c->b_conv1; e.gelu = 1;
-    gemm_tn(st, opnd(c->feat16, 3000, 3 * nm, nm, nb, 3002L * nm), opnd(c->w_conv1, d, 3 * nm, 3 * nm), 3000, d, 3 * nm, e);
+    e.out = conv1o + d; e.out_f32 = 0; e.ldm = d; e.ldn = 1; e.ob1 = 3002L * d; e.bias = c->b_conv1; e.gelu = 1;
+    gemm_tn(st, opnd(feat16, 3000, 3 * nm, nm, nb, 3002L * nm), opnd(c->w_conv1, d, 3 * nm, 3 * nm), 3000, d, 3 * nm, e);
   }
   {  // conv2 (stride 2) + GELU + positional table -> residual stream x (f32)
     GemmEpilogue e;
-    e.out = c->x; e.out_f32 = 1; e.ldm = d; e.ldn = 1; e.ob1 = (long)S_ENC * d; e.bias = c->b_conv2; e.gelu = 1;
+    e.out = x; e.out_f32 = 1; e.ldm = d; e.ldn = 1; e.ob1 = (long)S_ENC * d; e.bias = c->b_conv2; e.gelu = 1;
     e.resid = c->pos_enc; e.rldm = d; e.rldn = 1; e.rb1 = 0;
-    gemm_tn(st, opnd(c->conv1o, S_ENC, 3 * d, 2 * d, nb, 3002L * d), opnd(c->w_conv2, d, 3 * d, 3 * d), S_ENC, d, 3 * d, e);
+    gemm_tn(st, opnd(conv1o, S_ENC, 3 * d, 2 * d, nb, 3002L * d), opnd(c->w_conv2, d, 3 * d, 3 * d), S_ENC, d, 3 * d, e);
   }
+}
+
+// Encoder self-attention without the fused kernel (WLB200_FUSED_ATTN=0), AB streams at a time: the scores GEMM into
+// scores [AB][H][1500][S_PAD] f32, softmax_rows into probs16 (same shape, fp16, the pad columns written as 0), the P V
+// GEMM into attn.  qk [nb][1500][2d], vt [nb][d][S_PAD], attn [nb * 1500][d].
+static void encoder_attention_unfused(cudaStream_t st, const __half* qk, const __half* vt, __half* attn, float* scores,
+                                      __half* probs16, int nb, int H, int AB) {
+  const int d = H * 64;
+  for (int b0 = 0; b0 < nb; b0 += AB) {
+    const int ab = std::min(AB, nb - b0);
+    const __half* qb = qk + (long)b0 * S_ENC * 2 * d;
+    {
+      GemmEpilogue e;
+      e.out = scores; e.out_f32 = 1; e.ldm = S_PAD; e.ob1 = (long)S_ENC * S_PAD; e.ob2 = (long)H * S_ENC * S_PAD;
+      gemm_tn(st, opnd(qb, S_ENC, 64, 2 * d, H, 64, ab, (long)S_ENC * 2 * d),
+              opnd(qb + d, S_ENC, 64, 2 * d, H, 64, ab, (long)S_ENC * 2 * d), S_ENC, S_ENC, 64, e);
+    }
+    softmax_rows(st, scores, probs16, (long)ab * H * S_ENC, S_ENC, S_PAD, S_PAD, 0.125f);
+    {
+      GemmEpilogue e;
+      e.out = attn + (long)b0 * S_ENC * d; e.ldm = d; e.ob1 = 64; e.ob2 = (long)S_ENC * d;
+      gemm_tn(st, opnd(probs16, S_ENC, S_PAD, S_PAD, H, (long)S_ENC * S_PAD, ab, (long)H * S_ENC * S_PAD),
+              opnd(vt + (long)b0 * d * S_PAD, 64, S_PAD, S_PAD, H, 64L * S_PAD, ab, (long)d * S_PAD), S_ENC, 64, S_PAD, e);
+    }
+  }
+}
+
+static void encoder_pass(wl_ctx* c, int nb, const int* slots_host, const float* feat_dev) {
+  const int d = c->d, H = c->H, ff = 4 * c->d;
+  const long M = (long)nb * S_ENC;
+  cudaStream_t st = c->st;
+  encoder_stem(c, st, nb, feat_dev, c->feat16, c->conv1o, c->x);
   for (int l = 0; l < c->Le; ++l) {
     const EncLayer& L = c->enc[l];
     layernorm_rows(st, c->x, L.ln1_g, L.ln1_b, c->xn, nullptr, M, d);
@@ -816,23 +852,7 @@ static void encoder_pass(wl_ctx* c, int nb, const int* slots_host, const float* 
     }
     static const bool fused_attn = [] { const char* e = getenv("WLB200_FUSED_ATTN"); return e ? atoi(e) != 0 : true; }();
     if (fused_attn) encoder_attention_fused(st, c->qk, c->vt, c->attn, nb, H, d);
-    else for (int b0 = 0; b0 < nb; b0 += c->AB) {
-      const int ab = std::min(c->AB, nb - b0);
-      const __half* qb = c->qk + (long)b0 * S_ENC * 2 * d;
-      {
-        GemmEpilogue e;
-        e.out = c->scores; e.out_f32 = 1; e.ldm = S_PAD; e.ob1 = (long)S_ENC * S_PAD; e.ob2 = (long)H * S_ENC * S_PAD;
-        gemm_tn(st, opnd(qb, S_ENC, 64, 2 * d, H, 64, ab, (long)S_ENC * 2 * d),
-                opnd(qb + d, S_ENC, 64, 2 * d, H, 64, ab, (long)S_ENC * 2 * d), S_ENC, S_ENC, 64, e);
-      }
-      softmax_rows(st, c->scores, c->probs16, (long)ab * H * S_ENC, S_ENC, S_PAD, S_PAD, 0.125f);
-      {
-        GemmEpilogue e;
-        e.out = c->attn + (long)b0 * S_ENC * d; e.ldm = d; e.ob1 = 64; e.ob2 = (long)S_ENC * d;
-        gemm_tn(st, opnd(c->probs16, S_ENC, S_PAD, S_PAD, H, (long)S_ENC * S_PAD, ab, (long)H * S_ENC * S_PAD),
-                opnd(c->vt + (long)b0 * d * S_PAD, 64, S_PAD, S_PAD, H, 64L * S_PAD, ab, (long)d * S_PAD), S_ENC, 64, S_PAD, e);
-      }
-    }
+    else encoder_attention_unfused(st, c->qk, c->vt, c->attn, c->scores, c->probs16, nb, H, c->AB);
     {
       GemmEpilogue e;
       e.out = c->x; e.out_f32 = 1; e.ldm = d; e.bias = L.b_o; e.resid = c->x; e.rldm = d;
@@ -2385,6 +2405,84 @@ extern "C" int wl_test_fold(wl_ctx* c, int32_t mode, float* x, const float* part
   WL_CUDA(cudaStreamSynchronize(c->st));
   download_f16(dy, y, n);
   if (mode == 0) WL_CUDA(cudaMemcpy(x, dx, n * 4, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+// Test hooks of the encoder-pass kernels: each runs the code encoder_pass runs, on its own device copies of the inputs.
+extern "C" int wl_test_enc_attn(wl_ctx* c, const uint16_t* qk_f16, const uint16_t* vt_f16, uint16_t* out_f16, int32_t nb,
+                                int32_t H, int32_t path, int32_t ab) {
+  API_BEGIN(c)
+  WL_CHECK(qk_f16 && vt_f16 && out_f16 && nb >= 1 && H >= 1 && H <= 32 && (path == 0 || path == 1) && ab >= 0, WL_ERR_ARG,
+           "wl_test_enc_attn: bad arguments");
+  const int d = H * 64;
+  const size_t n_qk = (size_t)nb * S_ENC * 2 * d, n_vt = (size_t)nb * d * S_PAD, n_out = ((size_t)nb * S_ENC + 128) * d;
+  HookBufs hb;
+  const __half* dqk = hb.upload(reinterpret_cast<const __half*>(qk_f16), n_qk);
+  const __half* dvt = hb.upload(reinterpret_cast<const __half*>(vt_f16), n_vt);
+  __half* dout = hb.upload(reinterpret_cast<const __half*>(out_f16), n_out);
+  if (path == 0) {
+    WL_CUDA(cudaDeviceSynchronize());
+    encoder_attention_fused(c->st, dqk, dvt, dout, nb, H, d);
+  } else {
+    const int AB = ab ? ab : std::min(nb, enc_attn_streams(d));
+    float* scores = hb.alloc<float>((size_t)AB * H * S_ENC * S_PAD);
+    __half* probs16 = hb.alloc<__half>((size_t)AB * H * S_ENC * S_PAD);
+    // zeroed like the engine's workspaces: the scores GEMM never writes the pad columns, softmax_rows writes all of P
+    WL_CUDA(cudaMemset(scores, 0, (size_t)AB * H * S_ENC * S_PAD * 4));
+    WL_CUDA(cudaMemset(probs16, 0, (size_t)AB * H * S_ENC * S_PAD * 2));
+    WL_CUDA(cudaDeviceSynchronize());
+    encoder_attention_unfused(c->st, dqk, dvt, dout, scores, probs16, nb, H, AB);
+  }
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  WL_CUDA(cudaMemcpy(out_f16, dout, n_out * 2, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+extern "C" int wl_test_enc_stem(wl_ctx* c, const float* feats_f32, float* x_out_f32, int32_t nb) {
+  API_BEGIN(c)
+  WL_CHECK(c->finalized, WL_ERR_STATE, "weights not finalized");
+  WL_CHECK(feats_f32 && x_out_f32 && nb >= 1, WL_ERR_ARG, "wl_test_enc_stem: bad arguments");
+  const int d = c->d, nm = c->n_mels;
+  HookBufs hb;
+  const float* dfeat = hb.upload(feats_f32, (size_t)nb * nm * 3000);
+  // the engine's shapes, slack included; zeroed: rows 0 and 3001 of every stream are the conv padding
+  const size_t n16 = (size_t)nb * 3002 * nm + 4096, n1 = (size_t)nb * 3002 * d + 4096, nx = (size_t)nb * S_ENC * d;
+  __half* feat16 = hb.alloc<__half>(n16);
+  __half* conv1o = hb.alloc<__half>(n1);
+  float* x = hb.alloc<float>(nx);
+  WL_CUDA(cudaMemset(feat16, 0, n16 * 2));
+  WL_CUDA(cudaMemset(conv1o, 0, n1 * 2));
+  WL_CUDA(cudaMemset(x, 0xff, nx * 4));   // NaN: an element the stem did not write cannot pass as a value
+  WL_CUDA(cudaDeviceSynchronize());
+  encoder_stem(c, c->st, nb, dfeat, feat16, conv1o, x);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  WL_CUDA(cudaMemcpy(x_out_f32, x, nx * 4, cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
+extern "C" int wl_test_layernorm(wl_ctx* c, const float* x_f32, const float* gamma, const float* beta, float* y16_as_f32,
+                                 float* y32, int32_t rows, int32_t d) {
+  API_BEGIN(c)
+  WL_CHECK(x_f32 && gamma && beta && rows >= 1 && d >= 4, WL_ERR_ARG, "wl_test_layernorm: bad arguments");
+  // the outputs carry 8 guard rows after the last one: the grid covers whole blocks of 8 rows
+  const size_t n = (size_t)rows * d, ng = (size_t)(rows + 8) * d;
+  HookBufs hb;
+  const float* dx = hb.upload(x_f32, n);
+  const float* dg = hb.upload(gamma, d);
+  const float* db = hb.upload(beta, d);
+  __half* dy = nullptr;
+  float* dy32 = nullptr;
+  if (y16_as_f32) {
+    std::vector<__half> h(ng);
+    for (size_t i = 0; i < ng; ++i) h[i] = __float2half_rn(y16_as_f32[i]);
+    dy = hb.upload(h.data(), ng);
+  }
+  if (y32) dy32 = hb.upload(y32, ng);
+  WL_CUDA(cudaDeviceSynchronize());
+  layernorm_rows(c->st, dx, dg, db, dy, dy32, rows, d);
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  if (y16_as_f32) download_f16(dy, y16_as_f32, ng);
+  if (y32) WL_CUDA(cudaMemcpy(y32, dy32, ng * 4, cudaMemcpyDeviceToHost));
   API_END(c)
 }
 

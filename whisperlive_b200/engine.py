@@ -669,6 +669,52 @@ class B200Whisper:
                                        fp(beta), fp(y), rows, cols)
             _lib.check(self.lib, self.ctx, rc, "wl_test_fold")
 
+    def test_enc_attn(self, qk: np.ndarray, vt: np.ndarray, out: np.ndarray, path: int, ab: int = 0) -> np.ndarray:
+        """Encoder self-attention (wl_test_enc_attn).  qk fp16 [nb, 1500, 2*H*64] (Q | K); vt fp16 [nb, H*64, 1536] (V^T
+        per head, pad columns as given); out fp16 [nb*1500 + 128, H*64], the buffer as it is before the launch.  path 0:
+        the fused kernel; 1: the unfused sequence in sub-passes of ``ab`` streams (0: the engine's rule).  Returns the
+        whole output buffer after the launch, guard rows included."""
+        qk16 = np.ascontiguousarray(qk, dtype=np.float16)
+        vt16 = np.ascontiguousarray(vt, dtype=np.float16)
+        o16 = np.ascontiguousarray(out, dtype=np.float16).copy()
+        nb, d = qk16.shape[0], qk16.shape[2] // 2
+        assert qk16.shape == (nb, 1500, 2 * d) and vt16.shape == (nb, d, 1536) and o16.shape == (nb * 1500 + 128, d)
+        with self._lock:
+            rc = self.lib.wl_test_enc_attn(self.ctx, _lib.ptr(qk16.view(np.uint16), C.c_uint16), _lib.ptr(vt16.view(np.uint16), C.c_uint16),
+                                           _lib.ptr(o16.view(np.uint16), C.c_uint16), nb, d // 64, int(path), int(ab))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_enc_attn")
+        return o16
+
+    def test_enc_stem(self, feats: np.ndarray) -> np.ndarray:
+        """The conv stem with this model's weights (wl_test_enc_stem): features [nb, n_mels, 3000] -> the fp32 residual
+        stream [nb, 1500, d] after conv2 + GELU + the positional table."""
+        f = np.ascontiguousarray(feats, dtype=np.float32)
+        nb = f.shape[0]
+        assert f.shape == (nb, self.dims.n_mels, 3000)
+        x = np.empty((nb, 1500, self.dims.d_model), dtype=np.float32)
+        with self._lock:
+            rc = self.lib.wl_test_enc_stem(self.ctx, _lib.ptr(f, C.c_float), _lib.ptr(x, C.c_float), nb)
+            _lib.check(self.lib, self.ctx, rc, "wl_test_enc_stem")
+        return x
+
+    def test_layernorm(self, x: np.ndarray, gamma: np.ndarray, beta: np.ndarray, y16: Optional[np.ndarray],
+                       y32: Optional[np.ndarray]) -> Tuple[Optional[np.ndarray], Optional[np.ndarray]]:
+        """layernorm_rows (wl_test_layernorm) over x [rows, d].  y16 / y32: [rows + 8, d] buffers as they are before the
+        launch (y16 is rounded to fp16), or None to skip that output.  Returns both buffers after the launch, guard rows
+        included."""
+        x = np.ascontiguousarray(x, dtype=np.float32)
+        rows, d = x.shape
+        bufs = [None if y is None else np.ascontiguousarray(y, dtype=np.float32).copy() for y in (y16, y32)]
+        for y in bufs:
+            assert y is None or y.shape == (rows + 8, d)
+        g = np.ascontiguousarray(gamma, dtype=np.float32)
+        b = np.ascontiguousarray(beta, dtype=np.float32)
+        fp = lambda a: None if a is None else _lib.ptr(a, C.c_float)
+        with self._lock:
+            rc = self.lib.wl_test_layernorm(self.ctx, fp(x), fp(g), fp(b), fp(bufs[0]), fp(bufs[1]), rows, d)
+            _lib.check(self.lib, self.ctx, rc, "wl_test_layernorm")
+        return bufs[0], bufs[1]
+
     GEMM_OUT = {"f32": 0, "resid": 1, "f16": 2, "headsplit": 3}
     GEMM_VARIANT = {"auto": 0, "classic": 1, "pingpong": 2}
 
