@@ -13,6 +13,7 @@
  *   wl_detect_language   <- Whisper.detect_language        transcriber_faster_whisper.py:1140, :1771; batch_inference.py:283
  *   wl_align             <- Whisper.align                  transcriber_faster_whisper.py:1657-1663
  *   wl_slots_release     <- StorageView lifetime           transcriber_faster_whisper.py:1055, :1820-1823
+ *   wl_vad               <- faster_whisper.vad.get_speech_timestamps (the Silero model call) transcriber_faster_whisper.py:830-838
  *
  * Conventions: plain pointers and sizes only; the caller owns every host buffer; the library owns
  * device memory, streams, CUDA graphs.  Every function returns 0 or a negative WL_ERR_* code and
@@ -28,7 +29,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 6
+#define WL_ABI_VERSION 7
 
 typedef struct wl_ctx wl_ctx;
 
@@ -78,8 +79,8 @@ const char* wl_last_error(wl_ctx* ctx);   /* ctx may be NULL: last wl_init / wl_
 
 /* Device memory the context holds right now, in bytes, counted where the library allocates it: weights (the uploaded
  * tensors and their fused copies), the encoder workspaces and slot pool, the self-attention caches, both decode
- * states, an open session, the log-mel / prefill / align workspaces at their current grown size, and the weight-load
- * staging buffer while a load runs.  Not counted: buffers a call frees before it returns, CUDA graph executables and
+ * states, an open session, the log-mel / prefill / align / VAD workspaces at their current grown size, the VAD weights,
+ * and the weight-load staging buffer while a load runs.  Not counted: buffers a call frees before it returns, CUDA graph executables and
  * the CUDA context of the process. */
 int wl_device_bytes(wl_ctx* ctx, int64_t* out);
 /* Free and total device memory of CUDA ordinal `device` (cudaMemGetInfo); needs no context, so a load can be checked
@@ -262,7 +263,8 @@ int64_t wl_kernel_launches(wl_ctx* ctx);
 /* time (ms, CUDA events on the library stream) of the last wl_mel / wl_encode / wl_generate device work;
  * which = 3: average ms per cross-attention kernel launch since wl_profile_cross_attn(ctx, 1), 4: launches timed;
  * 2 also holds the last wl_session_run, 5 the last wl_session_admit */
-float wl_last_device_ms(wl_ctx* ctx, int32_t which /*0 mel, 1 encode, 2 generate, 3/4 cross-attention profile*/);
+float wl_last_device_ms(wl_ctx* ctx, int32_t which /*0 mel, 1 encode, 2 generate, 3/4 cross-attention profile,
+                                                      6 / 7 the last wl_vad's front end / recurrence*/);
 /* enable = 1: wl_generate calls made WITHOUT a CUDA graph bracket every cross-attention launch (K11, the dominant
  * decode kernel) with CUDA events on the library stream -- bench.py's live roofline measurement.  Resets the sums. */
 int wl_profile_cross_attn(wl_ctx* ctx, int32_t enable);
@@ -278,6 +280,21 @@ int wl_encode_windows(wl_ctx* ctx, int32_t B, const int32_t* win_stream, const i
  * host variant are reused (no H2D, no D2H) */
 int wl_mel_resident(wl_ctx* ctx);
 int wl_encode_resident(wl_ctx* ctx, int32_t B, const int32_t* slots);
+
+/* Silero VAD (16 kHz), fp32.  wl_vad_load_tensor takes a float32 host tensor under one of the fixed names
+ *   vad.stft.basis [258, 1, 256]     vad.conv0.weight [128, 129, 3]  vad.conv0.bias [128]
+ *   vad.conv1.weight [64, 128, 3]    vad.conv1.bias [64]             vad.conv2.weight [64, 64, 3]   vad.conv2.bias [64]
+ *   vad.conv3.weight [128, 64, 3]    vad.conv3.bias [128]
+ *   vad.lstm.weight_ih / vad.lstm.weight_hh [512, 128], vad.lstm.bias_ih / vad.lstm.bias_hh [512]  (gate order i, f, g, o)
+ *   vad.out.weight [1, 128, 1]       vad.out.bias [1]
+ * and rejects any other name or shape; it may be called before or after wl_finalize_weights (loading a name again
+ * replaces it).  wl_vad: pcm holds B waveforms concatenated at offsets[B+1] (samples); a waveform of n > 0 samples has
+ * n / 512 + 1 frames (the audio padded to the next multiple of 512, a whole frame of zeros when n already is one), one of
+ * 0 samples has none.  probs_out receives the speech probability of every frame, stream b's at
+ * [prob_off[b], prob_off[b+1]); prob_off must match the frame counts.  One upload, one download; host pointers.  Fails
+ * when any VAD tensor is missing. */
+int wl_vad_load_tensor(wl_ctx* ctx, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+int wl_vad(wl_ctx* ctx, const float* pcm, const int64_t* offsets, int32_t B, float* probs_out, const int64_t* prob_off);
 
 #ifdef __cplusplus
 }

@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 6
+ABI_VERSION = 7
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -98,6 +98,8 @@ SIGNATURES = {
     "wl_encode_windows": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p]),
     "wl_mel_resident": (C.c_int, [C.c_void_p]),
     "wl_encode_resident": (C.c_int, [C.c_void_p, C.c_int32, c_i32p]),
+    "wl_vad_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
+    "wl_vad": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p, c_i64p]),
 }
 
 _lock = threading.Lock()

@@ -35,6 +35,16 @@ except Exception as _e:  # pragma: no cover
 from .models import ModelRegistry, engine_footprint
 from .scheduler import BatchRequest, StreamScheduler
 
+
+def vad_from_env():
+    """``WLB200_VAD=device``: Silero probabilities on the model's GPU context (``vad.DeviceVad``); unset or ``cpu``:
+    faster-whisper's CPU module, as the reference."""
+    v = os.environ.get("WLB200_VAD", "cpu").strip().lower()
+    if v not in ("cpu", "device"):
+        raise ValueError(f"WLB200_VAD={v!r}: 'cpu' (default) or 'device'")
+    return "device" if v == "device" else None
+
+
 if ServeClientBase is not None:
 
     class ServeClientB200(ServeClientBase):
@@ -106,11 +116,12 @@ if ServeClientBase is not None:
             from .parallel import MultiDeviceWhisperModel, devices_from_env
             from .transcriber import B200WhisperModel
             devices = devices_from_env()     # WLB200_DEVICES=0,1,...: one engine context per GPU, streams placed i mod G
+            vad = vad_from_env()
             if len(devices) > 1:
                 return MultiDeviceWhisperModel(model_size_or_path, device_index=devices, device="cuda",
-                                               compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS)
+                                               compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS, vad=vad)
             return B200WhisperModel(model_size_or_path, device="cuda", device_index=devices[0],
-                                    compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS)
+                                    compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS, vad=vad)
 
         @classmethod
         def model_registry(cls) -> ModelRegistry:
@@ -126,7 +137,8 @@ if ServeClientBase is not None:
                         from .weights import resolve_model_dir
                         resolve = lambda name: resolve_model_dir(name, local_files_only=True)
                         kw = dict(resolve=resolve, devices=devices_from_env(), reserve_bytes=cls.MEMORY_RESERVE_BYTES,
-                                  footprint=lambda name: engine_footprint(name, cls.MAX_STREAMS, resolve=resolve))
+                                  footprint=lambda name: engine_footprint(name, cls.MAX_STREAMS, resolve=resolve,
+                                                                         vad=vad_from_env() == "device"))
                     cls.REGISTRY = ModelRegistry(cls.build_model, max_streams=cls.MAX_STREAMS,
                                                  batch_window_ms=cls.BATCH_WINDOW_MS, **kw)
                 return cls.REGISTRY

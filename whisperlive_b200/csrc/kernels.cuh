@@ -22,6 +22,18 @@ struct MelTables {
 void mel_forward(cudaStream_t st, const float* pcm, const long* pcm_off, float* out, const long* out_off, unsigned* gmax,
                  const MelTables& t, int B, int max_frames);
 
+// ---------------------------------------------------------------------------- Silero VAD (vad.cu)
+// Device copies in the layout wl_vad_load_tensor stores: basis [256][258], conv weights [ci][3][co], w_ih [128][512],
+// w_hh [512][128] (PyTorch rows, gate order i, f, g, o), w_out [128].
+struct VadWeights {
+  const float *basis, *w0, *b0, *w1, *b1, *w2, *b2, *w3, *b3, *w_ih, *w_hh, *b_ih, *b_hh, *w_out, *b_out;
+};
+// gx [total_frames][512]: the LSTM input projection of every frame (frame_off [B + 1] on the device)
+void vad_front(cudaStream_t st, const VadWeights& w, const float* pcm, const long* pcm_off, const long* frame_off, int B,
+               long total_frames, float* gx);
+// probs [total_frames]: the recurrence over each stream's frames
+void vad_lstm(cudaStream_t st, const VadWeights& w, const float* gx, const long* frame_off, int B, float* probs);
+
 // A value produced by a split-K GEMM: v(r, c) = bias[c] + sum_s ptr[s * stride + r * ld + c]  (fixed order).
 // nsplit == 1 with bias == nullptr is a plain buffer; nsplit == 0 means "nothing pending".
 struct PartialSrc {

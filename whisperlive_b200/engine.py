@@ -99,12 +99,13 @@ class EncoderOutput:
 
 
 def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
-                       n_align_heads: Optional[int] = None) -> int:
+                       n_align_heads: Optional[int] = None, vad: bool = False) -> int:
     """Device bytes a context of these shapes allocates through ``wl_init``, the weight load and one open decode session
     (csrc/engine.cu: ``wl_load_tensor``, ``finalize_impl``, ``alloc_decode_state``, ``wl_session_open``), plus the
     workspaces its first step round grows: the log-mel of ``max_streams`` 30-second chunks (``wl_mel``) and the batched
     prefill at its first size of 1024 rows (``prefill_reserve``).  What a model registry compares with the free memory
-    before a load.  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
+    before a load.  ``vad=True`` adds the Silero VAD weights and the VAD workspace of ``max_streams`` 30-second chunks
+    (``wl_vad_load_tensor``, ``wl_vad``).  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
     chunks, more prompt rows, the word-alignment buffers) and the allocator's rounding."""
     B, K = int(max_streams), int(max_beam)
     NS = int(enc_slots) if enc_slots is not None else 2 * B
@@ -146,7 +147,13 @@ def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 
     cap = 1024
     prefill = (4 * cap * i32 + 2 * (cap // 8 + 128) * i32 + (3 * R + 16) * i32 + cap * T * 2 + 5 * cap * d * f32
                + 2 * cap * d * f16 + cap * ff * f16 + 128 * H * 12 * MAX_ROWS * 66 * f32)
-    return int(weights + fused + mel_tables + encoder + pool + decoder + state + session + mel + prefill)
+    total = weights + fused + mel_tables + encoder + pool + decoder + state + session + mel + prefill
+    if vad:
+        vad_weights = (258 * 256 + 128 * 129 * 3 + 128 + 64 * 128 * 3 + 64 + 64 * 64 * 3 + 64 + 128 * 64 * 3 + 128
+                       + 2 * 512 * 128 + 2 * 512 + 128 + 1) * f32
+        vad_frames = B * (pcm // B // 512 + 1)
+        total += vad_weights + pcm * f32 + vad_frames * (512 + 1) * f32 + 2 * (B + 1) * 8
+    return int(total)
 
 
 def mem_info(device: int = 0) -> Tuple[int, int]:
@@ -292,6 +299,36 @@ class B200Whisper:
 
     def last_device_ms(self, which: int) -> float:
         return float(self.lib.wl_last_device_ms(self.ctx, which))
+
+    def vad_load(self, tensors: Dict[str, "np.ndarray"]) -> None:
+        """Upload the Silero VAD tensors (``vad.*`` names of include/wlb200.h) as float32."""
+        for name, t in tensors.items():
+            a = np.ascontiguousarray(t, dtype=np.float32)
+            shape = np.asarray(a.shape, dtype=np.int64)
+            with self._lock:
+                rc = self.lib.wl_vad_load_tensor(self.ctx, name.encode(), _lib.ptr(a, C.c_float), _lib.ptr(shape, C.c_int64),
+                                                 a.ndim)
+                _lib.check(self.lib, self.ctx, rc, f"wl_vad_load_tensor({name})")
+
+    def vad_probs(self, audios: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """Silero speech probability of every 512-sample frame of each waveform (``wl_vad``): one upload of all of
+        them, one launch of each kernel, one download."""
+        from .vad import n_frames
+        if not audios:
+            return []
+        waves = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in audios]
+        lens = np.asarray([w.shape[0] for w in waves], dtype=np.int64)
+        off = np.zeros(len(waves) + 1, dtype=np.int64)
+        off[1:] = np.cumsum(lens)
+        poff = np.zeros(len(waves) + 1, dtype=np.int64)
+        poff[1:] = np.cumsum([n_frames(int(n)) for n in lens])
+        pcm = np.concatenate(waves) if off[-1] else np.zeros(1, np.float32)
+        out = np.empty(max(int(poff[-1]), 1), dtype=np.float32)
+        with self._lock:
+            rc = self.lib.wl_vad(self.ctx, _lib.ptr(pcm, C.c_float), _lib.ptr(off, C.c_int64), len(waves),
+                                 _lib.ptr(out, C.c_float), _lib.ptr(poff, C.c_int64))
+            _lib.check(self.lib, self.ctx, rc, "wl_vad")
+        return [out[poff[i]:poff[i + 1]].copy() for i in range(len(waves))]
 
     def profile_cross_attn(self, enable: bool) -> None:
         """Bracket every cross-attention launch of graph-less generate calls with CUDA events (bench.py roofline)."""

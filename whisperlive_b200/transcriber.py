@@ -537,7 +537,18 @@ class TranscribeSession:
         t0 = time.perf_counter()
         def as_pcm(a):    # paths / bytes / file objects go through decode_audio like reference :820-821
             return a if isinstance(a, (str, bytes, bytearray, os.PathLike)) or hasattr(a, "read") else np.asarray(a)
-        prepared = [m._prepare_stream(as_pcm(a), dict(k)) for a, k in zip(audios, kws)]
+        vad = getattr(m, "_vad", None)
+        if hasattr(vad, "speech_timestamps_batch"):
+            # every VAD-gated stream of the call through one device VAD call, then the same gating per stream
+            inputs = [m._stream_input(as_pcm(a), dict(k)) for a, k in zip(audios, kws)]
+            gated = [i for i, (_a, k, _s) in enumerate(inputs) if k["vad_filter"] and k["clip_timestamps"] == "0"]
+            found = vad.speech_timestamps_batch([inputs[i][0] for i in gated],
+                                                [m._vad_options(vad, inputs[i][1]["vad_parameters"]) for i in gated]
+                                                ) if gated else []
+            chunks = dict(zip(gated, found))
+            prepared = [m._gate_stream(*inp, speech_chunks=chunks.get(i)) for i, inp in enumerate(inputs)]
+        else:
+            prepared = [m._prepare_stream(as_pcm(a), dict(k)) for a, k in zip(audios, kws)]
         tm["prepare"] = tm.get("prepare", 0.0) + time.perf_counter() - t0
         handles: List[int] = []
         live = [i for i, p in enumerate(prepared) if p is not None]
@@ -912,14 +923,23 @@ class B200WhisperModel:
         product path builds the CUDA engine (whisperlive_b200.engine.B200Whisper) and fails
         loudly when libwlb200.so, a GPU, the checkpoint or tokenizer.json is missing.
         ``weights="random"`` / ``hf_tokenizer="synthetic"`` are the explicit opt-ins bench.py and
-        the tests use (no checkpoints offline)."""
+        the tests use (no checkpoints offline).
+        ``vad``: None gates ``vad_filter`` streams with ``faster_whisper.vad`` (CPU Silero, as the reference does); a
+        module with that interface replaces it; ``"device"`` computes the Silero probabilities on this model's own GPU
+        context (``vad.DeviceVad``, the Silero weights from ``WLB200_VAD_MODEL`` or faster-whisper's bundled model; with
+        ``weights="random"`` seeded random ones)."""
         self.logger = logger
-        self._vad = vad
         if engine is None:
             from .engine import B200Whisper  # raises if the CUDA library cannot be loaded
             engine = B200Whisper.from_model(model_size_or_path, device_index=device_index, compute_type=compute_type,
                                             weights=weights, seed=seed, max_streams=max_streams, max_beam=max_beam,
                                             download_root=download_root, local_files_only=local_files_only)
+        if isinstance(vad, str):
+            if vad != "device":
+                raise ValueError(f"vad={vad!r}: pass None, a faster_whisper.vad-like module, or 'device'")
+            from .vad import DeviceVad
+            vad = DeviceVad(engine, weights="random" if weights == "random" else None, seed=seed)
+        self._vad = vad
         self.model = engine
         model_dir = getattr(engine, "model_dir", None) or model_size_or_path
         if isinstance(hf_tokenizer, str):
@@ -1028,6 +1048,11 @@ class B200WhisperModel:
                      language_detection_threshold=0.5, language_detection_segments=1)
 
     def _prepare_stream(self, audio: np.ndarray, kw: dict) -> Optional[dict]:
+        return self._gate_stream(*self._stream_input(audio, kw))
+
+    def _stream_input(self, audio, kw: dict) -> Tuple[np.ndarray, dict, bool]:
+        """The stream's PCM (decoded when given as a path / bytes / file), its full keyword set, and the bench-only
+        single-window flag."""
         single_window = bool(kw.pop("_single_window", False))   # not part of the reference surface (bench.py only)
         full = dict(self._DEFAULTS)
         unknown = set(kw) - set(full)
@@ -1043,17 +1068,27 @@ class B200WhisperModel:
             self.logger.warning("The current model is English-only but the multilingual parameter is set to True; "
                                 "setting to False instead.")
             kw["multilingual"] = False
+        return audio, kw, single_window
+
+    @staticmethod
+    def _vad_options(vad, vad_parameters):
+        if vad_parameters is None:
+            return vad.VadOptions()
+        if isinstance(vad_parameters, dict):
+            return vad.VadOptions(**vad_parameters)
+        return vad_parameters
+
+    def _gate_stream(self, audio: np.ndarray, kw: dict, single_window: bool, speech_chunks=None) -> Optional[dict]:
+        """VAD clipping (``speech_chunks``: already found for this stream by a batched VAD call) and the stream record."""
+        sr = self.feature_extractor.sampling_rate
         duration = audio.shape[0] / sr
         duration_after_vad = duration
-        speech_chunks = None
         vad_parameters = kw["vad_parameters"]
         if kw["vad_filter"] and kw["clip_timestamps"] == "0":
             vad = self._vad or _load_vad()
-            if vad_parameters is None:
-                vad_parameters = vad.VadOptions()
-            elif isinstance(vad_parameters, dict):
-                vad_parameters = vad.VadOptions(**vad_parameters)
-            speech_chunks = vad.get_speech_timestamps(audio, vad_parameters)
+            vad_parameters = self._vad_options(vad, vad_parameters)
+            if speech_chunks is None:
+                speech_chunks = vad.get_speech_timestamps(audio, vad_parameters)
             chunks, _meta = vad.collect_chunks(audio, speech_chunks)
             audio = np.concatenate(chunks, axis=0) if len(chunks) else audio[:0]
             duration_after_vad = audio.shape[0] / sr
