@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 7
+#define WL_ABI_VERSION 8
 
 typedef struct wl_ctx wl_ctx;
 
@@ -69,9 +69,7 @@ typedef struct wl_gen_opts {
                                         step per prompt token; the parity tests compare the two) */
 } wl_gen_opts;
 
-/* With WLB200_FUSE_POST=1 (a diagnostic switch, default off) wl_init refuses a second live context on a device: the
- * fused kernels' grid barrier is not safe with two contexts decoding at once.
- * A wl_init that fails frees whatever it had created; so does a wl_finalize_weights that fails (the tensors
+/* A wl_init that fails frees whatever it had created; so does a wl_finalize_weights that fails (the tensors
  * wl_load_tensor uploaded stay until wl_destroy).  A failed load leaves no device memory behind but the context's. */
 int wl_init(const wl_config* cfg, wl_ctx** out);
 void wl_destroy(wl_ctx* ctx);
@@ -199,8 +197,7 @@ int wl_test_gemm(wl_ctx* ctx, const uint16_t* a_f16, const uint16_t* b_f16, cons
 int wl_gemm_variant(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t* variant_out);
 /* test hook of the small-batch decode GEMM (csrc/wgemm.cu, R <= 32): out[R][n_out] = X[R][K] W[n_out][K]^T with the fused
  * epilogue `mode` -- 0: + bias; 1: out += acc + bias (residual in place); 2: gelu(acc + bias) through fp16;
- * 3: split-K partial sums (K > 1280), summed by the hook; mode | 8 (8, 9, 10): the cluster split-K GEMM (cgemm, any R)
- * with epilogue 0, 1, 2 */
+ * 3: split-K partial sums (K > 1280), summed by the hook */
 int wl_test_wgemm(wl_ctx* ctx, const uint16_t* w_f16, const uint16_t* x_f16, const float* bias, float* out, int32_t R,
                   int32_t n_out, int32_t K, int32_t mode);
 /* Test hooks of the decode-step kernels of the default path for more than 16 decoder rows.  Each launches the kernels

@@ -119,37 +119,6 @@ def test_wgemm_small_batch(case):
     np.testing.assert_allclose(got, ref, atol=2e-3 if mode != 2 else 4e-3, rtol=2e-3)
 
 
-CGEMM_CASES = [
-    # (R, n_out, K, mode)   every row-tile width (16/32/64/128 + a second row tile), K ranges of 1..8 CTAs, ragged edges
-    (128, 1280, 1280, 1), (128, 3840, 1280, 0), (128, 5120, 1280, 2), (128, 1280, 5120, 1), (64, 1280, 1280, 0), (32, 3840, 1280, 0),
-    (20, 768, 3072, 1), (160, 1280, 1280, 1), (100, 384, 1536, 2), (17, 200, 64, 0), (33, 1000, 704, 1), (128, 128, 128, 0),
-]
-
-
-@pytest.mark.parametrize("case", CGEMM_CASES)
-def test_cgemm_cluster_split_k(case):
-    """The cluster split-K decode GEMM (csrc/dec_gemm.cu::cgemm_kernel: wgmma pipeline, K ranges = the CTAs of a
-    cluster, reduction through distributed shared memory, fused epilogue) against fp32 numpy on the same fp16 inputs."""
-    eng, _ = engine("micro.en")
-    R, n_out, K, mode = case
-    rng = np.random.default_rng(abs(hash(case)) % (2 ** 31))
-    w = (rng.standard_normal((n_out, K)) / np.sqrt(K)).astype(np.float16)
-    x = rng.standard_normal((R, K)).astype(np.float16)
-    bias = rng.standard_normal(n_out).astype(np.float32)
-    resid = rng.standard_normal((R, n_out)).astype(np.float32) if mode == 1 else None
-    ref = x.astype(np.float32) @ w.astype(np.float32).T + bias[None, :]
-    if mode == 1:
-        ref = ref + resid
-    if mode == 2:
-        ref = torch.nn.functional.gelu(torch.from_numpy(ref)).numpy()
-    got = eng.test_wgemm(w, x, bias, mode=mode | 8, resid=resid)
-    again = eng.test_wgemm(w, x, bias, mode=mode | 8, resid=resid)
-    err = np.abs(got - ref).max()
-    print(f"cgemm {case}: max err {err:.3e}")
-    np.testing.assert_allclose(got, ref, atol=2e-3 if mode != 2 else 4e-3, rtol=2e-3)
-    assert np.array_equal(got, again), "the cluster reduction must be bit-reproducible"
-
-
 # --------------------------------------------------------------------------------------- K1 mel
 @pytest.mark.parametrize("n_mels_model", ["micro.en", "large-v3-mel"])
 def test_mel_matches_oracle(n_mels_model):

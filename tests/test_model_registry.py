@@ -10,7 +10,6 @@ from types import SimpleNamespace
 import numpy as np
 import pytest
 
-ROOT = os.path.abspath(os.path.join(os.path.dirname(__file__), ".."))
 REF = "/root/reference"
 
 
@@ -482,37 +481,6 @@ def test_device_bytes_and_footprint_estimate(name):
     finally:
         m.destroy()
     assert eng.device_bytes == 0
-
-
-FUSE_WORKER = r"""
-import sys
-sys.path.insert(0, sys.argv[1])
-from whisperlive_b200 import _lib
-from whisperlive_b200.config import dims_for
-from whisperlive_b200.engine import B200Whisper
-from whisperlive_b200.weights import random_init
-dims = dims_for("micro.en")
-w = random_init(dims, seed=0)
-a = B200Whisper(dims, w, max_streams=1, max_beam=1)
-try:
-    B200Whisper(dims, w, max_streams=1, max_beam=1)
-    print("second context allowed")
-except _lib.WlError as e:
-    print("refused:", e)
-a.destroy()
-b = B200Whisper(dims, w, max_streams=1, max_beam=1)
-print("after destroy: ok", b.device_bytes > 0)
-"""
-
-
-@pytest.mark.gpu
-def test_fused_post_switch_allows_one_context_per_device():
-    import subprocess
-    env = dict(os.environ, WLB200_FUSE_POST="1")
-    out = subprocess.run([sys.executable, "-c", FUSE_WORKER, ROOT], env=env, capture_output=True, text=True, timeout=300)
-    assert out.returncode == 0, out.stderr
-    assert "refused:" in out.stdout and "one engine context per device" in out.stdout, out.stdout
-    assert "after destroy: ok True" in out.stdout, out.stdout
 
 
 @pytest.mark.gpu

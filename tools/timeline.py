@@ -31,12 +31,7 @@ def main(path):
         (t0, k0), (t1, k1) = ready[i], ready[i + 1]
         name = NAMES.get(k0, str(k0))
         if k0 == 3:
-            if k1 == 3:
-                name += " (cold launch, WLB200_DUP)"
-            else:
-                name += {4: " qkv", 5: " q_cross", 7: " fc1", 8: " vocab"}.get(k1, " out/fc2 (->LN)")
-                if i > 0 and ready[i - 1][1] == 3:
-                    name += " [warm repeat]"
+            name += {4: " qkv", 5: " q_cross", 7: " fc1", 8: " vocab"}.get(k1, " out/fc2 (->LN)")
         iv[name].append((t1 - t0) / 1e3)
     tot = sum(sum(v) for v in iv.values())
     print(f"{'kernel':32s} {'n':>7s} {'mean us':>9s} {'p50':>8s} {'p90':>8s} {'share':>7s}")

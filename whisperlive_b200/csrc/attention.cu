@@ -217,7 +217,7 @@ void decoder_self_attn(cudaStream_t st, const DecodeState& s, const PartialSrc& 
 //   * two passes over the key range (scores -> exact max/sum -> weights), so no online rescaling; P is fed to the
 //     second MMA as fp16, the row sum is taken over the same rounded values.
 constexpr int XA_CHUNK = 128;                 // keys per pipeline stage
-constexpr int XA_STAGES_DEFAULT = 3;          // x 3 CTAs per SM at beam <= 4: 144 KB of K/V in flight per SM
+constexpr int XA_STAGES = 3;                  // x 3 CTAs per SM at beam <= 4: 144 KB of K/V in flight per SM
 constexpr int XA_STAGE_BYTES = XA_CHUNK * 128;  // 64 halves per key
 constexpr int XA_NCHUNK = (S_ENC + XA_CHUNK - 1) / XA_CHUNK;  // 12
 constexpr int XA_TAIL_KEYS = S_ENC - (XA_NCHUNK - 1) * XA_CHUNK;  // 92 keys in the last chunk
@@ -240,6 +240,16 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4],
                : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
                : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
+// A consumer warp hands a ring stage it has read with ldmatrix back to the producer.  The stage is refilled by
+// cp.async.bulk (async proxy), so the generic-proxy ldmatrix reads must be ordered before that write by a proxy fence;
+// the mbarrier arrive alone does not do it.  With CUDA 12.9, ptxas scheduled the arrive before the MMA that consumes the
+// last fragment, with no wait on that ldmatrix: the next chunk could overwrite K/V not yet read, and a stream's
+// attention output then depended on which other streams were still decoding.
+__device__ __forceinline__ void release_stage(uint64_t* empty, int lane) {
+  __syncwarp();
+  fence_proxy_async();
+  if (lane == 0) mbar_arrive(empty);
+}
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   const __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<const uint32_t*>(&h);
@@ -249,12 +259,12 @@ template <int NQ> struct XaCfg {
   static constexpr int SW = NQ <= 2 ? 2 : NQ <= 4 ? 4 : 8;   // score columns kept per key (fp32)
 };
 
-template <int NQ, int XA_STAGES>
+template <int NQ>
 __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialSrc q,
                                                          const __half* __restrict__ kc, const __half* __restrict__ vc,
                                                          long slot_stride, float* __restrict__ part,
                                                          float* __restrict__ probs, __half* __restrict__ out, int B,
-                                                         int rows_per_stream, int H, int d, int nsplit, int cps, int dbg) {
+                                                         int rows_per_stream, int H, int d, int nsplit, int cps) {
   constexpr int SW = XaCfg<NQ>::SW;
   extern __shared__ uint8_t xa_smem_raw[];
   uint8_t* base = xa_smem_raw + ((128u - (smem_u32(xa_smem_raw) & 127u)) & 127u);   // pointer arithmetic keeps the shared address space (LDS/STS)
@@ -398,7 +408,6 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
     for (int mt = 0; mt < 2; ++mt) {
       sc[mt][0] = sc[mt][1] = sc[mt][2] = sc[mt][3] = 0.f;
       const int key_l = warp * 32 + mt * 16 + ld_row;
-      if (dbg & 1) continue;
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
         uint32_t a[4];
@@ -408,8 +417,7 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
         mma_16816(sc[mt], a, ql[ks][0], ql[ks][1]);
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);  // K fragments are in registers now
+    release_stage(&empty[stage], lane);   // K fragments are in registers now
     if (++stage == XA_STAGES) { stage = 0; phase ^= 1; }
     if (2 * tq < SW) {
 #pragma unroll
@@ -431,7 +439,7 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
       const int idx = tid + e * 128, j = idx >> 6, dd = idx & 63;
-      const bool ok = j < rows_per_stream && !(dbg & 2);
+      const bool ok = j < rows_per_stream;
       qraw[e][0] = (ok && q.bias) ? __ldg(q.bias + h2 * 64 + dd) : 0.f;
       const float* qp = q.ptr + (long)(b2 * rows_per_stream + (ok ? j : 0)) * d + h2 * 64 + dd;
 #pragma unroll
@@ -445,9 +453,8 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
   float mx[NQ], sm[NQ];
 #pragma unroll
   for (int j = 0; j < NQ; ++j) mx[j] = -INFINITY;
-  const int nk_sm = (dbg & 4) ? 0 : nk_pad;
 #pragma unroll 1
-  for (int k = tid; k < nk_sm; k += 128) {
+  for (int k = tid; k < nk_pad; k += 128) {
 #pragma unroll
     for (int j = 0; j < NQ; ++j) mx[j] = fmaxf(mx[j], S[(long)k * SW + j]);
   }
@@ -466,7 +473,7 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
 #pragma unroll
   for (int j = 0; j < NQ; ++j) sm32[j] = 0.f;
 #pragma unroll 1
-  for (int k = tid; k < nk_sm; k += 128) {
+  for (int k = tid; k < nk_pad; k += 128) {
 #pragma unroll
     for (int j = 0; j < NQ; ++j) {
       const float e32 = __expf(S[(long)k * SW + j] - mx[j]);
@@ -513,7 +520,9 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
   for (int ci = 0; ci < nchunks; ++ci) {
     mbar_wait(&full[stage], phase);
     const uint32_t buf = smem_u32(stage_buf + stage * XA_STAGE_BYTES);
-#pragma unroll
+    // rolled: unrolled, ptxas hoists the second k-step's ldmatrix loads above the first one's MMAs and the 8-row
+    // instantiation spills
+#pragma unroll 1
     for (int kk = 0; kk < 2; ++kk) {
       const int kbase = warp * 32 + kk * 16;
       uint32_t b0 = 0u, b1 = 0u;
@@ -523,7 +532,6 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
         b1 = *reinterpret_cast<const uint32_t*>(pp + 8);
       }
       const int key_l = kbase + ldt_row;
-      if (dbg & 1) continue;
 #pragma unroll
       for (int mt = 0; mt < 4; ++mt) {
         uint32_t a[4];
@@ -532,8 +540,7 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
         mma_16816(o[mt], a, b0, b1);
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[stage]);
+    release_stage(&empty[stage], lane);
     if (++stage == XA_STAGES) { stage = 0; phase ^= 1; }
   }
   // reduce the 4 warps (key quarters) through smem: lane holds O[j = 2tq + {0,1}][dd = mt*16 + g (+8)]
@@ -546,7 +553,6 @@ __global__ void __launch_bounds__(160) cross_attn_kernel(DecodeState s, PartialS
     ob[64 + 8] = o[mt][3];
   }
   consumers_sync();
-  if (dbg & 8) { consumers_sync(); continue; }
   if (nsplit == 1) {   // the whole key range was here: normalise and store the attention output directly
     for (int idx = tid; idx < NQ * 64; idx += 128) {
       const int j = idx >> 6, dd = idx & 63;
@@ -628,31 +634,12 @@ __global__ void __launch_bounds__(64) cross_attn_combine_kernel(DecodeState s, c
 static int xa_template_nq(int rows_per_stream) {
   return rows_per_stream == 1 ? 1 : rows_per_stream == 2 ? 2 : rows_per_stream <= 4 ? 4 : rows_per_stream == 5 ? 5 : 8;
 }
-// WLB200_XA_DBG (profiling only, results become garbage): 1 skip the MMA work, 2 skip the q reduction, 4 skip the
-// softmax pass, 8 skip the write-out / merge -- isolates how much of the kernel time is pure K/V streaming
-static int xa_dbg() {
-  static const int v = [] { const char* e = getenv("WLB200_XA_DBG"); return e ? atoi(e) : 0; }();
-  return v;
-}
-static int xa_stages() {
-  static const int st = [] {
-    const char* e = getenv("WLB200_XA_STAGES");
-    const int v = e ? atoi(e) : XA_STAGES_DEFAULT;
-    return v == 2 || v == 4 ? v : 3;
-  }();
-  return st;
-}
 static int xa_smem_bytes(int cps, int NQ) {
   const int sw = NQ <= 2 ? 2 : NQ <= 4 ? 4 : 8;
   const int nk = cps * XA_CHUNK;
-  return 128 + xa_stages() * XA_STAGE_BYTES + std::max(nk * sw, 4 * 8 * 64) * 4 + NQ * (nk + 8) * 2 + 64 * 4 + 2 * xa_stages() * 8 + 64;
+  return 128 + XA_STAGES * XA_STAGE_BYTES + std::max(nk * sw, 4 * 8 * 64) * 4 + NQ * (nk + 8) * 2 + 64 * 4 + 2 * XA_STAGES * 8 + 64;
 }
 
-template <int NQ>
-static const void* xa_kernel_ptr() {
-  const int stg = xa_stages();
-  return stg == 2 ? (const void*)cross_attn_kernel<NQ, 2> : stg == 4 ? (const void*)cross_attn_kernel<NQ, 4> : (const void*)cross_attn_kernel<NQ, 3>;
-}
 // resident CTAs per SM for this key-range length, asked from the runtime (cached): the grid of the persistent
 // kernel is exactly occupancy x SMs
 static int xa_occupancy(int NQ, int cps) {
@@ -662,7 +649,11 @@ static int xa_occupancy(int NQ, int cps) {
   const int key = NQ * 64 + cps;
   auto it = cache.find(key);
   if (it != cache.end()) return it->second;
-  const void* k = NQ == 1 ? xa_kernel_ptr<1>() : NQ == 2 ? xa_kernel_ptr<2>() : NQ == 4 ? xa_kernel_ptr<4>() : NQ == 5 ? xa_kernel_ptr<5>() : xa_kernel_ptr<8>();
+  const void* k = NQ == 1   ? (const void*)cross_attn_kernel<1>
+                  : NQ == 2 ? (const void*)cross_attn_kernel<2>
+                  : NQ == 4 ? (const void*)cross_attn_kernel<4>
+                  : NQ == 5 ? (const void*)cross_attn_kernel<5>
+                            : (const void*)cross_attn_kernel<8>;
   int occ = 0;
   WL_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k, 160, (size_t)xa_smem_bytes(cps, NQ)));
   occ = std::max(1, occ);
@@ -673,7 +664,6 @@ static int xa_occupancy(int NQ, int cps) {
 // Choose how many CTAs share one (stream, head): the grid should fill whole waves of resident CTAs
 // (occupancy is set by shared memory: the score / weight buffers shrink with the split).
 int cross_attn_pick_nsplit(int B, int H, int num_sms, int rows_per_stream) {
-  static const int forced = [] { const char* e = getenv("WLB200_XA_NSPLIT"); return e ? atoi(e) : 0; }();
   const int NQ = xa_template_nq(rows_per_stream);
   // cost of a split = waves of resident CTAs x (chunks per CTA + a fixed per-CTA cost of ~3 chunk times: q reduction,
   // pipeline fill, the softmax pass between the two sweeps, partial write-out); ties go to fewer partials
@@ -683,7 +673,6 @@ int cross_attn_pick_nsplit(int B, int H, int num_sms, int rows_per_stream) {
     const int cps = (XA_NCHUNK + ns - 1) / ns;
     const int real = (XA_NCHUNK + cps - 1) / cps;
     if (real != ns) continue;
-    if (forced == ns) return ns;
     const int occ = xa_occupancy(NQ, cps);
     const long slots = (long)occ * num_sms, items = (long)B * H * ns;
     const long waves = (items + slots - 1) / slots;
@@ -704,19 +693,16 @@ static void launch_cross(cudaStream_t st, const DecodeState& s, const PartialSrc
   const int occ = xa_occupancy(NQ, cps);
   WL_CHECK(B <= MAX_STREAMS_CAP, WL_ERR_ARG, "cross attention: %d streams exceed the compiled cap %d", B, MAX_STREAMS_CAP);
   dim3 grid((unsigned)std::min<long>((long)B * H * nsplit, (long)occ * sms));
-  const int stg = xa_stages();
-  auto k = stg == 2 ? cross_attn_kernel<NQ, 2> : stg == 4 ? cross_attn_kernel<NQ, 4> : cross_attn_kernel<NQ, 3>;
   if (ws.ev0) WL_CUDA(cudaEventRecord(ws.ev0, st));
-  launch_kernel(k, grid, dim3(160), (size_t)smem, st, s, q, kc, vc, slot_stride, ws.part, ws.probs, out, B, rows_per_stream, H, d, nsplit, cps, xa_dbg());
+  launch_kernel(cross_attn_kernel<NQ>, grid, dim3(160), (size_t)smem, st, s, q, kc, vc, slot_stride, ws.part, ws.probs, out, B,
+                rows_per_stream, H, d, nsplit, cps);
   if (ws.ev1) WL_CUDA(cudaEventRecord(ws.ev1, st));
   note_launch(1);
 }
 
 template <int NQ>
 static void prime_cross() {
-  WL_CUDA(cudaFuncSetAttribute(cross_attn_kernel<NQ, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  WL_CUDA(cudaFuncSetAttribute(cross_attn_kernel<NQ, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-  WL_CUDA(cudaFuncSetAttribute(cross_attn_kernel<NQ, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+  WL_CUDA(cudaFuncSetAttribute(cross_attn_kernel<NQ>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
 }
 void attention_tl_bind(unsigned long long* p) { tl_bind_tu(p); }
 void attention_prime() {

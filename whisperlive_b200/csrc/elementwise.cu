@@ -132,41 +132,12 @@ __global__ void __launch_bounds__(256) layernorm_kernel(const float* __restrict_
 // launch costs there is the instruction fetch of whatever it executes (the kernels of a layer do not fit the SM's
 // instruction caches together), so it is written for size rather than generality.  It also folds in the residual update that the preceding split-K GEMM left as partial sums:
 // x += bias + sum_s partial_s, in a fixed order (bit-reproducible).
-constexpr int PF_PIECE = 32 * 1024;   // bytes per cp.async.bulk.prefetch.L2
-
-// PF = true (the first LayerNorm of a decoder layer, WLB200_XA_PREFETCH): warp 0 additionally asks L2 to fetch its share
-// of the layer's encoder K/V for the first pf.n_streams live streams -- fire and forget, issued before the dependency
-// wait (the pool, the slot ids and the done flags all predate the step).  The cross-attention that follows six
-// latency-bound kernels later then finds those streams in L2 instead of waiting for HBM.
-template <bool PF>
 __global__ void __launch_bounds__(384) layernorm_update_kernel(float* __restrict__ x, PartialSrc upd, const float* __restrict__ g,
-                                                               const float* __restrict__ be, __half* __restrict__ y, int d,
-                                                               L2Prefetch pf) {
+                                                               const float* __restrict__ be, __half* __restrict__ y, int d) {
   const long row = blockIdx.x;
   __shared__ float red[2][12];
   const int tid = threadIdx.x, nw = blockDim.x >> 5;
   pdl_trigger();
-  if constexpr (PF) {
-    if (tid < 32) {
-      const int per_region = (int)((pf.slot_bytes + PF_PIECE - 1) / PF_PIECE);      // pieces per (stream, K|V)
-      const int piece = (int)blockIdx.x + (int)gridDim.x * tid;                      // one piece per lane, strided over the grid
-      const int want = piece / (2 * per_region);                                     // index in the live list
-      int found = -1, base_n = 0;
-      for (int b0 = 0; b0 < pf.B; b0 += 32) {                                        // warp-uniform trip count
-        const bool alive = (b0 + tid < pf.B) && !pf.done[b0 + tid];
-        const unsigned m = __ballot_sync(0xffffffffu, alive);
-        const int c = __popc(m);
-        if (found < 0 && want >= base_n && want < base_n + c) found = b0 + (int)__fns(m, 0, want - base_n + 1);
-        base_n += c;
-      }
-      if (want < pf.n_streams && found >= 0) {
-        const int r = piece - want * 2 * per_region, kv = r / per_region, off = (r - kv * per_region) * PF_PIECE;
-        const char* src = reinterpret_cast<const char*>(kv ? pf.v : pf.k) + (long)pf.slot[found] * pf.slot_bytes + off;
-        const unsigned bytes = (unsigned)min((long)PF_PIECE, pf.slot_bytes - off);
-        asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(src), "r"(bytes) : "memory");
-      }
-    }
-  }
   // bias, gamma, beta are weights: fetched before waiting for the producer kernel
   float4 v = (upd.nsplit > 0 && upd.bias) ? __ldg(reinterpret_cast<const float4*>(upd.bias) + tid) : make_float4(0.f, 0.f, 0.f, 0.f);
   const float4 gg = __ldg(reinterpret_cast<const float4*>(g) + tid), bb = __ldg(reinterpret_cast<const float4*>(be) + tid);
@@ -206,16 +177,11 @@ __global__ void __launch_bounds__(384) layernorm_update_kernel(float* __restrict
 }
 
 void layernorm_update_rows(cudaStream_t st, float* x, const PartialSrc& upd, const float* gamma, const float* beta, __half* y,
-                           int rows, int d, const L2Prefetch* pf) {
+                           int rows, int d) {
   WL_CHECK(d <= 1536 && d % 128 == 0, WL_ERR_ARG, "layernorm_update: unsupported width %d", d);
   WL_CHECK(upd.nsplit >= 0 && upd.nsplit <= 8 && (upd.nsplit == 0 || upd.stride % 4 == 0), WL_ERR_ARG,
            "layernorm_update: at most 8 K ranges, stride a multiple of 4");
-  if (pf && pf->n_streams > 0) {
-    WL_CHECK(pf->slot_bytes % 16 == 0, WL_ERR_ARG, "layernorm_update: prefetch region not 16-byte aligned");
-    launch_kernel(layernorm_update_kernel<true>, dim3(rows), dim3(d / 4), 0, st, x, upd, gamma, beta, y, d, *pf);
-  } else {
-    launch_kernel(layernorm_update_kernel<false>, dim3(rows), dim3(d / 4), 0, st, x, upd, gamma, beta, y, d, L2Prefetch());
-  }
+  launch_kernel(layernorm_update_kernel, dim3(rows), dim3(d / 4), 0, st, x, upd, gamma, beta, y, d);
   note_launch(1);
 }
 

@@ -5,7 +5,6 @@
 #include <cstdlib>
 #include <cstring>
 #include <map>
-#include <mutex>
 #include <string>
 #include <thread>
 #include <vector>
@@ -30,17 +29,6 @@ void search_tl_bind(unsigned long long* p);
 }  // namespace wl
 
 static std::string g_init_error;
-
-// WLB200_FUSE_POST=1 (default off) fuses the split-K consumers into the producing GEMM behind a grid barrier that
-// needs every CTA of the grid resident at once.  Two contexts decoding at the same time on one device (two models of
-// one process) could each be partly resident and wait on each other, so with it on wl_init refuses a second context
-// on a device: g_live counts the contexts alive per device.
-static bool fuse_post_env() {
-  static const bool on = [] { const char* e = getenv("WLB200_FUSE_POST"); return e ? atoi(e) != 0 : false; }();
-  return on;
-}
-static std::mutex g_live_mu;
-static std::map<int, int> g_live;
 
 struct EncLayer {
   __half *w_qk, *w_v, *w_o, *w_fc1, *w_fc2;
@@ -71,7 +59,6 @@ struct wl_ctx {
   float last_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};   // [0] mel, [1] encode, [2] generate / session run, [5] session admit
                                                 // (prefill), [6] / [7] VAD front end / recurrence
   // per-kernel profiling of the dominant decode kernel (bench.py roofline): events around every cross-attention launch
-  unsigned* post_bar = nullptr;   // grid-barrier words of the fused split-K consumers
   int prof_cross = 0;
   cudaEvent_t pev0 = nullptr, pev1 = nullptr;
   double prof_cross_ms = 0.0;
@@ -79,7 +66,6 @@ struct wl_ctx {
   int num_sms = 132;
   int d, H, Le, Ld, n_mels, V, Vld, Bm, Km, Rm, NS;
   bool finalized = false;
-  bool counted_live = false;   // counted in g_live (a wl_init that succeeded)
   // every device buffer the context holds and its size in bytes (dalloc); dev_bytes is their sum plus the weight-load
   // staging buffer while it exists -- what wl_device_bytes reports
   std::vector<std::pair<void*, size_t>> allocs;
@@ -254,10 +240,6 @@ static void free_ctx(wl_ctx* c) {
   for (cudaEvent_t e : c->vad.ev)
     if (e) cudaEventDestroy(e);
   if (c->st) cudaStreamDestroy(c->st);
-  if (c->counted_live) {
-    std::lock_guard<std::mutex> g(g_live_mu);
-    --g_live[c->cfg.device];
-  }
   delete c;
 }
 
@@ -328,7 +310,6 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     gemm_prime();
     dec_gemm_prime();
     wgemm_prime();
-    cgemm_prime();
     attention_prime();
     search_prime();
     flash_attn_prime();
@@ -344,15 +325,6 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     c->dec.resize(c->Ld);
     for (int i = c->NS - 1; i >= 0; --i) c->slot_free.push_back(i);
     c->slot_used.assign(c->NS, 0);
-    {
-      std::lock_guard<std::mutex> g(g_live_mu);
-      int& live = g_live[cfg->device];
-      WL_CHECK(!(fuse_post_env() && live > 0), WL_ERR_STATE,
-               "WLB200_FUSE_POST=1 allows one engine context per device (its grid barrier needs every CTA resident, "
-               "which two contexts decoding at once on device %d cannot guarantee); %d already exist", cfg->device, live);
-      ++live;
-      c->counted_live = true;
-    }
   } catch (const wl::Error& e) {
     // a failed init frees the stream, the events and the timeline buffer it had made: nothing stays on the device
     g_init_error = e.msg;
@@ -398,7 +370,7 @@ extern "C" int wl_mem_info(int32_t device, int64_t* free_out, int64_t* total_out
 
 extern "C" const char* wl_last_error(wl_ctx* c) { return c ? c->err.c_str() : g_init_error.c_str(); }
 extern "C" int64_t wl_kernel_launches(wl_ctx* c) {
-  return c ? gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + cgemm_launch_count() + other_launch_count() - c->capture_counted + c->graph_launched : 0;
+  return c ? gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + other_launch_count() - c->capture_counted + c->graph_launched : 0;
 }
 extern "C" float wl_last_device_ms(wl_ctx* c, int32_t which) {
   if (!c) return -1.f;
@@ -653,7 +625,6 @@ static void finalize_impl(wl_ctx* c) {
   c->vcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
   c->xws.part = dalloc<float>(c, (size_t)c->Bm * H * 12 * MAX_ROWS_PER_STREAM * 66);
   c->xws.probs = nullptr;
-  c->post_bar = dalloc<unsigned>(c, 2);
   c->suppress_mask = dalloc<unsigned>(c, (V + 31) / 32 + 1);
   if (!c->align_heads.empty()) {
     c->align_heads_dev = dalloc<int>(c, c->align_heads.size());
@@ -1079,18 +1050,9 @@ void gather_align_probs(cudaStream_t st, const DecodeState& s, const float* prob
                         int layer, int B, int rows_per_stream, int H);
 }
 
-// Switches that are read at every call and are part of the graph key, so that one process can sweep them
-// (tools/sweep_prefetch.py): WLB200_XA_PREFETCH, WLB200_CGEMM
-static int xa_prefetch_streams() {
-  const char* e = getenv("WLB200_XA_PREFETCH");
-  return e ? atoi(e) : 0;
-}
-// The cluster split-K GEMM (cgemm) is off by default: in place of the consumers summing split-K partials it adds a serial
-// DSMEM reduction and two cluster barriers after the MMAs (DESIGN.md section 5.1).
-static bool cgemm_enabled() {
-  const char* e = getenv("WLB200_CGEMM");
-  return e ? atoi(e) != 0 : false;
-}
+// Decoder rows up to which every linear layer of the decode step is one wgemm launch (one m16 tile: with two, every CTA
+// re-reads 82 KB of X from L2, so from 17 rows on the split-K dec_gemm path is used).
+constexpr int WGEMM_MAX_ROWS = 16;
 
 static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const VocabIds& vi, int nsplit, bool align_mode) {
   const int d = c->d, H = c->H, ff = 4 * c->d, R = B * Kr;
@@ -1099,62 +1061,19 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
   const long slot_sz = (long)S_ENC * d;
   PdlScope pdl(true);   // every kernel of the step is launched as a programmatic dependent of its predecessor
   decoder_embed(st, s, c->emb, c->pos_dec, c->dx, R, d);
-  auto swap_gemm = [&](const __half* W, int n_out, int K, const __half* X, GemmEpilogue e) {
-    e.ldm = 1;
-    e.bias_on_m = 1;
-    gemm_tn(st, opnd(W, n_out, K, K), opnd(X, R, K, K), n_out, R, K, e);
-  };
-  static const bool splitk = [] { const char* e = getenv("WLB200_SPLITK"); return e ? atoi(e) != 0 : true; }();
   // Decode GEMMs are weight-streaming (M = out features, N = rows <= 256): K is split over enough CTAs to fill the
   // SMs; every K range stores its raw fp32 partial sum and the CONSUMER (LayerNorm, attention, GELU) adds the
   // ranges and the bias in a fixed order -- no atomics, bit-reproducible, and no separate reduction kernel.
   // part1 holds activations (qkv, q_cross, fc1), part2 the residual updates (out-proj, fc2) until the next LayerNorm.
-  // WLB200_FUSE_POST=1 (default OFF): run the LayerNorm-update after out-proj / FC2 and the GELU-cast after FC1 inside
-  // the producing split-K GEMM behind a grid barrier (13 -> 9 launches per layer).  The barrier gates every CTA on the
-  // slowest one and the row work then runs on fewer CTAs than the separate kernels chained by programmatic dependent
-  // launch get.
-  static const bool fuse_env = fuse_post_env();
-  static const bool simt_env = [] { const char* e = getenv("WLB200_GEMM_SIMT"); return e && atoi(e) != 0; }();
-  const bool fuse = fuse_env && splitk && !simt_env;
-  struct Post { int kind = GEMM_POST_NONE; const float* g = nullptr; const float* b = nullptr; };
-  auto part_gemm = [&](const __half* W, int n_out, int K, const __half* X, float* buf, const float* bias, Post post,
+  auto part_gemm = [&](const __half* W, int n_out, int K, const __half* X, float* buf, const float* bias,
                        int max_split = 8) -> PartialSrc {
-    GemmEpilogue e;
-    e.out = buf; e.out_f32 = 1; e.ldn = n_out; e.ldm = 1;
-    e.a_static = 1;
     PartialSrc ps;
     ps.ptr = buf; ps.bias = bias; ps.stride = (long)c->Rm * n_out;
-    if (splitk) {
-      int s2 = std::min(gemm_split_plan(n_out, R, K), max_split);
-      const int total_kb = cdiv(K, 64);
-      while (s2 > 1 && cdiv(total_kb, cdiv(total_kb, s2)) != s2) --s2;   // every K range must be non-empty
-      ps.nsplit = s2;
-      e.partials = ps.nsplit; e.part_stride = ps.stride;
-    } else {
-      ps.nsplit = 1;   // single pass, bias still added by the consumer
-    }
-    static const bool compact = [] { const char* e2 = getenv("WLB200_DEC_GEMM"); return e2 ? atoi(e2) != 0 : true; }();
-    if (compact && splitk && post.kind == GEMM_POST_NONE && !simt_env) {
-      ps.nsplit = dec_gemm_split_plan(n_out, R, K, max_split);
-      dec_gemm(st, W, n_out, K, X, R, buf, n_out, ps.stride, ps.nsplit);
-      // WLB200_DUP=1 (experiment): launch every decode GEMM twice (idempotent) -- the second launch finds its code in
-      // the instruction caches; the in-graph timeline shows what a warm launch of the same kernel costs
-      static const bool dup = [] { const char* e2 = getenv("WLB200_DUP"); return e2 && atoi(e2) != 0; }();
-      if (dup) dec_gemm(st, W, n_out, K, X, R, buf, n_out, ps.stride, ps.nsplit);
-      return ps;
-    }
-    if (post.kind != GEMM_POST_NONE) {
-      e.post = post.kind;
-      e.post_bias = bias;
-      e.post_bar = c->post_bar;
-      if (post.kind == GEMM_POST_LN) { e.post_x = c->dx; e.post_g = post.g; e.post_b = post.b; e.post_y = c->dxn; }
-      else e.post_y = c->dh;
-    }
-    gemm_tn(st, opnd(W, n_out, K, K), opnd(X, R, K, K), n_out, R, K, e);
+    ps.nsplit = dec_gemm_split_plan(n_out, R, K, max_split);
+    dec_gemm(st, W, n_out, K, X, R, buf, n_out, ps.stride, ps.nsplit);
     return ps;
   };
-  auto ln_post = [&](const float* g, const float* b) { Post p; if (fuse) { p.kind = GEMM_POST_LN; p.g = g; p.b = b; } return p; };
-  PartialSrc pending;   // residual update not yet folded into x (unfused path)
+  PartialSrc pending;   // residual update not yet folded into x
   auto cross = [&](int l, const PartialSrc& qc) {
     CrossAttnWorkspace ws = c->xws;
     ws.probs = align_mode ? c->align_probs : nullptr;
@@ -1173,39 +1092,18 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
     if (align_mode)
       gather_align_probs(st, s, c->align_probs, c->align_buf, c->align_heads_dev, (int)c->align_heads.size() / 2, l, B, Kr, H);
   };
-  // Small batches (R <= 32 decoder rows, e.g. 4-8 streams per GPU with beam 4): every linear layer is one wgemm launch
-  // whose epilogue writes FINAL values (bias, residual, GELU fused), so LayerNorm / attention read one value instead of
-  // summing partials and the GELU-cast launch is gone: 12 launches per layer instead of 13, each a fraction of the code.
-  static const bool wg_env = [] { const char* e = getenv("WLB200_WGEMM"); return e ? atoi(e) != 0 : true; }();
-  // (one m16 tile only: with two, every CTA re-reads 82 KB of X from L2; rows
-  // 17..32 take the wgmma path below until the K split moves into a cluster)
-  static const int wg_max_rows = [] { const char* e = getenv("WLB200_WGEMM_ROWS"); return e ? atoi(e) : 16; }();
-  const bool use_wg = wg_env && R <= wg_max_rows && wgemm_supported(R, d) && wgemm_supported(R, ff);
-  // Above that: split-K partials summed by the consumers (13 launches per layer), or with WLB200_CGEMM=1 cgemm, the
-  // wgmma pipeline with the K split inside a cluster (dec_gemm.cu) -- same fused epilogues as wgemm, 12 launches.
-  const bool cg_env = cgemm_enabled();
-  const bool small = !simt_env && !fuse && (use_wg || cg_env);
+  // Small batches (R <= WGEMM_MAX_ROWS decoder rows, e.g. 4 streams per GPU with beam 4): every linear layer is one wgemm
+  // launch whose epilogue writes FINAL values (bias, residual, GELU fused), so LayerNorm / attention read one value instead
+  // of summing partials and the GELU-cast launch is gone: 12 launches per layer instead of 13, each a fraction of the code.
+  const bool small = R <= WGEMM_MAX_ROWS && wgemm_supported(R, d) && wgemm_supported(R, ff);
   auto plain = [](const float* ptr) { PartialSrc ps; ps.ptr = ptr; ps.nsplit = 1; ps.stride = 0; ps.bias = nullptr; return ps; };
   // mode 0: out_f32 = X W^T + bias; 1: out_f32 += X W^T + bias; 2: out_f16 = gelu(X W^T + bias)
   auto lin = [&](const __half* W, int n_out, int K, const __half* X, const float* bias, int mode, float* of32, __half* of16) {
-    if (use_wg) wgemm(st, W, n_out, K, X, R, bias, mode, of32, of16, 0);
-    else cgemm(st, W, n_out, K, X, R, bias, mode, of32, of16);
+    wgemm(st, W, n_out, K, X, R, bias, mode, of32, of16, 0);
   };
-  // WLB200_XA_PREFETCH=n: the layer's first LayerNorm also asks L2 for the encoder K/V of the first n live streams --
-  // the six latency-bound kernels between it and the cross-attention leave HBM idle, the cross-attention is HBM-bound
-  const int xa_pf = xa_prefetch_streams();
-  L2Prefetch pf;
-  if (xa_pf > 0 && !align_mode) {
-    pf.slot = s.slot; pf.done = s.done; pf.B = B;
-    pf.slot_bytes = slot_sz * 2;
-    const long per_region = (pf.slot_bytes + 32 * 1024 - 1) / (32 * 1024);
-    pf.n_streams = (int)std::min<long>(std::min(xa_pf, B), (long)R * 32 / (2 * per_region));   // one 32 KB piece per lane of warp 0
-  }
   for (int l = 0; small && l < c->Ld; ++l) {
     const DecLayer& L = c->dec[l];
-    pf.k = c->ckv + ((long)l * 2 + 0) * c->NS * slot_sz;
-    pf.v = c->ckv + ((long)l * 2 + 1) * c->NS * slot_sz;
-    layernorm_update_rows(st, c->dx, pending, L.ln1_g, L.ln1_b, c->dxn, R, d, &pf);
+    layernorm_update_rows(st, c->dx, pending, L.ln1_g, L.ln1_b, c->dxn, R, d);
     lin(L.w_qkv, 3 * d, d, c->dxn, L.b_qkv, 0, c->part1, nullptr);
     decoder_self_attn(st, s, plain(c->part1), c->kcache + (long)l * c->cache_layer_stride, c->vcache + (long)l * c->cache_layer_stride,
                       c->cache_row_stride, c->datt, R, H, d);
@@ -1216,7 +1114,7 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
     lin(L.w_oc, d, d, c->datt, L.b_oc, 1, c->dx, nullptr);
     layernorm_update_rows(st, c->dx, PartialSrc(), L.ln3_g, L.ln3_b, c->dxn, R, d);
     lin(L.w_fc1, ff, d, c->dxn, L.b_fc1, 2, nullptr, c->dh);
-    const int ks2 = use_wg ? wgemm_ksplit(ff) : 1;
+    const int ks2 = wgemm_ksplit(ff);
     if (ks2 == 1) {
       lin(L.w_fc2, d, ff, c->dh, L.b_fc2, 1, c->dx, nullptr);
       pending = PartialSrc();
@@ -1227,40 +1125,22 @@ static void decode_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const Vo
   }
   for (int l = 0; !small && l < c->Ld; ++l) {
     const DecLayer& L = c->dec[l];
-    const bool last = l + 1 == c->Ld;
-    pf.k = c->ckv + ((long)l * 2 + 0) * c->NS * slot_sz;
-    pf.v = c->ckv + ((long)l * 2 + 1) * c->NS * slot_sz;
-    if (!fuse || l == 0) layernorm_update_rows(st, c->dx, pending, L.ln1_g, L.ln1_b, c->dxn, R, d, &pf);
-    const PartialSrc qkv = part_gemm(L.w_qkv, 3 * d, d, c->dxn, c->part1, L.b_qkv, Post());
+    layernorm_update_rows(st, c->dx, pending, L.ln1_g, L.ln1_b, c->dxn, R, d);
+    const PartialSrc qkv = part_gemm(L.w_qkv, 3 * d, d, c->dxn, c->part1, L.b_qkv);
     decoder_self_attn(st, s, qkv, c->kcache + (long)l * c->cache_layer_stride, c->vcache + (long)l * c->cache_layer_stride,
                       c->cache_row_stride, c->datt, R, H, d);
-    pending = part_gemm(L.w_o, d, d, c->datt, c->part2, L.b_o, ln_post(L.ln2_g, L.ln2_b));
-    if (!fuse) layernorm_update_rows(st, c->dx, pending, L.ln2_g, L.ln2_b, c->dxn, R, d);
-    const PartialSrc qc = part_gemm(L.w_qc, d, d, c->dxn, c->part1, L.b_qc, Post(), 4);   // cross-attention sums <= 4 ranges
+    pending = part_gemm(L.w_o, d, d, c->datt, c->part2, L.b_o);
+    layernorm_update_rows(st, c->dx, pending, L.ln2_g, L.ln2_b, c->dxn, R, d);
+    const PartialSrc qc = part_gemm(L.w_qc, d, d, c->dxn, c->part1, L.b_qc, 4);   // cross-attention sums <= 4 ranges
     cross(l, qc);
-    pending = part_gemm(L.w_oc, d, d, c->datt, c->part2, L.b_oc, ln_post(L.ln3_g, L.ln3_b));
-    if (!fuse) layernorm_update_rows(st, c->dx, pending, L.ln3_g, L.ln3_b, c->dxn, R, d);
-    Post gp;
-    if (fuse) gp.kind = GEMM_POST_GELU;
-    const PartialSrc h1 = part_gemm(L.w_fc1, ff, d, c->dxn, c->part1, L.b_fc1, gp);
-    if (!fuse) gelu_cast(st, h1, c->dh, R, ff);
-    // FC2's fused LayerNorm is the NEXT layer's ln1 (or the final LayerNorm after the last layer)
-    pending = part_gemm(L.w_fc2, d, ff, c->dh, c->part2, L.b_fc2,
-                        last ? ln_post(c->lnf_g, c->lnf_b) : ln_post(c->dec[l + 1].ln1_g, c->dec[l + 1].ln1_b));
+    pending = part_gemm(L.w_oc, d, d, c->datt, c->part2, L.b_oc);
+    layernorm_update_rows(st, c->dx, pending, L.ln3_g, L.ln3_b, c->dxn, R, d);
+    const PartialSrc h1 = part_gemm(L.w_fc1, ff, d, c->dxn, c->part1, L.b_fc1);
+    gelu_cast(st, h1, c->dh, R, ff);
+    pending = part_gemm(L.w_fc2, d, ff, c->dh, c->part2, L.b_fc2);
   }
-  if (!fuse) layernorm_update_rows(st, c->dx, pending, c->lnf_g, c->lnf_b, c->dxn, R, d);
-  {
-    static const bool compact = [] { const char* e2 = getenv("WLB200_DEC_GEMM"); return e2 ? atoi(e2) != 0 : true; }();
-    if (compact && !simt_env) {
-      dec_gemm(st, c->emb, c->V, d, c->dxn, R, c->logits, c->Vld, 0, 1);
-    } else {
-      GemmEpilogue e;
-      e.out = c->logits; e.out_f32 = 1; e.ldn = c->Vld;
-      e.ldm = 1;
-      e.a_static = 1;
-      gemm_tn(st, opnd(c->emb, c->V, d, d), opnd(c->dxn, R, d, d), c->V, R, d, e);
-    }
-  }
+  layernorm_update_rows(st, c->dx, pending, c->lnf_g, c->lnf_b, c->dxn, R, d);
+  dec_gemm(st, c->emb, c->V, d, c->dxn, R, c->logits, c->Vld, 0, 1);
   search_rows(st, s, c->logits, so, vi, R);
   search_streams(st, s, so, vi, B);
 }
@@ -1578,51 +1458,39 @@ static void emit_hyps(int NH, float length_penalty, int count, const int* h_len,
   }
 }
 
-// The captured decode step for one call shape (cached per context).  loop_graph: a conditional WHILE node whose body is
-// the step + loop_condition (the whole token loop is one launch); else the plain step.  `tag` separates the graphs of the
-// one-shot state ("g") from those of the decode session ("s"): the captures bake the state's device pointers in.
+// The captured token loop for one call shape (cached per context): a conditional WHILE node whose body is the decode
+// step + loop_condition, so the whole loop is one launch.  `tag` separates the graphs of the one-shot state ("g") from
+// those of the decode session ("s"): the captures bake the state's device pointers in.
 static cudaGraphExec_t decode_graph(wl_ctx* c, const char* tag, int B, int Kr, int K, const SearchOpts& so, const VocabIds& vi,
-                                    int nsplit, bool loop_graph, long* kernels) {
+                                    int nsplit, long* kernels) {
   cudaStream_t st = c->st;
   char key[160];
-  snprintf(key, sizeof(key), "%s/%d/%d/%d/%d/%d/%d/%d/%d", tag, B, Kr, K, so.max_cand, so.suppress_blank, so.max_initial_ts,
-           loop_graph ? 1 : 0, xa_prefetch_streams() * 2 + (cgemm_enabled() ? 1 : 0));
+  snprintf(key, sizeof(key), "%s/%d/%d/%d/%d/%d/%d", tag, B, Kr, K, so.max_cand, so.suppress_blank, so.max_initial_ts);
   GraphEntry& ge = c->graphs[key];
   if (!ge.exec) {
-    const long before = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + cgemm_launch_count() + other_launch_count();
+    const long before = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + other_launch_count();
     cudaGraph_t g = nullptr, cap = nullptr;
-    if (loop_graph) {
-      WL_CUDA(cudaGraphCreate(&g, 0));
-      cudaGraphConditionalHandle h;
-      WL_CUDA(cudaGraphConditionalHandleCreate(&h, g, 1, cudaGraphCondAssignDefault));
-      cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
-      np.conditional.handle = h;
-      np.conditional.type = cudaGraphCondTypeWhile;
-      np.conditional.size = 1;
-      cudaGraphNode_t node;
-      WL_CUDA(cudaGraphAddNode(&node, g, nullptr, 0, &np));
-      cudaGraph_t body = np.conditional.phGraph_out[0];
-      WL_CUDA(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
-      try {
-        decode_step(c, B, Kr, so, vi, nsplit, false);
-        loop_condition(st, c->ds, h, B);
-      } catch (...) {
-        cudaStreamEndCapture(st, &cap);
-        cudaGraphDestroy(g);
-        throw;
-      }
-      WL_CUDA(cudaStreamEndCapture(st, &cap));
-    } else {
-      WL_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-      try {
-        decode_step(c, B, Kr, so, vi, nsplit, false);
-      } catch (...) {
-        cudaStreamEndCapture(st, &g);
-        throw;
-      }
-      WL_CUDA(cudaStreamEndCapture(st, &g));
+    WL_CUDA(cudaGraphCreate(&g, 0));
+    cudaGraphConditionalHandle h;
+    WL_CUDA(cudaGraphConditionalHandleCreate(&h, g, 1, cudaGraphCondAssignDefault));
+    cudaGraphNodeParams np = {cudaGraphNodeTypeConditional};
+    np.conditional.handle = h;
+    np.conditional.type = cudaGraphCondTypeWhile;
+    np.conditional.size = 1;
+    cudaGraphNode_t node;
+    WL_CUDA(cudaGraphAddNode(&node, g, nullptr, 0, &np));
+    cudaGraph_t body = np.conditional.phGraph_out[0];
+    WL_CUDA(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
+    try {
+      decode_step(c, B, Kr, so, vi, nsplit, false);
+      loop_condition(st, c->ds, h, B);
+    } catch (...) {
+      cudaStreamEndCapture(st, &cap);
+      cudaGraphDestroy(g);
+      throw;
     }
-    ge.kernels = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + cgemm_launch_count() + other_launch_count() - before;
+    WL_CUDA(cudaStreamEndCapture(st, &cap));
+    ge.kernels = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + other_launch_count() - before;
     c->capture_counted += ge.kernels;
     WL_CUDA(cudaGraphInstantiate(&ge.exec, g, 0));
     cudaGraphDestroy(g);
@@ -1664,10 +1532,9 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
   int max_new = 0;
   int max_steps = upload_streams(c, slots, B, prompts, prompt_off, o->max_length, false, sample, o->sampling_temperature, o->seed, Kr,
                                  o->max_length_per_stream, &max_new);
-  // K8: every prompt position but the last goes through the decoder in ONE batched pass (WLB200_PREFILL=0: one decode
-  // step per prompt token, the round-1 behaviour)
-  static const bool prefill_env = [] { const char* e = getenv("WLB200_PREFILL"); return e ? atoi(e) != 0 : true; }();
-  const bool prefilled = o->prefill == 1 || (o->prefill == 0 && prefill_env);
+  // K8: every prompt position but the last goes through the decoder in ONE batched pass (prefill = 2: one decode step per
+  // prompt token)
+  const bool prefilled = o->prefill == 0 || o->prefill == 1;
   if (prefilled) max_steps = max_new;
   WL_CUDA(cudaMemcpyAsync(c->suppress_mask, mask.data(), nwords * 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaEventRecord(c->ev0, st));
@@ -1683,20 +1550,15 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
 
   // The whole token loop is ONE graph launch: a conditional WHILE node whose body is the captured decode step; the
   // body's last kernel (loop_condition) keeps the loop alive while some stream is still decoding and the step budget
-  // lasts.  No host round trip per token (round 1 synchronised every 4 steps), no wasted steps after the last EOT.
-  // WLB200_LOOP_GRAPH=0 falls back to one graph launch per step with a host check every 4 steps.
-  static const bool loop_graph = [] { const char* e = getenv("WLB200_LOOP_GRAPH"); return e ? atoi(e) != 0 : true; }();
+  // lasts.  No host round trip per token, no wasted steps after the last EOT.  Without graphs (use_cuda_graph = 0) the
+  // host launches the steps itself and checks for the end every 4 steps.
   cudaGraphExec_t exec = nullptr;
   long graph_kernels = 0;
-  bool is_loop = false;
-  if (o->use_cuda_graph) {
-    exec = decode_graph(c, "g", B, Kr, K, so, vi, nsplit, loop_graph, &graph_kernels);
-    is_loop = loop_graph;
-  }
+  if (o->use_cuda_graph) exec = decode_graph(c, "g", B, Kr, K, so, vi, nsplit, &graph_kernels);
   ensure_host(c, (size_t)B * (T_MAX + 16) + (size_t)B * MAX_HYPS * (T_MAX + 2) + 64, (size_t)B * (MAX_HYPS + 2));
   int* h_done = c->h_int;  // reuse (prompts are already on the device: the copies above are stream-ordered)
   WL_CUDA(cudaStreamSynchronize(st));
-  if (is_loop) {
+  if (exec) {
     h_done[0] = max_steps;
     WL_CUDA(cudaMemcpyAsync(c->ds.steps_left, h_done, sizeof(int), cudaMemcpyHostToDevice, st));
     WL_CUDA(cudaGraphLaunch(exec, st));
@@ -1708,14 +1570,7 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
     const int check_every = 4;
     while (ran < max_steps) {
       const int n = std::min(check_every, max_steps - ran);
-      for (int i = 0; i < n; ++i) {
-        if (exec) {
-          WL_CUDA(cudaGraphLaunch(exec, st));
-          c->graph_launched += graph_kernels;
-        } else {
-          decode_step(c, B, Kr, so, vi, nsplit, false);
-        }
-      }
+      for (int i = 0; i < n; ++i) decode_step(c, B, Kr, so, vi, nsplit, false);
       ran += n;
       WL_CUDA(cudaMemcpyAsync(h_done, c->ds.n_done, sizeof(int), cudaMemcpyDeviceToHost, st));
       WL_CUDA(cudaStreamSynchronize(st));
@@ -1921,7 +1776,7 @@ extern "C" int wl_session_run(wl_ctx* c, int32_t max_steps, int32_t break_on_fin
     WL_CUDA(cudaEventRecord(c->ev0, st));
     if (ss.use_graph) {
       long kernels = 0;
-      cudaGraphExec_t exec = decode_graph(c, "s", cap, ss.Kr, ss.K, ss.so, vi, ss.nsplit, true, &kernels);
+      cudaGraphExec_t exec = decode_graph(c, "s", cap, ss.Kr, ss.K, ss.so, vi, ss.nsplit, &kernels);
       WL_CUDA(cudaGraphLaunch(exec, st));
       WL_CUDA(cudaMemcpyAsync(h + 4, c->ds.steps_left, 4, cudaMemcpyDeviceToHost, st));
       WL_CUDA(cudaMemcpyAsync(h + 8, c->ds.done, (size_t)cap * 4, cudaMemcpyDeviceToHost, st));
@@ -2314,14 +2169,12 @@ extern "C" int wl_gemm_variant(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32
 extern "C" int wl_test_wgemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x_f16, const float* bias, float* out, int32_t R,
                              int32_t n_out, int32_t K, int32_t mode) {
   API_BEGIN(c)
-  const bool clustered = (mode & 8) != 0;   // modes 8, 9, 10: the cluster split-K GEMM (cgemm) with epilogue 0, 1, 2
-  mode &= 7;
-  WL_CHECK(w_f16 && x_f16 && out && mode >= 0 && mode <= (clustered ? 2 : 3), WL_ERR_ARG, "wl_test_wgemm: bad arguments");
-  WL_CHECK(clustered || wgemm_supported(R, K), WL_ERR_ARG, "wl_test_wgemm: unsupported shape R=%d K=%d", R, K);
+  WL_CHECK(w_f16 && x_f16 && out && mode >= 0 && mode <= 3, WL_ERR_ARG, "wl_test_wgemm: bad arguments");
+  WL_CHECK(wgemm_supported(R, K), WL_ERR_ARG, "wl_test_wgemm: unsupported shape R=%d K=%d", R, K);
   __half *dw = nullptr, *dx = nullptr, *dh = nullptr;
   float *db = nullptr, *dout = nullptr;
   const size_t nw = (size_t)n_out * K, nx = (size_t)R * K, no = (size_t)R * n_out;
-  const int ks = clustered ? 1 : wgemm_ksplit(K);
+  const int ks = wgemm_ksplit(K);
   WL_CUDA(cudaMalloc((void**)&dw, nw * 2));
   WL_CUDA(cudaMalloc((void**)&dx, nx * 2));
   WL_CUDA(cudaMalloc((void**)&dh, no * 2));
@@ -2334,8 +2187,7 @@ extern "C" int wl_test_wgemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x
     if (mode == 1) WL_CUDA(cudaMemcpy(dout, out, no * 4, cudaMemcpyHostToDevice));
     if (bias) WL_CUDA(cudaMemcpy(db, bias, (size_t)n_out * 4, cudaMemcpyHostToDevice));
     WL_CUDA(cudaDeviceSynchronize());
-    if (clustered) cgemm(c->st, dw, n_out, K, dx, R, bias ? db : nullptr, mode, dout, dh);
-    else wgemm(c->st, dw, n_out, K, dx, R, bias ? db : nullptr, mode, dout, dh, (long)no);
+    wgemm(c->st, dw, n_out, K, dx, R, bias ? db : nullptr, mode, dout, dh, (long)no);
     WL_CUDA(cudaStreamSynchronize(c->st));
     if (mode == 2) {
       std::vector<__half> h(no);

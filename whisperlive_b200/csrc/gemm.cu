@@ -24,9 +24,7 @@ struct GemmKParams {
   int a_pos[3], b_pos[3];  // tensor-map coordinate slots (1..3) of (row, i1, i2)
   GemmEpilogue e;
   int vec_ok;  // row-major output, 16-byte aligned rows: use vector stores
-  int nz;           // batch entries (or K splits in accum mode): tiles = tiles_m * tiles_n * nz
-  int accum;        // 1: grid z enumerates K ranges; range s stores its partial sum at out + s * part_stride
-  int kb_per_split; // k-blocks per split (accum mode)
+  int nz;           // batch entries: tiles = tiles_m * tiles_n * nz
   int n_fastest;    // tile order, see tile_decode()
 };
 
@@ -37,24 +35,12 @@ constexpr int A_STAGE_BYTES = BM * BK * 2;
 // Epilogue kinds are compile-time so that every kernel instantiation carries exactly one, compact epilogue: the
 // decode-step GEMMs run ~200 times per step on a few CTAs each, where instruction fetch of a fat multi-path
 // epilogue costs more than its arithmetic.
-enum EpiKind : int { EPI_ROW = 0, EPI_COL = 1, EPI_PART = 2, EPI_HEADSPLIT = 3 };
+enum EpiKind : int { EPI_ROW = 0, EPI_COL = 1, EPI_HEADSPLIT = 2 };
 
 template <int cnt, int KIND>
-__device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int n0, const uint32_t (&v)[cnt], int i1, int i2,
-                                               int split = 0) {
+__device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int n0, const uint32_t (&v)[cnt], int i1, int i2) {
   const GemmEpilogue& e = p.e;
   if (m >= p.M) return;
-  if constexpr (KIND == EPI_PART) {
-    // split-K: K range `split` stores its raw fp32 partial sum; whoever consumes the result adds the ranges
-    // (and the bias) in a fixed order -- no atomics, bit-reproducible.
-    float* dst = (float*)e.out + (long)split * e.part_stride + m * e.ldm;
-#pragma unroll
-    for (int i = 0; i < cnt; ++i) {
-      const int n = n0 + i;
-      if (n < p.N) dst[(long)n * e.ldn] = __uint_as_float(v[i]);
-    }
-    return;
-  }
   if constexpr (KIND == EPI_HEADSPLIT && cnt >= 8) {
     // m = (b, s), n = (h, dd); one thread writes cnt (<=32) consecutive dd of one head row.  The 16-byte pieces of a
     // 128-byte key row are stored XOR-swizzled by (s & 7): the layout ldmatrix wants in the cross-attention kernel.
@@ -198,126 +184,6 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
   }
 }
 
-// Sense-reversing grid barrier for a grid whose CTAs are all resident; called by ONE thread per CTA.
-__device__ __forceinline__ unsigned ld_acquire_u32(const unsigned* p) {
-  unsigned v;
-  asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-  return v;
-}
-__device__ __forceinline__ void grid_barrier(unsigned* bar, unsigned nblocks) {
-  const unsigned gen = ld_acquire_u32(bar + 1);
-  __threadfence();
-  if (atomicAdd(bar, 1u) == nblocks - 1u) {
-    atomicExch(bar, 0u);
-    __threadfence();
-    atomicAdd(bar + 1, 1u);
-  } else {
-    while (ld_acquire_u32(bar + 1) == gen) __nanosleep(20);
-  }
-  __threadfence();
-}
-template <int NT>
-__device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 3, %0;" ::"n"(NT) : "memory"); }
-
-// Row-wise consumer of the split-K partial sums, run by the NT epilogue threads of every CTA after the grid barrier
-// (same arithmetic, in the same order, as layernorm_update_kernel / gelu_cast_kernel).
-template <int NT>
-__device__ __forceinline__ void post_op(const GemmKParams& p, int te, float* red /*[16]*/) {
-  const GemmEpilogue& e = p.e;
-  const int S = e.partials, R = p.N, F = p.M;   // K ranges, rows, features
-  const float* part = reinterpret_cast<const float*>(e.out);
-  if (e.post == GEMM_POST_LN) {
-    const int n4 = F >> 2;
-    const float4* g4 = reinterpret_cast<const float4*>(e.post_g);
-    const float4* b4 = reinterpret_cast<const float4*>(e.post_b);
-    for (int r = blockIdx.x; r < R; r += gridDim.x) {
-      float4* x4 = reinterpret_cast<float4*>(e.post_x + (long)r * F);
-      constexpr int PER = 3;   // float4 per thread: d <= 4 * PER * NT
-      float4 v[PER];
-      float sum = 0.f;
-#pragma unroll
-      for (int i = 0; i < PER; ++i) {
-        const int c = i * NT + te;
-        v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (c < n4) {
-          if (e.post_bias) v[i] = __ldg(reinterpret_cast<const float4*>(e.post_bias) + c);
-          const float4 a = x4[c];
-          v[i].x += a.x; v[i].y += a.y; v[i].z += a.z; v[i].w += a.w;
-        }
-      }
-#pragma unroll 8
-      for (int sp = 0; sp < S; ++sp) {
-        const float4* p4 = reinterpret_cast<const float4*>(part + (long)sp * e.part_stride + (long)r * F);
-#pragma unroll
-        for (int i = 0; i < PER; ++i) {
-          const int c = i * NT + te;
-          if (c < n4) {
-            const float4 q = __ldcg(p4 + c);
-            v[i].x += q.x; v[i].y += q.y; v[i].z += q.z; v[i].w += q.w;
-          }
-        }
-      }
-#pragma unroll
-      for (int i = 0; i < PER; ++i) {
-        const int c = i * NT + te;
-        if (c < n4) x4[c] = v[i];
-        sum += (v[i].x + v[i].y) + (v[i].z + v[i].w);
-      }
-      sum = warp_sum(sum);
-      if ((te & 31) == 0) red[te >> 5] = sum;
-      epi_sync<NT>();
-      float tot = 0.f;
-#pragma unroll
-      for (int w = 0; w < NT / 32; ++w) tot += red[w];
-      const float mean = tot / F;
-      float sq = 0.f;
-#pragma unroll
-      for (int i = 0; i < PER; ++i) {
-        if (i * NT + te < n4) {
-          const float a = v[i].x - mean, b2 = v[i].y - mean, c2 = v[i].z - mean, d2 = v[i].w - mean;
-          sq += (a * a + b2 * b2) + (c2 * c2 + d2 * d2);
-        }
-      }
-      sq = warp_sum(sq);
-      if ((te & 31) == 0) red[8 + (te >> 5)] = sq;
-      epi_sync<NT>();
-      float tq = 0.f;
-#pragma unroll
-      for (int w = 0; w < NT / 32; ++w) tq += red[8 + w];
-      const float rstd = rsqrtf(tq / F + 1e-5f);
-#pragma unroll
-      for (int i = 0; i < PER; ++i) {
-        const int c = i * NT + te;
-        if (c < n4) {
-          const float4 gg = g4[c], bb = b4[c];
-          __align__(8) __half2 h[2] = {
-              __floats2half2_rn((v[i].x - mean) * rstd * gg.x + bb.x, (v[i].y - mean) * rstd * gg.y + bb.y),
-              __floats2half2_rn((v[i].z - mean) * rstd * gg.z + bb.z, (v[i].w - mean) * rstd * gg.w + bb.w)};
-          *reinterpret_cast<uint2*>(e.post_y + (long)r * F + 4 * c) = *reinterpret_cast<const uint2*>(h);
-        }
-      }
-      epi_sync<NT>();   // red is reused by the next row
-    }
-  } else if (e.post == GEMM_POST_GELU) {
-    const int c4n = F >> 2;
-    const long total4 = (long)R * c4n;
-    const long st4 = e.part_stride >> 2;
-    for (long i4 = (long)blockIdx.x * NT + te; i4 < total4; i4 += (long)gridDim.x * NT) {
-      const int c = (int)(i4 % c4n);
-      float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (e.post_bias) v = __ldg(reinterpret_cast<const float4*>(e.post_bias) + c);
-      const float4* p4 = reinterpret_cast<const float4*>(part) + i4;
-#pragma unroll 4
-      for (int sp = 0; sp < S; ++sp) {
-        const float4 q = __ldcg(p4 + sp * st4);
-        v.x += q.x; v.y += q.y; v.z += q.z; v.w += q.w;
-      }
-      __align__(8) __half2 h[2] = {__floats2half2_rn(gelu_erf(v.x), gelu_erf(v.y)), __floats2half2_rn(gelu_erf(v.z), gelu_erf(v.w))};
-      *reinterpret_cast<uint2*>(e.post_y + 4 * i4) = *reinterpret_cast<const uint2*>(h);
-    }
-  }
-}
-
 // Tile order inside one batch entry.  m fastest: CTAs running side by side share the B tile (right when B is the big
 // operand).  n fastest (p.n_fastest): they share the A tile and sweep B -- right when B is a weight matrix that stays
 // in L2 anyway and A is a large activation (FC2 of the encoder: A = 123 MB would otherwise be re-read per n tile).
@@ -346,27 +212,22 @@ struct EpiStage {
 template <int BN, int STAGES>
 __host__ __device__ constexpr int gemm_smem_bytes() { return STAGES * (A_STAGE_BYTES + BN * BK * 2) + EpiStage<BN>::BYTES + 1024 + 512; }
 
-// Where tile t's operands and output sit: batch entry (i1, i2), K range [kb0, kb0 + num_kb) in k-blocks.
+// Where tile t's operands and output sit: tile (tile_m, tile_n) of batch entry (i1, i2).
 struct TileCoord {
-  int tile_m, tile_n, split, i1, i2, kb0, num_kb;
+  int tile_m, tile_n, i1, i2;
 };
-template <int KIND>
-__device__ __forceinline__ TileCoord tile_coord(const GemmKParams& p, int t, int tiles_m, int tiles_n, int total_kb) {
+__device__ __forceinline__ TileCoord tile_coord(const GemmKParams& p, int t, int tiles_m, int tiles_n) {
   TileCoord c;
-  int zz;
-  tile_decode(p, t, tiles_m, tiles_n, c.tile_m, c.tile_n, zz);
-  const int z = KIND == EPI_PART ? 0 : zz;
-  c.split = KIND == EPI_PART ? zz : 0;
+  int z;
+  tile_decode(p, t, tiles_m, tiles_n, c.tile_m, c.tile_n, z);
   c.i1 = z % p.zn1;
   c.i2 = z / p.zn1;
-  c.kb0 = KIND == EPI_PART ? c.split * p.kb_per_split : 0;
-  c.num_kb = KIND == EPI_PART ? min(p.kb_per_split, total_kb - c.kb0) : total_kb;
   return c;
 }
 
 // TMA producer (one elected thread): fills the stage ring with the k-blocks of this CTA's tiles t = blockIdx.x,
 // blockIdx.x + gridDim.x, ... in that order, each stage once its consumers have handed it back.
-template <int BN, int STAGES, int KIND>
+template <int BN, int STAGES>
 __device__ __forceinline__ void gemm_produce(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmKParams& p, uint8_t* sA,
                                              uint8_t* sB, uint64_t* full, uint64_t* empty, int tiles_m, int tiles_n,
                                              int total_tiles, int total_kb) {
@@ -379,39 +240,25 @@ __device__ __forceinline__ void gemm_produce(const CUtensorMap* tmA, const CUten
     return pos[0] == s ? row : (pos[1] == s ? j1 : (pos[2] == s ? j2 : 0));
   };
   for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-    const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
+    const TileCoord tc = tile_coord(p, t, tiles_m, tiles_n);
     const int a1 = p.a_batched ? tc.i1 : 0, a2 = p.a_batched ? tc.i2 : 0;
     const int b1 = p.b_batched ? tc.i1 : 0, b2 = p.b_batched ? tc.i2 : 0;
     const int ca1 = slot(p.a_pos, 1, tc.tile_m * BM, a1, a2), ca2 = slot(p.a_pos, 2, tc.tile_m * BM, a1, a2),
               ca3 = slot(p.a_pos, 3, tc.tile_m * BM, a1, a2);
     const int cb1 = slot(p.b_pos, 1, tc.tile_n * BN, b1, b2), cb2 = slot(p.b_pos, 2, tc.tile_n * BN, b1, b2),
               cb3 = slot(p.b_pos, 3, tc.tile_n * BN, b1, b2);
-    int pre = 0;
     if (first) {
-      // First tile of this CTA.  When A is a weight matrix (decode: swap-AB, A = W) its k-blocks are requested
-      // BEFORE the dependency wait, so the weight stream overlaps the tail of the kernel that produces B.
-      if (p.e.a_static) {
-        pre = min(tc.num_kb, STAGES);
-        for (int kb = 0; kb < pre; ++kb) {
-          mbar_expect_tx(&full[kb], A_STAGE_BYTES + B_STAGE_BYTES);
-          tma_load_4d(sA + kb * A_STAGE_BYTES, tmA, &full[kb], (tc.kb0 + kb) * BK, ca1, ca2, ca3);
-        }
-      }
-      if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 0);
+      if (blockIdx.x == 0) tl_stamp_any(TL_GEMM, 0);
       pdl_wait();
-      if (blockIdx.x == 0) tl_stamp_any(KIND == EPI_PART ? TL_GEMM_PART : TL_GEMM, 1);
+      if (blockIdx.x == 0) tl_stamp_any(TL_GEMM, 1);
       first = false;
     }
-    for (int kb = 0; kb < tc.num_kb; ++kb) {
-      const int k0 = (tc.kb0 + kb) * BK;
-      if (kb < pre) {
-        tma_load_4d(sB + stage * B_STAGE_BYTES, tmB, &full[stage], k0, cb1, cb2, cb3);
-      } else {
-        mbar_wait(&empty[stage], phase ^ 1);
-        mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
-        tma_load_4d(sA + stage * A_STAGE_BYTES, tmA, &full[stage], k0, ca1, ca2, ca3);
-        tma_load_4d(sB + stage * B_STAGE_BYTES, tmB, &full[stage], k0, cb1, cb2, cb3);
-      }
+    for (int kb = 0; kb < total_kb; ++kb) {
+      const int k0 = kb * BK;
+      mbar_wait(&empty[stage], phase ^ 1);
+      mbar_expect_tx(&full[stage], A_STAGE_BYTES + B_STAGE_BYTES);
+      tma_load_4d(sA + stage * A_STAGE_BYTES, tmA, &full[stage], k0, ca1, ca2, ca3);
+      tma_load_4d(sB + stage * B_STAGE_BYTES, tmB, &full[stage], k0, cb1, cb2, cb3);
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     }
   }
@@ -422,7 +269,7 @@ __device__ __forceinline__ void gemm_produce(const CUtensorMap* tmA, const CUten
 // bar_id: the warpgroup's own named barrier (128 threads).
 template <int BN, int KIND>
 __device__ __forceinline__ void epilogue_rows64(const GemmKParams& p, const float (&acc)[BN / 2], float* stg, int bar_id, long m0,
-                                                int n0, int i1, int i2, int split) {
+                                                int n0, int i1, int i2) {
   using ES = EpiStage<BN>;
   const int tw = threadIdx.x & 127;
   const int row = tw & 63, half = tw >> 6;
@@ -442,7 +289,7 @@ __device__ __forceinline__ void epilogue_rows64(const GemmKParams& p, const floa
       v[4 * i + 2] = __float_as_uint(q.z); v[4 * i + 3] = __float_as_uint(q.w);
     }
     named_bar_sync(bar_id, 128);   // the next chunk reuses the staging buffer
-    epilogue_chunk<CNT, KIND>(p, m0 + row, n0 + ch * ES::CH + half * CNT, v, i1, i2, split);
+    epilogue_chunk<CNT, KIND>(p, m0 + row, n0 + ch * ES::CH + half * CNT, v, i1, i2);
   }
 }
 
@@ -463,7 +310,6 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   float* stg_all = reinterpret_cast<float*>(sB + STAGES * B_STAGE_BYTES);
   uint64_t* full = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg_all) + ES::BYTES);
   uint64_t* empty = full + STAGES;
-  float* post_red = reinterpret_cast<float*>(empty + STAGES);   // [16]
 
   const int warp = threadIdx.x >> 5;
   const int tiles_m = (p.M + BM - 1) / BM, tiles_n = (p.N + BN - 1) / BN;
@@ -485,7 +331,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   __syncthreads();
 
   if (warp == 0) {
-    if (elect_one()) gemm_produce<BN, STAGES, KIND>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
+    if (elect_one()) gemm_produce<BN, STAGES>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
   } else if (warp >= 4) {
     const int wg = (warp >> 2) - 1;                  // consumer warpgroup: tile rows 64 wg .. 64 wg + 63
     float* stg = stg_all + wg * 64 * ES::LD;
@@ -493,12 +339,12 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     uint32_t phase = 0;
     pdl_wait();   // the residual / output buffers belong to the preceding kernels
     for (int t = blockIdx.x; t < total_tiles; t += gridDim.x) {
-      const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
+      const TileCoord tc = tile_coord(p, t, tiles_m, tiles_n);
       float acc[BN / 2];
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
       int prev = -1;
-      for (int kb = 0; kb < tc.num_kb; ++kb) {
+      for (int kb = 0; kb < total_kb; ++kb) {
         mbar_wait(&full[stage], phase);
         wgmma_fence();
         wgmma_tile_k64<BN>(acc, sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, wg, kb > 0);
@@ -512,18 +358,7 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       wgmma_wait<0>();
       wgmma_fence_regs(acc);
       if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
-      epilogue_rows64<BN, KIND>(p, acc, stg, 1 + wg, (long)tc.tile_m * BM + wg * 64, tc.tile_n * BN, tc.i1, tc.i2, tc.split);
-    }
-    if constexpr (KIND == EPI_PART) {
-      if (p.e.post != GEMM_POST_NONE) {
-        constexpr int NT = 256;                    // consumer threads
-        const int te = threadIdx.x - 128;
-        __threadfence();                           // this thread's partial sums are visible device-wide
-        epi_sync<NT>();
-        if (te == 0) grid_barrier(p.e.post_bar, gridDim.x);
-        epi_sync<NT>();
-        post_op<NT>(p, te, post_red);
-      }
+      epilogue_rows64<BN, KIND>(p, acc, stg, 1 + wg, (long)tc.tile_m * BM + wg * 64, tc.tile_n * BN, tc.i1, tc.i2);
     }
   }
 }
@@ -537,14 +372,13 @@ gemm_tn_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 // Registers: the producer warpgroup drops to PP_PRODUCER_REGS, the consumers (2 x 64 accumulators a thread) rise to
 // PP_CONSUMER_REGS; 128 x 40 + 256 x 232 <= 64 K.
 constexpr int PP_STAGES = 5;   // 5 x 32 KB ring + 2 x 17 KB staging: the most that fits 227 KB
-constexpr int PP_BAR = 4;      // named barriers 4, 5 (1, 2: per-warpgroup epilogue staging, 3: epi_sync)
+constexpr int PP_BAR = 4;      // named barriers 4, 5 (1, 2: per-warpgroup epilogue staging)
 constexpr int PP_PRODUCER_REGS = 40, PP_CONSUMER_REGS = 232;
 
 template <int KIND>
 __global__ void __launch_bounds__(384, 1)
 gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                      const __grid_constant__ GemmKParams p) {
-  static_assert(KIND != EPI_PART, "split-K partials stay on gemm_tn_kernel");
   constexpr int BN = 128, STAGES = PP_STAGES;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* base = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -578,7 +412,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   if (warp < 4) {
     setmaxnreg_dec<PP_PRODUCER_REGS>();
     if (warp == 0 && elect_one())
-      gemm_produce<BN, STAGES, KIND>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
+      gemm_produce<BN, STAGES>(&tmA, &tmB, p, sA, sB, full, empty, tiles_m, tiles_n, total_tiles, total_kb);
     return;
   }
   setmaxnreg_inc<PP_CONSUMER_REGS>();
@@ -587,7 +421,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
   pdl_wait();   // the residual / output buffers belong to the preceding kernels
   if (wg == 1) named_bar_arrive(PP_BAR, 256);   // warpgroup 0 takes the first tile (grid <= tiles: it exists)
   for (int j = wg, t = blockIdx.x + wg * gridDim.x; t < total_tiles; j += 2, t += 2 * gridDim.x) {
-    const TileCoord tc = tile_coord<KIND>(p, t, tiles_m, tiles_n, total_kb);
+    const TileCoord tc = tile_coord(p, t, tiles_m, tiles_n);
     // every tile has total_kb k-blocks: tile j starts at ring position j * total_kb
     const long it0 = (long)j * total_kb;
     int stage = (int)(it0 % STAGES);
@@ -599,7 +433,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
       for (int i = 0; i < BN / 2; ++i) acc[h][i] = 0.f;
     named_bar_sync(PP_BAR + wg, 256);   // our turn: the other warpgroup has issued all MMAs of tile j - 1
     int prev = -1;
-    for (int kb = 0; kb < tc.num_kb; ++kb) {
+    for (int kb = 0; kb < total_kb; ++kb) {
       mbar_wait(&full[stage], phase);
       wgmma_fence();
       wgmma_tile_k64<BN>(acc[0], sA + stage * A_STAGE_BYTES, sB + stage * B_STAGE_BYTES, 0, kb > 0);
@@ -617,7 +451,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_const
     if (prev >= 0 && lane_id() == 0) mbar_arrive(&empty[prev]);
 #pragma unroll
     for (int h = 0; h < 2; ++h)
-      epilogue_rows64<BN, KIND>(p, acc[h], stg, 1 + wg, (long)tc.tile_m * BM + h * 64, tc.tile_n * BN, tc.i1, tc.i2, 0);
+      epilogue_rows64<BN, KIND>(p, acc[h], stg, 1 + wg, (long)tc.tile_m * BM + h * 64, tc.tile_n * BN, tc.i1, tc.i2);
   }
 }
 
@@ -749,7 +583,6 @@ static void prime_pingpong() {
 void gemm_prime() {
   prime_kind<EPI_ROW>();
   prime_kind<EPI_COL>();
-  prime_kind<EPI_PART>();
   prime_kind<EPI_HEADSPLIT>();
   prime_pingpong<EPI_ROW>();
   prime_pingpong<EPI_COL>();
@@ -785,10 +618,8 @@ static GemmKParams make_params(const GemmOperand& A, const GemmOperand& B, int M
   *Z = za > zb ? za : zb;
   p.e = epi;
   p.vec_ok = 0;
-  p.accum = 0;
   // B (N x K halves) small enough to live in L2 while A is larger than B: sweep n fastest
   p.n_fastest = (zb == 1 && (long)N * K * 2 <= (24L << 20) && (long)M * K > (long)N * K) ? 1 : 0;
-  p.kb_per_split = 0;
   if (epi.mode == GEMM_STORE && epi.ldn == 1) {
     const int a = epi.out_f32 ? 4 : 8;  // elements per 16 bytes
     bool ok = ((uintptr_t)epi.out & 15) == 0 && epi.ldm % 8 == 0 && epi.ob1 % 8 == 0 && epi.ob2 % 8 == 0;
@@ -803,18 +634,6 @@ static GemmKParams make_params(const GemmOperand& A, const GemmOperand& B, int M
              "gemm_tn: bad head-split epilogue");
   }
   return p;
-}
-
-// Number of K ranges for a weight-streaming (swap-AB) GEMM so that tiles x ranges fills the SMs; always a value
-// gemm_tn accepts (every range non-empty).
-int gemm_split_plan(int M, int N, int K) {
-  static int sms = 0;
-  if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); }
-  const int bn = N <= 16 ? 16 : N <= 32 ? 32 : N <= 64 ? 64 : 128;
-  const int tiles = cdiv(N, bn) * cdiv(M, BM), total_kb = cdiv(K, BK);
-  int s = std::max(1, std::min(std::min(total_kb, 8), sms / std::max(1, tiles)));
-  const int kbs = cdiv(total_kb, s);
-  return cdiv(total_kb, kbs);
 }
 
 static int pick_bn(int N) {
@@ -837,47 +656,24 @@ GemmVariant gemm_tn_variant(int M, int N, int K, int Z) {
 
 void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K, const GemmEpilogue& epi,
              GemmVariant variant) {
-  static const int force_simt = env_int("WLB200_GEMM_SIMT", 0);
-  if (force_simt) return gemm_tn_simt(stream, A, B, M, N, K, epi);
   int Z;
   GemmKParams p = make_params(A, B, M, N, K, epi, &Z);
   int bn = pick_bn(N);
   if (epi.mode == GEMM_HEADSPLIT && bn < 64) bn = 64;
-  if (epi.partials > 0) {
-    WL_CHECK(Z == 1 && epi.out_f32 && !epi.gelu && !epi.resid && !epi.bias && epi.mode == GEMM_STORE, WL_ERR_ARG,
-             "gemm_tn: split-K partial output must be plain fp32 without bias");
-  } else {
-    WL_CHECK(epi.post == GEMM_POST_NONE, WL_ERR_ARG, "gemm_tn: a fused post-op needs the split-K partial output");
-  }
-  if (epi.partials > 0) {
-    if (epi.post != GEMM_POST_NONE) {
-      WL_CHECK(epi.post_bar && epi.post_y && M % 4 == 0 && epi.part_stride % 4 == 0 && epi.ldm == 1 && epi.ldn == M, WL_ERR_ARG,
-               "gemm_tn: fused post-op needs the [range][row][feature] partial layout");
-      WL_CHECK(epi.post != GEMM_POST_LN || (epi.post_x && epi.post_g && epi.post_b && M <= 4 * 3 * 128), WL_ERR_ARG,
-               "gemm_tn: fused LayerNorm supports rows of at most 1536 features");
-    }
-    const int total_kb = cdiv(K, BK);
-    p.accum = 1;
-    p.kb_per_split = cdiv(total_kb, epi.partials);
-    Z = cdiv(total_kb, p.kb_per_split);
-    WL_CHECK(Z == epi.partials, WL_ERR_ARG, "gemm_tn: %d K ranges cannot be formed from %d k-blocks (use gemm_split_plan)", epi.partials, total_kb);
-  }
   const TmapInfo ia = get_tmap(A, BM), ib = get_tmap(B, bn);
   const CUtensorMap& ta = ia.tm;
   const CUtensorMap& tb = ib.tm;
   for (int i = 0; i < 3; ++i) { p.a_pos[i] = ia.pos[i]; p.b_pos[i] = ib.pos[i]; }
-  bool pingpong = !p.accum && pingpong_pays(bn, (long)cdiv(M, BM) * cdiv(N, bn) * Z);
+  bool pingpong = pingpong_pays(bn, (long)cdiv(M, BM) * cdiv(N, bn) * Z);
   if (variant != GEMM_AUTO) {
-    WL_CHECK(variant == GEMM_CLASSIC || (!p.accum && bn == 128), WL_ERR_ARG,
-             "gemm_tn: the ping-pong kernel needs N tiles of 128 and no split-K");
+    WL_CHECK(variant == GEMM_CLASSIC || bn == 128, WL_ERR_ARG, "gemm_tn: the ping-pong kernel needs N tiles of 128");
     pingpong = variant == GEMM_PINGPONG;
   }
   if (pingpong) {
     if (epi.mode == GEMM_HEADSPLIT) launch_pingpong<EPI_HEADSPLIT>(stream, ta, tb, p, Z);
     else if (p.vec_ok) launch_pingpong<EPI_ROW>(stream, ta, tb, p, Z);
     else launch_pingpong<EPI_COL>(stream, ta, tb, p, Z);
-  } else if (p.accum) launch_kind<EPI_PART>(bn, stream, ta, tb, p, Z);
-  else if (epi.mode == GEMM_HEADSPLIT) launch_kind<EPI_HEADSPLIT>(bn, stream, ta, tb, p, Z);
+  } else if (epi.mode == GEMM_HEADSPLIT) launch_kind<EPI_HEADSPLIT>(bn, stream, ta, tb, p, Z);
   else if (p.vec_ok) launch_kind<EPI_ROW>(bn, stream, ta, tb, p, Z);
   else launch_kind<EPI_COL>(bn, stream, ta, tb, p, Z);
 }
@@ -896,11 +692,6 @@ __global__ void gemm_tn_simt_kernel(GemmOperand A, GemmOperand B, GemmKParams p)
   const int kk = ka < kb ? ka : kb;
   for (int k = 0; k < kk; ++k) acc = fmaf(__half2float(a[k]), __half2float(b[k]), acc);
   uint32_t v[1] = {__float_as_uint(acc)};
-  if (p.e.partials > 0) {  // same contract as the split-K path: range 0 carries the sum, the others zero
-    for (int sp = 0; sp < p.e.partials; ++sp)
-      ((float*)p.e.out)[(long)sp * p.e.part_stride + m * p.e.ldm + n * p.e.ldn] = sp == 0 ? acc : 0.f;
-    return;
-  }
   GemmKParams q = p;
   q.vec_ok = 0;
   if (q.e.mode == GEMM_HEADSPLIT) {

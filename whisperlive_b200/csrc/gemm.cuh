@@ -18,8 +18,6 @@ struct GemmOperand {
   long s2 = 0;
 };
 
-enum GemmPost : int { GEMM_POST_NONE = 0, GEMM_POST_LN = 1, GEMM_POST_GELU = 2 };
-
 enum GemmMode : int {
   GEMM_STORE = 0,      // out[z][m*ldm + n*ldn]
   GEMM_HEADSPLIT = 1,  // cross-KV cache layout: row m=(b,s), col n=(h,dd) -> out[slot[b]][h][s][dd]
@@ -35,21 +33,6 @@ struct GemmEpilogue {
   int gelu = 0;              // exact erf GELU after bias
   const float* resid = nullptr;  // fp32 residual added last; same indexing scheme as out
   long rldm = 0, rldn = 1, rb1 = 0, rb2 = 0;
-  int partials = 0;          // >0: split K into `partials` ranges; range s stores its raw fp32 partial sum at
-  long part_stride = 0;      //     out + s*part_stride (no bias); the consumer adds them in order (deterministic)
-  // Fused consumer of a split-K result (partials > 0 only): after its partial stores every CTA passes a grid-wide
-  // barrier (all CTAs are resident: the kernel is persistent) and the epilogue warps run the row-wise operation that
-  // would otherwise be the next kernel.  GEMM_POST_LN: x[r] += bias + sum_s partial_s[r]; y[r] = LayerNorm(x[r]) (fp16).
-  // GEMM_POST_GELU: y = gelu(bias + sum_s partial_s) (fp16).  Rows are the GEMM's n index (swap-AB), features its m.
-  int post = 0;
-  float* post_x = nullptr;
-  const float* post_bias = nullptr;
-  const float* post_g = nullptr;
-  const float* post_b = nullptr;
-  __half* post_y = nullptr;
-  unsigned* post_bar = nullptr;   // {arrival count, generation}, zero-initialised, one pair per context
-  int a_static = 0;          // A is a weight matrix: under programmatic dependent launch its first k-blocks are
-                             //     fetched before waiting for the preceding kernel (which only produces B)
   int mode = GEMM_STORE;
   // GEMM_HEADSPLIT parameters
   int hs_S = 0, hs_H = 0;
@@ -59,22 +42,20 @@ struct GemmEpilogue {
 
 // Which persistent wgmma kernel runs a GEMM (gemm.cu).  CLASSIC: both consumer warpgroups share each 128 x BN tile.
 // PINGPONG: each warpgroup owns whole 128 x 128 tiles and its epilogue overlaps the other's MMAs; chosen when every CTA
-// gets at least two tiles and there is no split-K.  AUTO picks from the shape; the others force one (tests).
+// gets at least two tiles.  AUTO picks from the shape; the others force one (tests).
 enum GemmVariant : int { GEMM_AUTO = 0, GEMM_CLASSIC = 1, GEMM_PINGPONG = 2 };
 
 // Launch on `stream`. M/N/K are the logical sizes per batch entry. Throws wl::Error.
 void gemm_tn(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K,
              const GemmEpilogue& epi, GemmVariant variant = GEMM_AUTO);
-// The variant GEMM_AUTO selects for a non-split-K GEMM of this shape (Z batch entries).
+// The variant GEMM_AUTO selects for a GEMM of this shape (Z batch entries).
 GemmVariant gemm_tn_variant(int M, int N, int K, int Z);
 
-// Plain CUDA-core reference of the same contract (debug/bisect aid on the GPU box, WLB200_GEMM=simt;
-// also what the GEMM unit test compares against on-device).
+// Plain CUDA-core reference of the same contract: what the GEMM unit test compares against on-device.
 void gemm_tn_simt(cudaStream_t stream, const GemmOperand& A, const GemmOperand& B, int M, int N, int K,
                   const GemmEpilogue& epi);
 
 long gemm_launch_count();
-int gemm_split_plan(int M, int N, int K);
 
 // Compact decode-step GEMM (dec_gemm.cu): out[s][r][ldn] (s < nsplit) = partial sums over K range s of
 // W[n_out, K] x X[R, K]^T, fp32, no bias.  nsplit from dec_gemm_split_plan (1 for the vocabulary projection).
@@ -84,20 +65,12 @@ int dec_gemm_split_plan(int n_out, int R, int K, int max_split = 8);
 long dec_gemm_launch_count();
 void dec_gemm_prime();
 void dec_gemm_tl_bind(unsigned long long* p);
-// The same pipeline with the K split inside a thread-block cluster and the reduction through distributed shared memory:
-// final values with the epilogue fused (mode 0: + bias; 1: out_f32 += acc + bias; 2: out_f16 = gelu(acc + bias)).
-void cgemm(cudaStream_t st, const __half* W, int n_out, int K, const __half* X, int R, const float* bias, int mode, float* out_f32,
-           __half* out_f16);
-int cgemm_split_plan(int n_out, int R, int K);
-long cgemm_launch_count();
-void cgemm_prime();
 
 // Small-batch decode GEMM with fused epilogue (wgemm.cu, R <= 32 rows, mma.sync + bulk-copied weight slices).
 // mode 0: out_f32 = acc + bias; 1: out_f32 += acc + bias (in place); 2: out_f16 = gelu(acc + bias);
 // 3: out_f32[ks] = raw partial sum of K range ks (only when K > 1280)
-// prefetch_ptr / prefetch_bytes: the weights of the next linear layer, requested into L2 by this launch (optional)
 void wgemm(cudaStream_t st, const __half* W, int n_out, int K, const __half* X, int R, const float* bias, int mode, float* out_f32,
-           __half* out_f16, long part_stride, const void* prefetch_ptr = nullptr, long prefetch_bytes = 0);
+           __half* out_f16, long part_stride);
 bool wgemm_supported(int R, int K);
 int wgemm_ksplit(int K);
 long wgemm_launch_count();

@@ -55,19 +55,9 @@ void gather_windows(cudaStream_t st, const float* mel, const long* mel_off, cons
 // y = LayerNorm(x) * gamma + beta ; x f32 [rows][d] -> y fp16 [rows][d] (and optionally f32 copy)
 void layernorm_rows(cudaStream_t st, const float* x, const float* gamma, const float* beta, __half* y, float* y32,
                     long rows, int d);
-// L2 prefetch request riding on a decode-step kernel: pull the encoder K/V (one layer) of the first n_streams LIVE
-// streams into L2 while the latency-bound kernels that precede the cross-attention leave HBM idle (engine.cu).
-struct L2Prefetch {
-  const __half* k = nullptr;   // layer base of the cross K pool [slot][H][1500][64]
-  const __half* v = nullptr;
-  const int* slot = nullptr;   // [B] pool slot of each stream
-  const int* done = nullptr;   // [B]
-  int B = 0, n_streams = 0;
-  long slot_bytes = 0;         // bytes of one stream's K (or V) for one layer
-};
 // decode step: x[r] += upd(r, :) (residual update pending from a split-K GEMM), then y = LayerNorm(x) as fp16
 void layernorm_update_rows(cudaStream_t st, float* x, const PartialSrc& upd, const float* gamma, const float* beta, __half* y,
-                           int rows, int d, const L2Prefetch* pf = nullptr);
+                           int rows, int d);
 // out[r][c] = fp16(gelu(in(r, c))), rows x cols (cols % 4 == 0)
 void gelu_cast(cudaStream_t st, const PartialSrc& in, __half* out, int rows, int cols);
 // scores f32 [rows][ld_in] (first n valid) -> softmax(scale * s) as fp16 [rows][ld_out], columns >= n zeroed

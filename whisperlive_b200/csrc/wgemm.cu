@@ -180,7 +180,7 @@ int wgemm_ksplit(int K) {
 // mode 0: out_f32 = acc + bias; 1: out_f32 += acc + bias (in place); 2: out_f16 = gelu(acc + bias);
 // 3: out_f32[ks] = raw partial sum of K range ks (K > 1280: the consumer adds the ranges and the bias)
 void wgemm(cudaStream_t st, const __half* W, int n_out, int K, const __half* X, int R, const float* bias, int mode, float* out_f32,
-           __half* out_f16, long part_stride, const void* prefetch_ptr, long prefetch_bytes) {
+           __half* out_f16, long part_stride) {
   WL_CHECK(wgemm_supported(R, K) && n_out % 8 == 0, WL_ERR_ARG, "wgemm: unsupported problem R=%d n_out=%d K=%d", R, n_out, K);
   const int ksplit = wgemm_ksplit(K);
   WL_CHECK(ksplit == 1 || mode == 3, WL_ERR_ARG, "wgemm: K=%d needs %d K ranges: only the partial-sum epilogue supports that", K, ksplit);
@@ -190,9 +190,6 @@ void wgemm(cudaStream_t st, const __half* W, int n_out, int K, const __half* X, 
   WgemmParams p;
   p.W = W; p.X = X; p.bias = bias; p.out_f32 = out_f32; p.out_f16 = out_f16; p.part_stride = part_stride;
   p.n_out = n_out; p.K = K; p.R = R; p.ksplit = ksplit; p.mode = mode;
-  // (prefetch_ptr / prefetch_bytes: an L2 prefetch of the next layer's weights from here gained nothing -- the slices are
-  // already requested ahead of the dependency -- and was removed)
-  (void)prefetch_ptr; (void)prefetch_bytes;
   // K range per CTA: equal ranges, multiples of 32
   p.kr = cdiv(cdiv(K, ksplit), 32) * 32;
   // features per CTA: the smallest multiple of 8 (<= 40) for which the grid fits one wave of one CTA per SM; the weight

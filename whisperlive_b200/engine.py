@@ -136,7 +136,7 @@ def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 
     mask = ((V + 31) // 32 + 1) * 4
     caches = 2 * Ld * R * H * T * 64 * f16
     decoder = (R * d * f32 + (R * 16 * d + R * 4 * ff) * f32 + R * 16 * d * f32 + R * ((V + 3) // 4 * 4) * f32
-               + 2 * Rp * d * f16 + Rp * ff * f16 + caches + B * H * 12 * MAX_ROWS * 66 * f32 + 2 * 4 + mask
+               + 2 * Rp * d * f16 + Rp * ff * f16 + caches + B * H * 12 * MAX_ROWS * 66 * f32 + mask
                + (2 * n_align_heads * i32 if n_align_heads else 0))
     state = (8 * R * 4 + R * T * i32 + R * T * 2 + 2 * R * MAX_CAND * 4 + 22 * B * 4 + B * T * i32
              + 2 * B * MAX_HYPS * 4 + B * MAX_HYPS * T * i32 + B * T * f32 + 4 * 4)
@@ -587,8 +587,7 @@ class B200Whisper:
 
     def test_wgemm(self, w: np.ndarray, x: np.ndarray, bias: Optional[np.ndarray] = None, mode: int = 0,
                    resid: Optional[np.ndarray] = None) -> np.ndarray:
-        """Y[R, n_out] = X[R, K] W[n_out, K]^T through the small-batch decode GEMM (wl_test_wgemm); ``mode | 8`` runs the
-        cluster split-K GEMM (any row count) with epilogue ``mode``."""
+        """Y[R, n_out] = X[R, K] W[n_out, K]^T through the small-batch decode GEMM (wl_test_wgemm) with epilogue ``mode``."""
         w16 = np.ascontiguousarray(w, dtype=np.float16)
         x16 = np.ascontiguousarray(x, dtype=np.float16)
         n_out, K = w16.shape
