@@ -14,6 +14,7 @@
  *   wl_align             <- Whisper.align                  transcriber_faster_whisper.py:1657-1663
  *   wl_slots_release     <- StorageView lifetime           transcriber_faster_whisper.py:1055, :1820-1823
  *   wl_vad               <- faster_whisper.vad.get_speech_timestamps (the Silero model call) transcriber_faster_whisper.py:830-838
+ *   wl_spk_embed         <- SpeakerDiarizer._compute_embedding (pyannote Inference)  diarization.py:100-118
  *
  * Conventions: plain pointers and sizes only; the caller owns every host buffer; the library owns
  * device memory, streams, CUDA graphs.  Every function returns 0 or a negative WL_ERR_* code and
@@ -29,7 +30,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 8
+#define WL_ABI_VERSION 9
 
 typedef struct wl_ctx wl_ctx;
 
@@ -78,7 +79,7 @@ const char* wl_last_error(wl_ctx* ctx);   /* ctx may be NULL: last wl_init / wl_
 /* Device memory the context holds right now, in bytes, counted where the library allocates it: weights (the uploaded
  * tensors and their fused copies), the encoder workspaces and slot pool, the self-attention caches, both decode
  * states, an open session, the log-mel / prefill / align / VAD workspaces at their current grown size, the VAD weights,
- * and the weight-load staging buffer while a load runs.  Not counted: buffers a call frees before it returns, CUDA graph executables and
+ * the speaker-embedding weights and workspace, and the weight-load staging buffer while a load runs.  Not counted: buffers a call frees before it returns, CUDA graph executables and
  * the CUDA context of the process. */
 int wl_device_bytes(wl_ctx* ctx, int64_t* out);
 /* Free and total device memory of CUDA ordinal `device` (cudaMemGetInfo); needs no context, so a load can be checked
@@ -261,7 +262,8 @@ int64_t wl_kernel_launches(wl_ctx* ctx);
  * which = 3: average ms per cross-attention kernel launch since wl_profile_cross_attn(ctx, 1), 4: launches timed;
  * 2 also holds the last wl_session_run, 5 the last wl_session_admit */
 float wl_last_device_ms(wl_ctx* ctx, int32_t which /*0 mel, 1 encode, 2 generate, 3/4 cross-attention profile,
-                                                      6 / 7 the last wl_vad's front end / recurrence*/);
+                                                      6 / 7 the last wl_vad's front end / recurrence,
+                                                      8 / 9 the last wl_spk_embed's fbank + CMN / network*/);
 /* enable = 1: wl_generate calls made WITHOUT a CUDA graph bracket every cross-attention launch (K11, the dominant
  * decode kernel) with CUDA events on the library stream -- bench.py's live roofline measurement.  Resets the sums. */
 int wl_profile_cross_attn(wl_ctx* ctx, int32_t enable);
@@ -292,6 +294,34 @@ int wl_encode_resident(wl_ctx* ctx, int32_t B, const int32_t* slots);
  * when any VAD tensor is missing. */
 int wl_vad_load_tensor(wl_ctx* ctx, const char* name, const float* data, const int64_t* shape, int32_t ndim);
 int wl_vad(wl_ctx* ctx, const float* pcm, const int64_t* offsets, int32_t B, float* probs_out, const int64_t* prob_off);
+
+/* Speaker embedding: the wespeaker ResNet34 of pyannote's wespeaker-voxceleb-resnet34-LM over Kaldi fbank (the protocol
+ * whisperlive_b200/speaker.py names).  wl_spk_load_tensor takes a float32 host tensor, BatchNorm already folded into each
+ * conv, under one of the fixed names
+ *   spk.conv1.weight [32, 1, 3, 3]                      spk.conv1.bias [32]
+ *   spk.layerL.i.conv1.weight / .conv2.weight [C, C_in, 3, 3] (.conv1.bias / .conv2.bias [C])
+ *   spk.layerL.0.shortcut.weight [C, C_in, 1, 1]        spk.layerL.0.shortcut.bias [C]        (L = 2, 3, 4)
+ *     L = 1..4 with C = 32, 64, 128, 256 and i < 3, 4, 6, 3; C_in = C except for the first conv / shortcut of a stage
+ *   spk.seg_1.weight [256, 5120]                        spk.seg_1.bias [256]
+ * and rejects any other name or shape; it may be called before or after wl_finalize_weights (loading a name again
+ * replaces it).  wl_spk_embed: pcm holds B waveforms in [-1, 1] concatenated at offsets[B+1] (samples, 16 kHz), each at
+ * least 400 samples (one fbank frame; checked before anything is launched); emb_out [B][256] receives the embeddings.
+ * A segment of fewer than 8 frames pools over one time step, whose unbiased variance is 0/0: its std half is NaN, as in
+ * PyTorch.  One upload of the samples and the offset tables, one download; fp16 activations, fp32 accumulation; a
+ * stream's embedding does not depend on the other streams of the call.  Fails when any tensor is missing. */
+int wl_spk_load_tensor(wl_ctx* ctx, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+int wl_spk_embed(wl_ctx* ctx, const float* pcm, const int64_t* offsets, int32_t B, float* emb_out);
+/* Test hook: wl_spk_embed's fbank launch over B waveforms (offsets[B+1], each >= 400 samples): feat_out [frames][80], the
+ * log mel energies before CMN, streams concatenated (stream b has 1 + (n_b - 400) / 160 frames). */
+int wl_test_spk_fbank(wl_ctx* ctx, const float* pcm, const int64_t* offsets, int32_t B, float* feat_out);
+/* Test hook: the launch wl_spk_embed makes for one convolution, on device copies of the inputs.  x fp16 [positions][C_in]
+ * with B streams of frames[b] time steps x H_in frequency rows, time-major per stream; w fp16 [C_out][ksize * ksize][C_in]
+ * (tap = kh * ksize + kw, kh over frequency); bias fp32 [C_out]; res fp16 [out positions][C_out] or NULL; relu 0/1;
+ * out fp16 [out positions][C_out] (uploaded as given, copied back whole).  ksize 3 pads by one, ksize 1 not; stride 2
+ * gives ceil(H_in / 2) x ceil(frames / 2) outputs per stream. */
+int wl_test_spk_conv(wl_ctx* ctx, const uint16_t* x_f16, const int64_t* frames, int32_t B, int32_t H_in, int32_t C_in,
+                     int32_t C_out, int32_t ksize, int32_t stride, const uint16_t* w_f16, const float* bias,
+                     const uint16_t* res_f16, int32_t relu, uint16_t* out_f16);
 
 #ifdef __cplusplus
 }

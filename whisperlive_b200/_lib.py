@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 8
+ABI_VERSION = 9
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -100,6 +100,11 @@ SIGNATURES = {
     "wl_encode_resident": (C.c_int, [C.c_void_p, C.c_int32, c_i32p]),
     "wl_vad_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
     "wl_vad": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p, c_i64p]),
+    "wl_spk_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
+    "wl_spk_embed": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p]),
+    "wl_test_spk_fbank": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p]),
+    "wl_test_spk_conv": (C.c_int, [C.c_void_p, c_u16p, c_i64p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_int32, c_u16p, c_f32p, c_u16p, C.c_int32, c_u16p]),
 }
 
 _lock = threading.Lock()

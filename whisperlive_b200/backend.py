@@ -45,6 +45,15 @@ def vad_from_env():
     return "device" if v == "device" else None
 
 
+def diarize_from_env() -> str:
+    """``WLB200_DIARIZE=device``: speaker embeddings on the model's GPU context (``speaker.DeviceSpeakerDiarizer``);
+    unset or ``cpu``: the diarizer the reference passes in, untouched."""
+    v = os.environ.get("WLB200_DIARIZE", "cpu").strip().lower()
+    if v not in ("cpu", "device"):
+        raise ValueError(f"WLB200_DIARIZE={v!r}: 'cpu' (default) or 'device'")
+    return v
+
+
 if ServeClientBase is not None:
 
     class ServeClientB200(ServeClientBase):
@@ -101,6 +110,10 @@ if ServeClientBase is not None:
                 self.websocket.close()
                 return
             self.use_vad = use_vad
+            if self.diarization is not None and diarize_from_env() == "device":
+                from .speaker import DeviceSpeakerDiarizer
+                worker = self.scheduler if self.registry is not None else ServeClientB200.BATCH_WORKER
+                self.diarization = DeviceSpeakerDiarizer.replacing(self.diarization, worker)
             self.trans_thread = threading.Thread(target=self.speech_to_text)
             self.trans_thread.start()
             self.websocket.send(json.dumps({"uid": self.client_uid, "message": self.SERVER_READY, "backend": "faster_whisper"}))
@@ -138,7 +151,8 @@ if ServeClientBase is not None:
                         resolve = lambda name: resolve_model_dir(name, local_files_only=True)
                         kw = dict(resolve=resolve, devices=devices_from_env(), reserve_bytes=cls.MEMORY_RESERVE_BYTES,
                                   footprint=lambda name: engine_footprint(name, cls.MAX_STREAMS, resolve=resolve,
-                                                                         vad=vad_from_env() == "device"))
+                                                                         vad=vad_from_env() == "device",
+                                                                         diarize=diarize_from_env() == "device"))
                     cls.REGISTRY = ModelRegistry(cls.build_model, max_streams=cls.MAX_STREAMS,
                                                  batch_window_ms=cls.BATCH_WINDOW_MS, **kw)
                 return cls.REGISTRY

@@ -34,6 +34,33 @@ void vad_front(cudaStream_t st, const VadWeights& w, const float* pcm, const lon
 // probs [total_frames]: the recurrence over each stream's frames
 void vad_lstm(cudaStream_t st, const VadWeights& w, const float* gx, const long* frame_off, int B, float* probs);
 
+// ---------------------------------------------------------------------------- speaker embedding (spk.cu)
+// fbank [frames][80] fp32 of every stream's frames (frame_off [B + 1]) and the per-stream bin means [B][80];
+// melw [80][257] with the non-zero range of each bin in mel_range [80][2]
+void spk_fbank(cudaStream_t st, const float* pcm, const long* pcm_off, const long* frame_off, int B, long frames,
+               const float* melw, const int* mel_range, float* feat, float* mean);
+// conv3x3 1 -> 32 of the CMN'd fbank (H = 80, positions = frames x 80), folded BN + ReLU, fp16 [position][32]
+void spk_stem(cudaStream_t st, const float* feat, const float* mean, const long* frame_off, int B, long frames, const float* w,
+              const float* bias, __half* out);
+// out[m][n] = act(bias[n] + sum_k x(m, k) w[n][k] (+ res[m][n])): x fp16 [in position][C_in], w fp16 [C_out][taps][C_in]
+// (tap = kh * 3 + kw, kh over frequency), positions of stream b at in_off[b] / out_off[b] (device, [B + 1]), time-major
+struct SpkConvParams {
+  const __half* x;
+  const __half* w;
+  const float* bias;
+  const __half* res;   // nullptr, or [M][C_out] (may be `out`)
+  __half* out;
+  const long* in_off;
+  const long* out_off;
+  long M;
+  int B, H_in, H_out, C_in, C_out, taps, stride, relu;
+};
+bool spk_conv_supported(int C_in, int C_out, int taps, int stride);
+void spk_conv(cudaStream_t st, const SpkConvParams& p);
+// TSTP of x fp16 [position][256] (H frequency rows) -> pooled [B][2 * 256 * H], then emb [B][256] = seg_1 (wt [2*256*H][256])
+void spk_pool_embed(cudaStream_t st, const __half* x, const long* pos_off, int B, int H, const float* wt, const float* bias,
+                    float* pooled, float* emb);
+
 // A value produced by a split-K GEMM: v(r, c) = bias[c] + sum_s ptr[s * stride + r * ld + c]  (fixed order).
 // nsplit == 1 with bias == nullptr is a plain buffer; nsplit == 0 means "nothing pending".
 struct PartialSrc {

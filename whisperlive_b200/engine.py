@@ -99,13 +99,14 @@ class EncoderOutput:
 
 
 def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
-                       n_align_heads: Optional[int] = None, vad: bool = False) -> int:
+                       n_align_heads: Optional[int] = None, vad: bool = False, diarize: bool = False) -> int:
     """Device bytes a context of these shapes allocates through ``wl_init``, the weight load and one open decode session
     (csrc/engine.cu: ``wl_load_tensor``, ``finalize_impl``, ``alloc_decode_state``, ``wl_session_open``), plus the
     workspaces its first step round grows: the log-mel of ``max_streams`` 30-second chunks (``wl_mel``) and the batched
     prefill at its first size of 1024 rows (``prefill_reserve``).  What a model registry compares with the free memory
     before a load.  ``vad=True`` adds the Silero VAD weights and the VAD workspace of ``max_streams`` 30-second chunks
-    (``wl_vad_load_tensor``, ``wl_vad``).  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
+    (``wl_vad_load_tensor``, ``wl_vad``); ``diarize=True`` the speaker-embedding weights and the workspace of its first
+    call, ``max_streams`` segments of 30 s (``wl_spk_load_tensor``, ``wl_spk_embed``).  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
     chunks, more prompt rows, the word-alignment buffers) and the allocator's rounding."""
     B, K = int(max_streams), int(max_beam)
     NS = int(enc_slots) if enc_slots is not None else 2 * B
@@ -153,7 +154,31 @@ def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 
                        + 2 * 512 * 128 + 2 * 512 + 128 + 1) * f32
         vad_frames = B * (pcm // B // 512 + 1)
         total += vad_weights + pcm * f32 + vad_frames * (512 + 1) * f32 + 2 * (B + 1) * 8
+    if diarize:
+        total += spk_footprint(B)
     return int(total)
+
+
+def spk_footprint(max_streams: int) -> int:
+    """Device bytes of the speaker-embedding weights as ``wl_spk_load_tensor`` stores them (fp16 tensor-core conv
+    weights, fp32 stem, biases and embedding layer) plus the workspace ``wl_spk_embed`` allocates at its first call."""
+    from . import speaker as S
+    B, f32, f16 = int(max_streams), 4, 2
+    weights = 0
+    for name, co, ci, k in S.conv_names():
+        weights += co * ci * k * k * (f32 if ci == 1 else f16) + co * f32
+    weights += (S.POOL_DIM * S.EMBED_DIM + S.EMBED_DIM) * f32
+    mel = S.MEL_BINS * (S.N_FFT // 2 + 1) * f32 + 2 * S.MEL_BINS * 4
+    pcm = B * 30 * S.SAMPLING_RATE
+    frames = B * S.n_frames(30 * S.SAMPLING_RATE)
+    per_stream = (S.MEL_BINS + S.POOL_DIM + S.EMBED_DIM) * f32 + 6 * 8
+    acts, T = [], S.n_frames(30 * S.SAMPLING_RATE)
+    for L, (c, _nb, _stride) in enumerate(S.STAGES):
+        if L:
+            T = (T + 1) // 2
+        acts.append(B * (S.MEL_BINS >> L) * T * c)
+    act = max(acts[0], acts[2]) + max(acts) + max(acts[1], acts[3])
+    return int(weights + mel + pcm * f32 + frames * S.MEL_BINS * f32 + B * per_stream + 6 * 8 + act * f16)
 
 
 def mem_info(device: int = 0) -> Tuple[int, int]:
@@ -329,6 +354,72 @@ class B200Whisper:
                                  _lib.ptr(out, C.c_float), _lib.ptr(poff, C.c_int64))
             _lib.check(self.lib, self.ctx, rc, "wl_vad")
         return [out[poff[i]:poff[i + 1]].copy() for i in range(len(waves))]
+
+    def spk_load(self, tensors: Dict[str, "np.ndarray"]) -> None:
+        """Upload the speaker-embedding tensors (``spk.*`` names of include/wlb200.h, BN folded) as float32."""
+        for name, t in tensors.items():
+            a = np.ascontiguousarray(t, dtype=np.float32)
+            shape = np.asarray(a.shape, dtype=np.int64)
+            with self._lock:
+                rc = self.lib.wl_spk_load_tensor(self.ctx, name.encode(), _lib.ptr(a, C.c_float), _lib.ptr(shape, C.c_int64),
+                                                 a.ndim)
+                _lib.check(self.lib, self.ctx, rc, f"wl_spk_load_tensor({name})")
+
+    def spk_embeddings(self, audios: Sequence[np.ndarray]) -> np.ndarray:
+        """Speaker embeddings [B, 256] of 16 kHz waveforms of at least 400 samples (``wl_spk_embed``): one upload of all
+        of them, one pass of the network, one download."""
+        if not audios:
+            return np.zeros((0, 256), np.float32)
+        waves = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in audios]
+        off = np.zeros(len(waves) + 1, dtype=np.int64)
+        off[1:] = np.cumsum([w.shape[0] for w in waves])
+        pcm = np.concatenate(waves)
+        out = np.empty((len(waves), 256), dtype=np.float32)
+        with self._lock:
+            rc = self.lib.wl_spk_embed(self.ctx, _lib.ptr(pcm, C.c_float), _lib.ptr(off, C.c_int64), len(waves),
+                                       _lib.ptr(out, C.c_float))
+            _lib.check(self.lib, self.ctx, rc, "wl_spk_embed")
+        return out
+
+    def test_spk_fbank(self, audios: Sequence[np.ndarray]) -> List[np.ndarray]:
+        """``wl_spk_embed``'s fbank of each waveform (``wl_test_spk_fbank``): [frames, 80] before CMN."""
+        from .speaker import n_frames
+        waves = [np.ascontiguousarray(a, dtype=np.float32).reshape(-1) for a in audios]
+        off = np.zeros(len(waves) + 1, dtype=np.int64)
+        off[1:] = np.cumsum([w.shape[0] for w in waves])
+        foff = np.zeros(len(waves) + 1, dtype=np.int64)
+        foff[1:] = np.cumsum([n_frames(w.shape[0]) for w in waves])
+        pcm = np.concatenate(waves)
+        out = np.empty((max(int(foff[-1]), 1), 80), dtype=np.float32)
+        with self._lock:
+            rc = self.lib.wl_test_spk_fbank(self.ctx, _lib.ptr(pcm, C.c_float), _lib.ptr(off, C.c_int64), len(waves),
+                                            _lib.ptr(out, C.c_float))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_spk_fbank")
+        return [out[foff[i]:foff[i + 1]].copy() for i in range(len(waves))]
+
+    def test_spk_conv(self, x: np.ndarray, frames: Sequence[int], H_in: int, w: np.ndarray, bias: np.ndarray, stride: int,
+                      res: Optional[np.ndarray] = None, relu: bool = True, out: Optional[np.ndarray] = None) -> np.ndarray:
+        """One convolution launch of ``wl_spk_embed`` (``wl_test_spk_conv``): x fp16 [positions, C_in], w fp16
+        [C_out, taps, C_in], res / out fp16 [out positions, C_out] (out: the buffer as it is before the launch)."""
+        x16 = np.ascontiguousarray(x, dtype=np.float16)
+        w16 = np.ascontiguousarray(w, dtype=np.float16)
+        C_out, taps, C_in = w16.shape
+        k = int(round(taps ** 0.5))
+        fr = np.ascontiguousarray(frames, dtype=np.int64)
+        H_out = (H_in + 1) // 2 if stride == 2 else H_in
+        T_out = (fr + 1) // 2 if stride == 2 else fr
+        M = int(H_out * T_out.sum())
+        o16 = np.zeros((M, C_out), np.float16) if out is None else np.ascontiguousarray(out, dtype=np.float16).copy()
+        b32 = np.ascontiguousarray(bias, dtype=np.float32)
+        r16 = None if res is None else np.ascontiguousarray(res, dtype=np.float16)
+        with self._lock:
+            rc = self.lib.wl_test_spk_conv(self.ctx, _lib.ptr(x16.view(np.uint16), C.c_uint16), _lib.ptr(fr, C.c_int64), len(fr),
+                                           int(H_in), C_in, C_out, k, int(stride), _lib.ptr(w16.view(np.uint16), C.c_uint16),
+                                           _lib.ptr(b32, C.c_float),
+                                           None if r16 is None else _lib.ptr(r16.view(np.uint16), C.c_uint16), int(relu),
+                                           _lib.ptr(o16.view(np.uint16), C.c_uint16))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_spk_conv")
+        return o16
 
     def profile_cross_attn(self, enable: bool) -> None:
         """Bracket every cross-attention launch of graph-less generate calls with CUDA events (bench.py roofline)."""

@@ -246,10 +246,11 @@ def _wl_free_bytes(device: int) -> int:
 
 
 def engine_footprint(name: str, max_streams: int = 8, max_beam: int = 5, resolve: Optional[Callable[[str], str]] = None,
-                     vad: bool = False) -> Optional[int]:
+                     vad: bool = False, diarize: bool = False) -> Optional[int]:
     """``footprint_estimate`` of the CUDA engine for a size name, or for a model directory whose HF ``config.json``
     gives the shapes; None when the shapes cannot be known before the weights are read.  ``vad``: the model runs the
-    Silero VAD on its context (``vad="device"``)."""
+    Silero VAD on its context (``vad="device"``); ``diarize``: it computes speaker embeddings there
+    (``WLB200_DIARIZE=device``)."""
     from .config import WhisperDims, dims_for
     from .engine import footprint_estimate
     try:
@@ -267,4 +268,4 @@ def engine_footprint(name: str, max_streams: int = 8, max_beam: int = 5, resolve
                                    int(cfg["decoder_layers"]), int(cfg["num_mel_bins"]), int(cfg["vocab_size"]))
         if dims is None:
             return None
-    return footprint_estimate(dims, max_streams=max_streams, max_beam=max_beam, vad=vad)
+    return footprint_estimate(dims, max_streams=max_streams, max_beam=max_beam, vad=vad, diarize=diarize)

@@ -79,6 +79,11 @@ class MultiDeviceWhisperModel:
         self._next = (self._next + 1) % len(self.models)
         return self.models[g].transcribe(audio, **kw)
 
+    def speaker_embeddings(self, audios: Sequence[np.ndarray]) -> np.ndarray:
+        """Speaker embeddings on the first device's context (``B200WhisperModel.speaker_embeddings``): the segments of
+        a round are few and short next to its decode work, so they stay in one call on one GPU."""
+        return self.models[0].speaker_embeddings(audios)
+
     def open_session(self) -> "MultiDeviceSession":
         """What ``RoundScheduler`` drives: one ``TranscribeSession`` per GPU advanced concurrently, so the step-level
         admission (streams join the running decode loop of THEIR device) works across all of them."""

@@ -16,7 +16,9 @@ the drop-in schema a client thread fills in and waits on); the control flow is d
   of a finished stream is refilled immediately;
 * an engine error fails the streams it touched, never the scheduler (``TranscribeSession`` isolates them);
 * between step rounds the owner thread publishes interim segments for the requests that want them (one batched peek of
-  the decode session) and drops cancelled requests, freeing their decode index and encoder slots.
+  the decode session) and drops cancelled requests, freeing their decode index and encoder slots;
+* speaker-embedding requests (``embed``, the device diarizer's) are answered at every round boundary, all that are
+  pending in one ``speaker_embeddings`` call, and right away when nothing is in flight.
 
 ``linger_ms`` (default 0) optionally waits for more requests when the engine is idle and a single request arrived --
 the latency / batching trade the reference hard-codes as its 50 ms window.
@@ -101,6 +103,24 @@ class BatchRequest:
                     word_timestamps=self.word_timestamps)
 
 
+class EmbeddingRequest:
+    """A speaker-embedding request (``RoundScheduler.embed``): ``wait()`` returns the [256] float32 vector or raises the
+    error of the call that failed it."""
+
+    def __init__(self, audio: np.ndarray):
+        self.audio = audio
+        self.future = threading.Event()
+        self.result: Optional[np.ndarray] = None
+        self.error: Optional[Exception] = None
+
+    def wait(self, timeout: Optional[float] = 60.0) -> np.ndarray:
+        if not self.future.wait(timeout):
+            raise TimeoutError(f"speaker embedding not answered within {timeout} s")
+        if self.error is not None:
+            raise self.error
+        return self.result
+
+
 class RoundScheduler:
     def __init__(self, transcriber, max_batch_size: int = 8, batch_window_ms: int = 0, linger_ms: Optional[int] = None,
                  step_tokens: Optional[int] = 16):
@@ -114,6 +134,7 @@ class RoundScheduler:
         self.capacity = max(1, int(max_batch_size))
         self.linger_s = (batch_window_ms if linger_ms is None else linger_ms) / 1000.0
         self._inbox: Deque[BatchRequest] = collections.deque()
+        self._embeds: List[EmbeddingRequest] = []
         self._cv = threading.Condition()
         self._stop = False
         self._thread: Optional[threading.Thread] = None
@@ -122,6 +143,7 @@ class RoundScheduler:
         self.streams_done = 0
         self.max_in_flight = 0
         self.admitted_mid_flight = 0   # streams that joined while others were already decoding
+        self.embedding_calls = 0
 
     # ------------------------------------------------------------------ client side
     def submit(self, request: BatchRequest) -> None:
@@ -129,6 +151,15 @@ class RoundScheduler:
         with self._cv:
             self._inbox.append(request)
             self._cv.notify()
+
+    def embed(self, audio: np.ndarray) -> EmbeddingRequest:
+        """Queue one segment for a speaker embedding; the owner thread answers it with every other pending one at the
+        next round boundary, or at once when the engine is idle."""
+        request = EmbeddingRequest(np.asarray(audio, dtype=np.float32).reshape(-1))
+        with self._cv:
+            self._embeds.append(request)
+            self._cv.notify()
+        return request
 
     def start(self) -> None:
         self._thread = threading.Thread(target=self._owner_loop, daemon=True, name="wlb200-rounds")
@@ -145,11 +176,11 @@ class RoundScheduler:
     def _take(self, room: int, block: bool) -> List[BatchRequest]:
         with self._cv:
             if block:
-                while not self._inbox and not self._stop:
+                while not self._inbox and not self._embeds and not self._stop:
                     self._cv.wait(timeout=0.5)
-                if self.linger_s > 0 and len(self._inbox) < room and not self._stop:
+                if self.linger_s > 0 and self._inbox and len(self._inbox) < room and not self._stop:
                     end = time.monotonic() + self.linger_s      # idle engine, first request: optionally wait for company
-                    while len(self._inbox) < room and not self._stop:
+                    while len(self._inbox) < room and not self._embeds and not self._stop:
                         left = end - time.monotonic()
                         if left <= 0:
                             break
@@ -164,7 +195,7 @@ class RoundScheduler:
         in_flight: Dict[int, BatchRequest] = {}
         while True:
             with self._cv:
-                if self._stop and not in_flight and not self._inbox:
+                if self._stop and not in_flight and not self._inbox and not self._embeds:
                     close = getattr(session, "close", None)
                     if close is not None:
                         close()             # hands the engine's decode session back
@@ -185,6 +216,7 @@ class RoundScheduler:
                     log.error("admission failed: %s", e)
                     for r in new:
                         self._finish(r, None, None, e)
+            self._answer_embeddings()
             self.max_in_flight = max(self.max_in_flight, len(in_flight))
             self._drop_cancelled(session, in_flight)
             if not in_flight:
@@ -214,6 +246,24 @@ class RoundScheduler:
                     self._finish(r, None, None, e)
             if step:
                 self._publish_partials(session, in_flight)
+
+    def _answer_embeddings(self) -> None:
+        """Every pending embedding request in one ``speaker_embeddings`` call; an error fails only these requests."""
+        with self._cv:
+            batch, self._embeds = self._embeds, []
+        if not batch:
+            return
+        try:
+            out = self.transcriber.speaker_embeddings([r.audio for r in batch])
+            self.embedding_calls += 1
+            for r, v in zip(batch, out):
+                r.result = np.asarray(v, dtype=np.float32)
+        except Exception as e:
+            log.error("speaker embeddings failed: %s", e)
+            for r in batch:
+                r.error = e
+        for r in batch:
+            r.future.set()
 
     def _drop_cancelled(self, session, in_flight: Dict[int, BatchRequest]) -> None:
         """Take the cancelled requests out of the session (index and encoder slots back) and answer them."""

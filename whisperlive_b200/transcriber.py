@@ -941,6 +941,9 @@ class B200WhisperModel:
             vad = DeviceVad(engine, weights="random" if weights == "random" else None, seed=seed)
         self._vad = vad
         self.model = engine
+        self._spk_weights = "random" if weights == "random" else None   # loaded by the first speaker_embeddings call
+        self._spk_seed = seed
+        self._spk_loaded = False
         model_dir = getattr(engine, "model_dir", None) or model_size_or_path
         if isinstance(hf_tokenizer, str):
             if hf_tokenizer != "synthetic":
@@ -1003,6 +1006,17 @@ class B200WhisperModel:
     def destroy(self) -> None:
         """Free the engine context and its device memory now (a model registry evicting this model)."""
         self.model.destroy()
+
+    def speaker_embeddings(self, audios: Sequence[np.ndarray]) -> np.ndarray:
+        """Speaker embeddings [B, 256] of 16 kHz segments (at least 400 samples each) on this model's engine context, one
+        ``wl_spk_embed`` call for all of them.  The first call loads the wespeaker weights (``speaker.resolve_weights``:
+        ``WLB200_SPK_MODEL`` or a local snapshot of the reference's default embedding model; seeded random ones when the
+        model itself was built with ``weights="random"``)."""
+        if not self._spk_loaded:
+            from .speaker import resolve_weights
+            self.model.spk_load(resolve_weights(self._spk_weights, self._spk_seed))
+            self._spk_loaded = True
+        return self.model.spk_embeddings(audios)
 
     # -- Boundary B ---------------------------------------------------------------------------
     def transcribe(self, audio: np.ndarray, language: Optional[str] = None, task: str = "transcribe",
