@@ -30,7 +30,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 9
+#define WL_ABI_VERSION 10
 
 typedef struct wl_ctx wl_ctx;
 
@@ -53,7 +53,7 @@ typedef struct wl_config {
 
 typedef struct wl_gen_opts {
   int32_t beam_size;                 /* 1 = greedy / sampling */
-  float patience;
+  float patience;                    /* beam search ends with round(beam_size * patience) <= 16 hypotheses (more is an error) */
   int32_t num_hypotheses;
   float length_penalty;
   int32_t max_length;                /* CT2 max_length (448) */
@@ -251,6 +251,21 @@ int wl_test_enc_stem(wl_ctx* ctx, const float* feats_f32, float* x_out_f32, int3
  * copied back whole, so the 8 guard rows after the last one show what the kernel wrote past it. */
 int wl_test_layernorm(wl_ctx* ctx, const float* x_f32, const float* gamma, const float* beta, float* y16_as_f32, float* y32,
                       int32_t rows, int32_t d);
+/* Search on scripted logits: wl_generate with the decoder replaced.  Each step's logits are a pure function of the
+ * tokens a row has consumed (tests/search_script.py restates the function); no encoder slot is read.  Everything else
+ * -- prompt upload, decode_init, the captured or host-driven loop, the search kernels, the hypothesis ranking -- is
+ * wl_generate's own code.  opts->prefill = 1: the stream starts at its last prompt token (the no-speech probability is
+ * then written from the scripted logits at the sot position); 2: the prompt is fed token by token.  Outputs as
+ * wl_generate, plus out_hyp_count [B] (hypotheses each stream finished with) and, when not NULL, out_logits
+ * [B * rows per stream][(vocab + 3) / 4 * 4]: the logits of the first decode step. */
+typedef struct wl_search_script {
+  uint32_t seed;
+  int32_t pattern;   /* 0 none, 1 one selection thread's strided set, 2 one float4 group, 3 the vocabulary's last tokens,
+                        4 a grid of 1/4, 5 one or two dominant tokens; -1 chosen per step */
+} wl_search_script;
+int wl_test_search(wl_ctx* ctx, int32_t B, const int32_t* prompts, const int32_t* prompt_off, const wl_gen_opts* opts,
+                   const wl_search_script* script, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
+                   int32_t* out_steps, int32_t* out_hyp_count, float* out_logits);
 /* device-resident timing of the GEMM kernel: C = A(MxK) * B(NxK)^T, `iters` launches between CUDA events;
  * bn = 0 picks the tile like the engine does. ms_out = average milliseconds per launch. */
 int wl_bench_gemm(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,

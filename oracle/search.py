@@ -27,12 +27,15 @@ Semantics restated:
   then log-softmax.
   beam search: candidates = top 2K of (cum + logp) over the K live rows (first step:
   one row); walking the top K, an EOT candidate closes a hypothesis and its slot is
-  refilled from candidates K..2K; a stream ends with round(K*patience) hypotheses or
-  at the last step (everything in the top K closes).  Ties break toward the lower
-  flat index (row-major beam*vocab).
+  refilled from candidates K..2K; a stream ends with max(1, round(K*patience))
+  hypotheses or at the last step (everything in the top K closes).  The rounding is
+  half away from zero, CT2's ``std::round`` as recalled from its sources, not pinned
+  against a CT2 run: K=5 with patience 0.5 gives 3, K=3 with patience 1.5 gives 5.
+  Ties break toward the lower flat index (row-major beam*vocab).
   greedy/sampling (K=1): argmax, or Gumbel-max with a counter hash
   (``gumbel_noise``) when sampling_topk != 1 and temperature > 0, ``num_hypotheses``
-  independent rows.
+  independent rows.  A row whose every token is masked finishes without a token
+  (the device's behaviour; CT2 leaves that case undefined).
 """
 from __future__ import annotations
 
@@ -160,12 +163,16 @@ def apply_processors(logits: torch.Tensor, gen: List[int], spec: VocabSpec, opts
             if stamps:
                 cutoff = stamps[-1] if (last_ts and not penult_ts) else stamps[-1] + 1
                 x[tb:cutoff] = NEG_INF
+            if not bool(torch.isfinite(x).any()):
+                return x          # every token masked: no candidate (not the NaN row of a log-softmax over nothing)
             logp = torch.log_softmax(x, dim=-1)
             ts_lp = torch.logsumexp(logp[tb:], dim=-1)
             if rule_margin is not None:
                 rule_margin.append(abs(float(ts_lp - logp[:tb].max())))
             if ts_lp > logp[:tb].max():
                 x[:tb] = NEG_INF
+    if not bool(torch.isfinite(x).any()):
+        return x
     return torch.log_softmax(x, dim=-1)
 
 
@@ -204,12 +211,21 @@ class StreamResult:
     # sampling only: per hypothesis row, the margin of the Gumbel-perturbed arg-max at every step
     row_margins: dict = field(default_factory=dict)
     row_tokens: List[List[int]] = field(default_factory=list)
+    # beam search: hypotheses finished before the best num_hypotheses were kept, and why the search ended
+    # ("max_cand", "last_step" or "no_alive")
+    n_hypotheses: int = 0
+    stop: str = ""
 
 
 def _normalise(cum: float, n_tokens: int, length_penalty: float) -> float:
     if length_penalty == 0:
         return cum
     return cum / (max(n_tokens, 1) ** length_penalty)
+
+
+def max_candidates(beam_size: int, patience: float) -> int:
+    """Hypotheses that end a beam search: round(K * patience) half away from zero, at least 1."""
+    return max(1, int(math.floor(abs(beam_size * patience) + 0.5)))
 
 
 def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions, stream_index: int = 0) -> StreamResult:
@@ -258,6 +274,10 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
                 rule = []
                 logp = apply_processors(logits[r], gens[r], spec, opts, use_ts, prefix, rule)
                 rule_m = min(rule) if rule else float("inf")
+                if not bool(torch.isfinite(logp).any()):   # every token masked: the row ends with no token
+                    done[r] = True
+                    nxt.append(spec.eot)
+                    continue
                 if sampling:
                     z = logp / opts.sampling_temperature
                     if opts.sampling_topk > 0:
@@ -290,7 +310,7 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
         res.row_tokens = [list(g) for g in gens]
     else:
         K = opts.beam_size
-        max_cand = int(round(K * opts.patience))
+        max_cand = max_candidates(K, opts.patience)
         alive_tokens: List[List[int]] = [[]]
         alive_cum = [0.0]
         hyps: List[Hypothesis] = []
@@ -315,6 +335,7 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
             last_step = step + 1 == n_new
             new_tokens, new_cum, new_parent = [], [], []
             secondary = K
+            ev = {"closed_eot": 0, "closed_last": 0, "refilled": 0, "ran_out": 0}
             for k in range(min(K, n_c)):
                 beam, tok, sc = cand[k]
                 if not math.isfinite(sc):
@@ -322,6 +343,7 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
                 if tok == spec.eot or last_step:
                     toks = alive_tokens[beam] + ([] if tok == spec.eot else [tok])
                     hyps.append(Hypothesis(toks, sc, _normalise(sc, len(toks), opts.length_penalty)))
+                    ev["closed_last" if last_step else "closed_eot"] += 1
                     if last_step:
                         continue
                     repl = None
@@ -332,13 +354,19 @@ def search_stream(step_fn, prompt: List[int], spec: VocabSpec, opts: GenOptions,
                             repl = (b2, t2, s2)
                             break
                     if repl is None:
+                        ev["ran_out"] += 1
                         continue
+                    ev["refilled"] += 1
                     beam, tok, sc = repl
                 new_tokens.append(alive_tokens[beam] + [tok])
                 new_cum.append(sc)
                 new_parent.append(beam)
             res.steps = step + 1
+            if opts.trace:
+                res.trace[-1].update(ev, n_alive=len(new_tokens))
+            res.n_hypotheses = len(hyps)
             if len(hyps) >= max_cand or last_step or not new_tokens:
+                res.stop = "max_cand" if len(hyps) >= max_cand else ("last_step" if last_step else "no_alive")
                 break
             alive_tokens, alive_cum = new_tokens, new_cum
             parents = torch.tensor(new_parent, dtype=torch.long)

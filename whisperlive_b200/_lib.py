@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 9
+ABI_VERSION = 10
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -45,6 +45,10 @@ class WlStreamSearch(C.Structure):
         ("sample", C.c_int32), ("num_hypotheses", C.c_int32), ("temperature", C.c_float), ("seed", C.c_uint32),
         ("noise_key", C.c_int32),
     ]
+
+
+class WlSearchScript(C.Structure):
+    _fields_ = [("seed", C.c_uint32), ("pattern", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/wlb200.h declares
@@ -90,6 +94,8 @@ SIGNATURES = {
     "wl_test_enc_attn": (C.c_int, [C.c_void_p, c_u16p, c_u16p, c_u16p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "wl_test_enc_stem": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int32]),
     "wl_test_layernorm": (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_int32, C.c_int32]),
+    "wl_test_search": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, C.POINTER(WlGenOpts), C.POINTER(WlSearchScript),
+                                 c_i32p, c_i32p, c_f32p, c_f32p, c_i32p, c_i32p, c_f32p]),
     "wl_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_f32p]),
     "wl_kernel_launches": (C.c_int64, [C.c_void_p]),
     "wl_last_device_ms": (C.c_float, [C.c_void_p, C.c_int32]),

@@ -1683,9 +1683,9 @@ static VocabIds vocab_ids(wl_ctx* c) {
 // hp_row[T_MAX]; search_meta writes the other rows).  Returns the
 // decode steps the stream may need without prefill; *n_new_out = the new tokens it may emit.
 static int stream_meta(wl_ctx* c, int b, int slot, const int32_t* prompt, int P, int ml, bool forced, int* hp_row, int* meta, int col,
-                       int ncol, int* n_new_out) {
+                       int ncol, int* n_new_out, bool reads_slot = true) {
   WL_CHECK(P >= 1 && P <= T_MAX, WL_ERR_ARG, "stream %d: prompt length %d out of range", b, P);
-  WL_CHECK(slot >= 0 && slot < c->NS && c->slot_used[slot], WL_ERR_ARG, "stream %d: bad encoder slot %d", b, slot);
+  WL_CHECK(!reads_slot || (slot >= 0 && slot < c->NS && c->slot_used[slot]), WL_ERR_ARG, "stream %d: bad encoder slot %d", b, slot);
   int sot = -1;
   for (int i = 0; i < P; ++i) {
     const int t = prompt[i];
@@ -1748,7 +1748,8 @@ static void upload_state_tables(wl_ctx* c, const int* hp, const int* meta, int B
   for (int k = 0; k < META_ROWS; ++k) WL_CUDA(cudaMemcpyAsync(dst[k], meta + (size_t)k * B, B * 4, cudaMemcpyHostToDevice, st));
 }
 
-// upload prompts & per-stream metadata, every stream with the same search (key = batch position); returns max steps
+// upload prompts & per-stream metadata, every stream with the same search (key = batch position); returns max steps.
+// slots == nullptr: the call reads no encoder slot (wl_test_search), every stream gets slot 0.
 static int upload_streams(wl_ctx* c, const int32_t* slots, int B, const int32_t* prompts, const int32_t* off, int max_length,
                           bool forced, int sample, float temperature, uint32_t seed, int rows, const int32_t* max_len_ps = nullptr,
                           int* max_new_out = nullptr) {
@@ -1758,8 +1759,9 @@ static int upload_streams(wl_ctx* c, const int32_t* slots, int B, const int32_t*
   int max_steps = 0, max_new = 0;
   for (int b = 0; b < B; ++b) {
     int n_new = 0;
-    const int steps = stream_meta(c, b, slots[b], prompts + off[b], off[b + 1] - off[b], max_len_ps ? max_len_ps[b] : max_length,
-                                  forced, hp + (size_t)b * T_MAX, meta, b, B, &n_new);
+    const int steps = stream_meta(c, b, slots ? slots[b] : 0, prompts + off[b], off[b + 1] - off[b],
+                                  max_len_ps ? max_len_ps[b] : max_length, forced, hp + (size_t)b * T_MAX, meta, b, B, &n_new,
+                                  slots != nullptr);
     search_meta(meta, b, B, sample, temperature, seed, b, rows);
     max_steps = std::max(max_steps, steps);
     max_new = std::max(max_new, n_new);
@@ -1799,14 +1801,28 @@ static void emit_hyps(int NH, float length_penalty, int count, const int* h_len,
   }
 }
 
+// One token step of a generate call: the decoder's (decode_step), or with `script` (wl_test_search) the scripted logits
+// followed by the same two search kernels.
+static void token_step(wl_ctx* c, int B, int Kr, const SearchOpts& so, const VocabIds& vi, int nsplit, const SearchScript* script) {
+  if (!script) {
+    decode_step(c, B, Kr, so, vi, nsplit, false);
+    return;
+  }
+  PdlScope pdl(true);
+  scripted_logits(c->st, c->ds, so, vi, *script, c->logits, B * Kr);
+  search_rows(c->st, c->ds, c->logits, so, vi, B * Kr);
+  search_streams(c->st, c->ds, so, vi, B);
+}
+
 // The captured token loop for one call shape (cached per context): a conditional WHILE node whose body is the decode
 // step + loop_condition, so the whole loop is one launch.  `tag` separates the graphs of the one-shot state ("g") from
-// those of the decode session ("s"): the captures bake the state's device pointers in.
+// those of the decode session ("s"): the captures bake the state's device pointers in (and a script's parameters).
 static cudaGraphExec_t decode_graph(wl_ctx* c, const char* tag, int B, int Kr, int K, const SearchOpts& so, const VocabIds& vi,
-                                    int nsplit, long* kernels) {
+                                    int nsplit, long* kernels, const SearchScript* script = nullptr) {
   cudaStream_t st = c->st;
   char key[160];
   snprintf(key, sizeof(key), "%s/%d/%d/%d/%d/%d/%d", tag, B, Kr, K, so.max_cand, so.suppress_blank, so.max_initial_ts);
+  if (script) snprintf(key + strlen(key), sizeof(key) - strlen(key), "/script/%u/%d", script->seed, script->pattern);
   GraphEntry& ge = c->graphs[key];
   if (!ge.exec) {
     const long before = gemm_launch_count() + dec_gemm_launch_count() + wgemm_launch_count() + other_launch_count();
@@ -1823,7 +1839,7 @@ static cudaGraphExec_t decode_graph(wl_ctx* c, const char* tag, int B, int Kr, i
     cudaGraph_t body = np.conditional.phGraph_out[0];
     WL_CUDA(cudaStreamBeginCaptureToGraph(st, body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal));
     try {
-      decode_step(c, B, Kr, so, vi, nsplit, false);
+      token_step(c, B, Kr, so, vi, nsplit, script);
       loop_condition(st, c->ds, h, B);
     } catch (...) {
       cudaStreamEndCapture(st, &cap);
@@ -1840,24 +1856,37 @@ static cudaGraphExec_t decode_graph(wl_ctx* c, const char* tag, int B, int Kr, i
   return ge.exec;
 }
 
-extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int32_t* prompts, const int32_t* prompt_off,
-                           const wl_gen_opts* o, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
-                           int32_t* out_steps) {
-  API_BEGIN(c)
+// round(K * patience) of a beam search, half away from zero like CT2's std::round [recalled, not pinned]; at least 1
+static int max_candidates(int K, float patience, const char* who) {
+  if (K == 1) return 1;
+  const long mc = std::max(1L, lroundf(K * patience));
+  WL_CHECK(mc <= MAX_FINISHED, WL_ERR_ARG, "%s: round(beam_size * patience) = %ld exceeds the limit of %d finished hypotheses",
+           who, mc, MAX_FINISHED);
+  return (int)mc;
+}
+
+// wl_generate and wl_test_search.  `script` == nullptr: the decoder computes the logits of every step from the encoder
+// slots; otherwise the scripted logits replace the decoder and no slot is read (slots may be null).  Everything else --
+// the uploads, decode_init, the captured or host-driven loop, the search kernels, the hypothesis ranking -- is the same
+// code for both.  out_hyp_count [B] (optional): hypotheses each stream finished with; out_logits (optional, script only):
+// the [B * rows per stream][vocab_ld] logits of the first decode step.
+static void generate_run(wl_ctx* c, const int32_t* slots, int32_t B, const int32_t* prompts, const int32_t* prompt_off,
+                         const wl_gen_opts* o, const SearchScript* script, int32_t* out_ids, int32_t* out_len, float* out_score,
+                         float* out_no_speech, int32_t* out_steps, int32_t* out_hyp_count, float* out_logits) {
   WL_CHECK(c->finalized, WL_ERR_STATE, "weights not finalized");
-  WL_CHECK(slots && prompts && prompt_off && o && out_ids && out_len && out_score, WL_ERR_ARG, "wl_generate: null argument");
+  WL_CHECK((slots || script) && prompts && prompt_off && o && out_ids && out_len && out_score, WL_ERR_ARG, "wl_generate: null argument");
   WL_CHECK(B >= 1 && B <= c->Bm, WL_ERR_ARG, "wl_generate: B=%d exceeds max_streams=%d", B, c->Bm);
   WL_CHECK(o->beam_size >= 1 && o->num_hypotheses >= 1, WL_ERR_ARG, "wl_generate: beam_size / num_hypotheses must be >= 1");
   const int K = o->beam_size;
   const int Kr = K > 1 ? K : o->num_hypotheses;
   WL_CHECK(Kr <= c->Km, WL_ERR_ARG, "wl_generate: %d rows per stream exceed max_beam=%d", Kr, c->Km);
-  WL_CHECK(K == 1 || o->num_hypotheses <= MAX_HYPS, WL_ERR_ARG, "too many hypotheses");
+  WL_CHECK(K == 1 || o->num_hypotheses <= MAX_FINISHED, WL_ERR_ARG, "too many hypotheses");
   WL_CHECK(o->sampling_topk == 0 || o->sampling_topk == 1, WL_ERR_ARG, "sampling_topk must be 0 (full) or 1 (arg-max)");
   WL_CHECK(o->max_length >= 2 && o->max_length <= T_MAX, WL_ERR_ARG, "max_length %d out of range", o->max_length);
   const int R = B * Kr;
   SearchOpts so;
   so.beam = K; so.rows_per_stream = Kr;
-  so.max_cand = std::max(1, std::min(MAX_HYPS, (int)lroundf(K * o->patience)));
+  so.max_cand = max_candidates(K, o->patience, "wl_generate");
   so.suppress_blank = o->suppress_blank; so.max_initial_ts = o->max_initial_timestamp_index;
   so.suppress_mask = c->suppress_mask;
   const int sample = (K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f) ? 1 : 0;
@@ -1871,15 +1900,19 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
     if (t >= 0 && t < c->V) mask[t >> 5] |= 1u << (t & 31);
   }
   int max_new = 0;
-  int max_steps = upload_streams(c, slots, B, prompts, prompt_off, o->max_length, false, sample, o->sampling_temperature, o->seed, Kr,
-                                 o->max_length_per_stream, &max_new);
+  int max_steps = upload_streams(c, script ? nullptr : slots, B, prompts, prompt_off, o->max_length, false, sample,
+                                 o->sampling_temperature, o->seed, Kr, o->max_length_per_stream, &max_new);
   // K8: every prompt position but the last goes through the decoder in ONE batched pass (prefill = 2: one decode step per
   // prompt token)
   const bool prefilled = o->prefill == 0 || o->prefill == 1;
   if (prefilled) max_steps = max_new;
   WL_CUDA(cudaMemcpyAsync(c->suppress_mask, mask.data(), nwords * 4, cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaEventRecord(c->ev0, st));
-  if (prefilled) {
+  if (prefilled && script) {
+    // the batched prefill pass is what writes the no-speech probability of a stream whose sot precedes its last token
+    WL_CUDA(cudaMemsetAsync(c->ds.no_speech, 0, B * sizeof(float), st));
+    scripted_no_speech(st, c->ds, vi, *script, B);
+  } else if (prefilled) {
     // upload_streams staged the prompts in pinned host memory: h_int = [B][T_MAX] tokens, then the per-stream metadata
     WL_CUDA(cudaStreamSynchronize(st));
     const int* hp = c->h_int;
@@ -1887,6 +1920,10 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
     prefill_forward(c, B, Kr, hp, meta + 1 * B, meta + 2 * B, slots);
   }
   decode_init(st, c->ds, so, vi, B, R, prefilled ? 1 : 0);
+  if (script && out_logits) {   // a pure function of the state: the first step below recomputes the same values
+    scripted_logits(st, c->ds, so, vi, *script, c->logits, R);
+    WL_CUDA(cudaMemcpyAsync(out_logits, c->logits, (size_t)R * c->Vld * sizeof(float), cudaMemcpyDeviceToHost, st));
+  }
   const int nsplit = cross_attn_pick_nsplit(B, c->H, c->num_sms, Kr);
 
   // The whole token loop is ONE graph launch: a conditional WHILE node whose body is the captured decode step; the
@@ -1895,7 +1932,7 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
   // host launches the steps itself and checks for the end every 4 steps.
   cudaGraphExec_t exec = nullptr;
   long graph_kernels = 0;
-  if (o->use_cuda_graph) exec = decode_graph(c, "g", B, Kr, K, so, vi, nsplit, &graph_kernels);
+  if (o->use_cuda_graph) exec = decode_graph(c, script ? "t" : "g", B, Kr, K, so, vi, nsplit, &graph_kernels, script);
   ensure_host(c, (size_t)B * (T_MAX + 16) + (size_t)B * MAX_HYPS * (T_MAX + 2) + 64, (size_t)B * (MAX_HYPS + 2));
   int* h_done = c->h_int;  // reuse (prompts are already on the device: the copies above are stream-ordered)
   WL_CUDA(cudaStreamSynchronize(st));
@@ -1911,7 +1948,7 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
     const int check_every = 4;
     while (ran < max_steps) {
       const int n = std::min(check_every, max_steps - ran);
-      for (int i = 0; i < n; ++i) decode_step(c, B, Kr, so, vi, nsplit, false);
+      for (int i = 0; i < n; ++i) token_step(c, B, Kr, so, vi, nsplit, script);
       ran += n;
       WL_CUDA(cudaMemcpyAsync(h_done, c->ds.n_done, sizeof(int), cudaMemcpyDeviceToHost, st));
       WL_CUDA(cudaStreamSynchronize(st));
@@ -1948,7 +1985,29 @@ extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int
               out_score + (size_t)b * o->num_hypotheses);
     if (out_no_speech) out_no_speech[b] = h_ns[b];
     if (out_steps) out_steps[b] = h_steps[b];
+    if (out_hyp_count) out_hyp_count[b] = h_cnt[b];
   }
+}
+
+extern "C" int wl_generate(wl_ctx* c, const int32_t* slots, int32_t B, const int32_t* prompts, const int32_t* prompt_off,
+                           const wl_gen_opts* o, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
+                           int32_t* out_steps) {
+  API_BEGIN(c)
+  WL_CHECK(slots, WL_ERR_ARG, "wl_generate: null argument");
+  generate_run(c, slots, B, prompts, prompt_off, o, nullptr, out_ids, out_len, out_score, out_no_speech, out_steps, nullptr, nullptr);
+  API_END(c)
+}
+
+extern "C" int wl_test_search(wl_ctx* c, int32_t B, const int32_t* prompts, const int32_t* prompt_off, const wl_gen_opts* o,
+                              const wl_search_script* script, int32_t* out_ids, int32_t* out_len, float* out_score,
+                              float* out_no_speech, int32_t* out_steps, int32_t* out_hyp_count, float* out_logits) {
+  API_BEGIN(c)
+  WL_CHECK(script, WL_ERR_ARG, "wl_test_search: null script");
+  WL_CHECK(script->pattern >= -1 && script->pattern <= 5, WL_ERR_ARG, "wl_test_search: pattern %d out of range", script->pattern);
+  SearchScript sc;
+  sc.seed = script->seed; sc.pattern = script->pattern;
+  generate_run(c, nullptr, B, prompts, prompt_off, o, &sc, out_ids, out_len, out_score, out_no_speech, out_steps, out_hyp_count,
+               out_logits);
   API_END(c)
 }
 
@@ -1980,7 +2039,7 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   WL_CHECK(o->beam_size >= 1 && o->num_hypotheses >= 1, WL_ERR_ARG, "wl_session_open: beam_size / num_hypotheses must be >= 1");
   const int K = o->beam_size, Kr = K > 1 ? K : o->num_hypotheses;
   WL_CHECK(Kr <= c->Km, WL_ERR_ARG, "wl_session_open: %d rows per stream exceed max_beam=%d", Kr, c->Km);
-  WL_CHECK(K == 1 || o->num_hypotheses <= MAX_HYPS, WL_ERR_ARG, "too many hypotheses");
+  WL_CHECK(K == 1 || o->num_hypotheses <= MAX_FINISHED, WL_ERR_ARG, "too many hypotheses");
   // the session's own search is beam or greedy: sampling is chosen per stream at admission (wl_session_admit_ex), where
   // each sampled stream brings the seed and noise key its draws are keyed by
   WL_CHECK(!(K == 1 && o->sampling_topk == 0 && o->sampling_temperature > 0.f), WL_ERR_ARG,
@@ -1998,7 +2057,7 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   ss.use_graph = o->use_cuda_graph;
   SearchOpts& so = ss.so;
   so.beam = K; so.rows_per_stream = Kr;
-  so.max_cand = std::max(1, std::min(MAX_HYPS, (int)lroundf(K * o->patience)));
+  so.max_cand = max_candidates(K, o->patience, "wl_session_open");
   so.suppress_blank = o->suppress_blank; so.max_initial_ts = o->max_initial_timestamp_index;
   so.suppress_mask = ss.mask;
   ss.nsplit = cross_attn_pick_nsplit(capacity, c->H, c->num_sms, Kr);

@@ -8,7 +8,10 @@ constexpr int T_MAX = 448;      // decoder positions
 constexpr int S_ENC = 1500;     // encoder positions
 constexpr int S_PAD = 1536;     // padded key dimension for materialised attention scores
 constexpr int MAX_ROWS_PER_STREAM = 8;
-constexpr int MAX_HYPS = 16;
+constexpr int MAX_FINISHED = 16;   // largest round(K * patience): a beam search ends once it has this many hypotheses
+// Hypothesis table of a stream: a step may close up to K hypotheses while fewer than max_cand exist, so the table
+// holds max_cand - 1 + K <= MAX_FINISHED - 1 + MAX_ROWS_PER_STREAM entries (rounded up to 24).
+constexpr int MAX_HYPS = MAX_FINISHED + MAX_ROWS_PER_STREAM;
 constexpr int MAX_CAND = 16;    // 2 * beam, beam <= 8
 
 // ---------------------------------------------------------------------------- K1 mel
@@ -181,6 +184,18 @@ int cross_attn_pick_nsplit(int B, int H, int num_sms, int rows_per_stream);
 // K12: per-row masked log-softmax + top candidates, then per-stream beam / greedy update.
 void search_rows(cudaStream_t st, const DecodeState& s, const float* logits, const SearchOpts& o, const VocabIds& v, int R);
 void search_streams(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, int B);
+
+// Test only (wl_test_search): the logits of every row as a pure function of the tokens the row has consumed, in place of
+// the decoder's (tests/search_script.py restates it).  Inactive rows and the padding columns are NaN.
+struct SearchScript {
+  uint32_t seed;
+  int pattern;   // 0 none, 1 one thread's strided set, 2 one float4 group, 3 vocabulary tail, 4 1/4 grid, 5 dominant; -1 mixed
+};
+void scripted_logits(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, const SearchScript& sc,
+                     float* logits, int R);
+// no_speech[b] = softmax(scripted logits of prompt[0 .. sot])[no_speech] for every stream whose sot precedes its last
+// prompt token (what the batched prefill writes in production)
+void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B);
 
 // Last node of the loop body of the conditional WHILE graph: keep iterating while some stream is still decoding and the
 // step budget is not used up (one thread; it runs after search_streams, so n_done is final for this step).

@@ -309,7 +309,9 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
 
   if (tid == 0) {
     s.steps_run[b] += 1;
-    if (fed == s.sot_index[b]) s.no_speech[b] = s.nospeech_row[row0];
+    // the probability at the sot position: when sot is the last prompt token, fed stays there for the whole search and
+    // only the first decode step's row is that position
+    if (fed == s.sot_index[b] && (fed < P - 1 || s.step[b] == 0)) s.no_speech[b] = s.nospeech_row[row0];
   }
   // ---- teacher-forced feeding only (detect_language / align / logits hook)
   if (s.force_len[b] > 0) {
@@ -510,6 +512,145 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
 
 void search_streams(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, int B) {
   launch_kernel(search_streams_kernel, dim3(B), dim3(128), 0, st, s, o, v);
+  note_launch(1);
+}
+
+// ============================================================================ scripted logits (wl_test_search only)
+// A row's logits are a pure function of the tokens it has consumed: prompt[0 .. fed] while the prompt is fed, then the
+// whole prompt and the row's generated tokens.  Every value is an exact fp32 number (a multiple of 2^-11), so
+// tests/search_script.py reproduces them bit for bit.  h = lowbias32(FNV-1a(seed, tokens)) picks, per step:
+//   base(t)   = ((lowbias32(h ^ t * 0x9E3779B1) >> 20) - 2048) / 256, a 1/256 grid over [-8, 8)
+//   + a timestamp bias and an EOT bias from 4-entry tables (bits 0-1 / 2-3), + 10 on no_speech after sot (bit 4);
+//   a pattern (SearchScript::pattern, or bits 5.. of h when it is -1) that puts the top candidates where the selection
+//   code is fragile; and, on a row that searches, 60 + base / 8 on every token some rule must mask at this step, so a
+//   missed mask changes the arg-max.
+__constant__ float SCRIPT_TS_BIAS[4] = {-8.f, -5.f, -2.f, 2.f};
+__constant__ float SCRIPT_EOT_BIAS[4] = {-8.f, -2.f, 2.f, 8.f};
+
+struct ScriptRow {
+  uint32_t h, g;
+  int pattern, after_sot, search;
+  MaskCtx c;   // the rules of this step (search != 0)
+};
+
+// h of the first n tokens of `prompt` followed by the first glen of `gen`
+__device__ uint32_t script_hash(uint32_t seed, const int* prompt, int n, const int* gen, int glen) {
+  uint32_t h = (2166136261u ^ seed) * 16777619u;
+  for (int i = 0; i < n; ++i) h = (h ^ (uint32_t)prompt[i]) * 16777619u;
+  for (int i = 0; i < glen; ++i) h = (h ^ (uint32_t)gen[i]) * 16777619u;
+  return hash_u32(h);
+}
+
+__device__ void script_row_setup(ScriptRow& w, uint32_t h, int last, const SearchScript& sc) {
+  w.h = h;
+  w.g = hash_u32(h ^ 0x5BD1E995u);
+  w.pattern = sc.pattern >= 0 ? sc.pattern : (int)((h >> 5) % 6u);
+  w.after_sot = last;
+}
+
+__device__ __forceinline__ float script_quarter(float x) { return floorf(x * 4.f) * 0.25f; }
+
+__device__ float script_logit(int t, const ScriptRow& w, const VocabIds& v) {
+  const float base = (float)((int)(hash_u32(w.h ^ ((uint32_t)t * 0x9E3779B1u)) >> 20) - 2048) * (1.f / 256.f);
+  if (w.search) {
+    const bool sup = (w.c.suppress[t >> 5] >> (t & 31)) & 1u;
+    const bool ts_masked = w.c.use_ts && t >= v.ts_begin &&
+                           (w.c.first ? t > v.ts_begin + w.c.max_initial : (w.c.has_ts && t < w.c.ts_cutoff));
+    if (sup || ts_masked || (w.c.use_ts && t == v.no_timestamps) || (w.c.suppress_blank && (t == v.blank || t == v.eot)))
+      return 60.f + base * 0.125f;
+  }
+  float x = base;
+  if (t >= v.ts_begin) x += SCRIPT_TS_BIAS[w.h & 3u];
+  else if (t == v.eot) x += SCRIPT_EOT_BIAS[(w.h >> 2) & 3u];
+  else if (t == v.no_speech && w.after_sot && ((w.h >> 4) & 1u)) x += 10.f;
+  switch (w.pattern) {
+    case 1: if (((t % 4096) >> 2) == (int)(w.g % 1024u)) x = 8.f + script_quarter(base); break;
+    case 2: if ((t >> 2) == (int)(w.g % (uint32_t)(v.vocab >> 2))) x = 8.f + script_quarter(base); break;
+    case 3: if (t >= v.vocab - 8) x = 8.f + script_quarter(base); break;
+    case 4: x = script_quarter(x); break;
+    case 5: {
+      const int d = (int)(w.g % (uint32_t)v.eot), d2 = (d + 1 + (int)((w.g >> 24) & 63u)) % v.eot;
+      if (t == d || (((w.h >> 7) & 1u) && t == d2)) x = 48.f;
+      break;
+    }
+    default: break;
+  }
+  return x;
+}
+
+__global__ void __launch_bounds__(256) scripted_logits_kernel(DecodeState s, SearchOpts o, VocabIds v, SearchScript sc,
+                                                              float* __restrict__ logits) {
+  const int r = blockIdx.x, b = r / o.rows_per_stream, tid = threadIdx.x;
+  float* out = logits + (long)r * v.vocab_ld;
+  __shared__ ScriptRow w;
+  // wait first: the state comes from the previous step's search_streams, and search_rows (launched as soon as every
+  // CTA here has triggered) reads its per-step flags before its own wait
+  pdl_wait();
+  pdl_trigger();
+  if (!s.active[r] || s.done[b]) {
+    for (int t = tid; t < v.vocab_ld; t += blockDim.x) out[t] = __int_as_float(0x7fc00000);
+    return;
+  }
+  if (tid == 0) {
+    const int fed = s.fed[b], P = s.prompt_len[b];
+    const int* prompt = s.prompt + (long)b * T_MAX;
+    const int glen = fed >= P - 1 ? s.gen_len[r] : 0;
+    const int* hist = s.hist + (long)r * T_MAX;
+    const int last = glen > 0 ? hist[glen - 1] : prompt[fed];
+    script_row_setup(w, script_hash(sc.seed, prompt, fed + 1, hist, glen), last == v.sot, sc);
+    w.search = fed >= P - 1;
+    // the rules of search_rows_kernel for this row
+    MaskCtx& c = w.c;
+    const int npre = s.pre_n[b], nhist = glen + npre;
+    c.suppress = o.suppress_mask;
+    c.first = nhist == 0;
+    c.suppress_blank = o.suppress_blank && glen == 0;
+    c.use_ts = s.use_ts[b];
+    c.max_initial = o.max_initial_ts;
+    const int penult = glen > 1 ? hist[glen - 2] : (glen == 1 ? s.pre_last[b] : s.pre_penult[b]);
+    const int plast = glen > 0 ? last : s.pre_last[b];
+    c.last_is_ts = nhist > 0 && plast >= v.ts_begin;
+    c.penult_is_ts = nhist < 2 || penult >= v.ts_begin;
+    const int lts = s.last_ts[r];
+    c.has_ts = lts >= 0;
+    c.ts_cutoff = (c.last_is_ts && !c.penult_is_ts) ? lts : lts + 1;
+  }
+  __syncthreads();
+  for (int t = tid; t < v.vocab_ld; t += blockDim.x) out[t] = t < v.vocab ? script_logit(t, w, v) : __int_as_float(0x7fc00000);
+}
+
+void scripted_logits(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, const SearchScript& sc,
+                     float* logits, int R) {
+  launch_kernel(scripted_logits_kernel, dim3(R), dim3(256), 0, st, s, o, v, sc, logits);
+  note_launch(1);
+}
+
+__global__ void __launch_bounds__(256) scripted_no_speech_kernel(DecodeState s, VocabIds v, SearchScript sc) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int sot = s.sot_index[b];
+  if (sot < 0 || sot >= s.prompt_len[b] - 1) return;
+  __shared__ ScriptRow w;
+  __shared__ float red[2 * 8];
+  if (tid == 0) {
+    script_row_setup(w, script_hash(sc.seed, s.prompt + (long)b * T_MAX, sot + 1, nullptr, 0), 1, sc);
+    w.search = 0;
+  }
+  __syncthreads();
+  float m = -INFINITY, sm = 0.f;
+  for (int t = tid; t < v.vocab; t += blockDim.x) lse_merge(m, sm, script_logit(t, w, v), 1.f);
+#pragma unroll
+  for (int off = 16; off > 0; off >>= 1) lse_merge(m, sm, __shfl_xor_sync(0xffffffffu, m, off), __shfl_xor_sync(0xffffffffu, sm, off));
+  if ((tid & 31) == 0) { red[tid >> 5] = m; red[8 + (tid >> 5)] = sm; }
+  __syncthreads();
+  if (tid == 0) {
+    for (int i = 1; i < 8; ++i) lse_merge(m, sm, red[i], red[8 + i]);
+    s.no_speech[b] = __expf(script_logit(v.no_speech, w, v) - m) / sm;
+  }
+}
+
+void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B) {
+  scripted_no_speech_kernel<<<B, 256, 0, st>>>(s, v, sc);
+  WL_CUDA(cudaGetLastError());
   note_launch(1);
 }
 

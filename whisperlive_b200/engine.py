@@ -112,7 +112,8 @@ def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 
     NS = int(enc_slots) if enc_slots is not None else 2 * B
     d, H, Le, Ld, nm, V = dims.d_model, dims.n_heads, dims.enc_layers, dims.dec_layers, dims.n_mels, dims.vocab
     ff, dd, S, S_PAD, T = 4 * d, d * d, 1500, 1536, T_MAX
-    MAX_HYPS, MAX_CAND, MAX_ROWS, PEEK_STRIDE = 16, 16, 8, 8 + 2 * 16 + T_MAX
+    MAX_HYPS, MAX_CAND, MAX_ROWS = 24, 16, 8          # csrc/kernels.cuh
+    PEEK_STRIDE = 8 + 2 * MAX_HYPS + T_MAX
     if n_align_heads is None:
         n_align_heads = len(dims.default_alignment_heads())
     f32 = i32 = 4
@@ -189,6 +190,19 @@ def mem_info(device: int = 0) -> Tuple[int, int]:
     if rc != 0:
         raise _lib.WlError(f"wl_mem_info failed ({rc}): {lib.wl_last_error(None).decode()}")
     return int(free.value), int(total.value)
+
+
+def _gen_opts(beam_size, patience, num_hypotheses, length_penalty, max_length, suppress_blank, max_initial_timestamp_index,
+              sampling_topk, sampling_temperature, seed, sup: np.ndarray, use_cuda_graph, prefill) -> "_lib.WlGenOpts":
+    """wl_gen_opts of a generate call (``sup`` must outlive the call; ``max_length_per_stream`` is left unset)."""
+    return _lib.WlGenOpts(
+        beam_size=int(beam_size), patience=float(patience), num_hypotheses=int(num_hypotheses),
+        length_penalty=float(length_penalty), max_length=int(max_length), suppress_blank=int(bool(suppress_blank)),
+        max_initial_timestamp_index=int(max_initial_timestamp_index), sampling_topk=int(sampling_topk),
+        sampling_temperature=float(sampling_temperature), seed=int(seed) & 0xFFFFFFFF,
+        suppress_tokens=_lib.ptr(sup, C.c_int32) if len(sup) else None, n_suppress=len(sup),
+        use_cuda_graph=int(use_cuda_graph), max_length_per_stream=None,
+        prefill=0 if prefill is None else (1 if prefill else 2))
 
 
 class B200Whisper:
@@ -565,14 +579,8 @@ class B200Whisper:
             off[1:] = np.cumsum([len(p) for p in ps])
             flat = np.asarray([t for p in ps for t in p], dtype=np.int32)
             slots = np.asarray(enc.slots[b0:b0 + B], dtype=np.int32)
-            opts = _lib.WlGenOpts(
-                beam_size=int(beam_size), patience=float(patience), num_hypotheses=NH, length_penalty=float(length_penalty),
-                max_length=int(max_length), suppress_blank=int(bool(suppress_blank)),
-                max_initial_timestamp_index=int(max_initial_timestamp_index), sampling_topk=int(sampling_topk),
-                sampling_temperature=float(sampling_temperature), seed=int(seed) & 0xFFFFFFFF,
-                suppress_tokens=_lib.ptr(sup, C.c_int32) if len(sup) else None, n_suppress=len(sup),
-                use_cuda_graph=int(self.use_cuda_graph), max_length_per_stream=None,
-                prefill=0 if prefill is None else (1 if prefill else 2))
+            opts = _gen_opts(beam_size, patience, NH, length_penalty, max_length, suppress_blank, max_initial_timestamp_index,
+                             sampling_topk, sampling_temperature, seed, sup, self.use_cuda_graph, prefill)
             mlps = None
             if max_length_per_stream is not None:
                 mlps = np.asarray(list(max_length_per_stream)[b0:b0 + B], dtype=np.int32)
@@ -675,6 +683,55 @@ class B200Whisper:
                                            _lib.ptr(off, C.c_int32), _lib.ptr(out, C.c_float))
             _lib.check(self.lib, self.ctx, rc, "wl_decode_logits")
         return [out[off[b]:off[b + 1]] for b in range(B)]
+
+    def test_search(self, prompts: Sequence[Sequence[int]], script: Tuple[int, int], *, beam_size: int = 5, patience: float = 1,
+                    num_hypotheses: int = 1, length_penalty: float = 1, max_length: int = 448,
+                    max_initial_timestamp_index: int = 50, suppress_blank: bool = True,
+                    suppress_tokens: Optional[Sequence[int]] = (), sampling_topk: int = 1, sampling_temperature: float = 1,
+                    seed: int = 0, max_length_per_stream: Optional[Sequence[int]] = None, prefill: Optional[bool] = None,
+                    use_cuda_graph: Optional[bool] = None, return_logits: bool = False
+                    ) -> Tuple[List[WhisperGenerationResult], List[int], Optional[np.ndarray]]:
+        """``generate`` on scripted logits (wl_test_search): ``script = (seed, pattern)`` of the function that
+        tests/search_script.py restates replaces the decoder; no encoder output is needed.  At most ``max_streams``
+        prompts.  Returns the results, the hypothesis count of every stream and, with ``return_logits``, the logits of
+        the first decode step [B * rows per stream, (vocab + 3) // 4 * 4]."""
+        ps = [list(map(int, p)) for p in prompts]
+        B = len(ps)
+        if not 1 <= B <= self.max_streams:
+            raise ValueError(f"{B} prompts for max_streams={self.max_streams}")
+        NH = int(num_hypotheses)
+        Kr = int(beam_size) if int(beam_size) > 1 else NH
+        off = np.zeros(B + 1, dtype=np.int32)
+        off[1:] = np.cumsum([len(p) for p in ps])
+        flat = np.asarray([t for p in ps for t in p], dtype=np.int32)
+        sup = np.asarray(sorted({int(t) for t in (suppress_tokens or ()) if t >= 0}), dtype=np.int32)
+        graph = self.use_cuda_graph if use_cuda_graph is None else use_cuda_graph
+        opts = _gen_opts(beam_size, patience, NH, length_penalty, max_length, suppress_blank, max_initial_timestamp_index,
+                         sampling_topk, sampling_temperature, seed, sup, graph, prefill)
+        mlps = None
+        if max_length_per_stream is not None:
+            mlps = np.asarray(list(max_length_per_stream), dtype=np.int32)
+            opts.max_length_per_stream = _lib.ptr(mlps, C.c_int32)
+        sc = _lib.WlSearchScript(seed=int(script[0]) & 0xFFFFFFFF, pattern=int(script[1]))
+        ids = np.zeros((B, NH, T_MAX), dtype=np.int32)
+        lens = np.zeros((B, NH), dtype=np.int32)
+        score = np.zeros((B, NH), dtype=np.float32)
+        nsp = np.zeros(B, dtype=np.float32)
+        steps = np.zeros(B, dtype=np.int32)
+        nhyp = np.zeros(B, dtype=np.int32)
+        logits = np.empty((B * Kr, (self.dims.vocab + 3) // 4 * 4), dtype=np.float32) if return_logits else None
+        with self._lock:
+            rc = self.lib.wl_test_search(self.ctx, B, _lib.ptr(flat, C.c_int32), _lib.ptr(off, C.c_int32), C.byref(opts),
+                                         C.byref(sc), _lib.ptr(ids, C.c_int32), _lib.ptr(lens, C.c_int32),
+                                         _lib.ptr(score, C.c_float), _lib.ptr(nsp, C.c_float), _lib.ptr(steps, C.c_int32),
+                                         _lib.ptr(nhyp, C.c_int32), None if logits is None else _lib.ptr(logits, C.c_float))
+            _lib.check(self.lib, self.ctx, rc, "wl_test_search")
+        results = []
+        for b in range(B):
+            keep = [h for h in range(NH) if lens[b, h] >= 0]
+            results.append(WhisperGenerationResult([ids[b, h, :lens[b, h]].tolist() for h in keep],
+                                                   [float(score[b, h]) for h in keep], float(nsp[b]), int(steps[b])))
+        return results, nhyp.tolist(), logits
 
     def test_wgemm(self, w: np.ndarray, x: np.ndarray, bias: Optional[np.ndarray] = None, mode: int = 0,
                    resid: Optional[np.ndarray] = None) -> np.ndarray:
