@@ -15,6 +15,7 @@
  *   wl_slots_release     <- StorageView lifetime           transcriber_faster_whisper.py:1055, :1820-1823
  *   wl_vad               <- faster_whisper.vad.get_speech_timestamps (the Silero model call) transcriber_faster_whisper.py:830-838
  *   wl_spk_embed         <- SpeakerDiarizer._compute_embedding (pyannote Inference)  diarization.py:100-118
+ *   wl_mt_translate      <- ServeClientTranslation.translate_text (M2M100 generate)  backend/translation_backend.py:73-100
  *
  * Conventions: plain pointers and sizes only; the caller owns every host buffer; the library owns
  * device memory, streams, CUDA graphs.  Every function returns 0 or a negative WL_ERR_* code and
@@ -30,7 +31,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 10
+#define WL_ABI_VERSION 11
 
 typedef struct wl_ctx wl_ctx;
 
@@ -337,6 +338,65 @@ int wl_test_spk_fbank(wl_ctx* ctx, const float* pcm, const int64_t* offsets, int
 int wl_test_spk_conv(wl_ctx* ctx, const uint16_t* x_f16, const int64_t* frames, int32_t B, int32_t H_in, int32_t C_in,
                      int32_t C_out, int32_t ksize, int32_t stride, const uint16_t* w_f16, const float* bias,
                      const uint16_t* res_f16, int32_t relu, uint16_t* out_f16);
+
+/* Translation: an M2M100 encoder-decoder (SMaLL-100) with Hugging Face's beam search, in a context of its own (one per
+ * process, shared by every connection; it belongs to no Whisper model).  wl_mt_load_tensor takes float32 host tensors
+ * under the engine's names (whisperlive_b200/translation.py maps the checkpoint onto them):
+ *   shared [vocab, d] (token embedding and LM head)     positions [max_positions + 2, d] (sinusoidal table, pad row zero;
+ *   a source token's row is pad + its count of non-pad tokens so far, a decoder token's pad + 1 + its position)
+ *   enc.L.{ln1,ln2}.{w,b} [d]   enc.L.qkv.w [3d, d]  enc.L.qkv.b [3d]  enc.L.out.{w [d, d], b [d]}
+ *   enc.L.fc1.{w [ffn, d], b [ffn]}  enc.L.fc2.{w [d, ffn], b [d]}  enc.ln.{w,b} [d]
+ *   dec.L.{ln1,ln2,ln3}.{w,b}, dec.L.qkv.*, dec.L.out.*, dec.L.xq.{w [d, d], b}, dec.L.xout.*, dec.L.fc1.*, dec.L.fc2.*,
+ *   dec.ln.{w,b}, dec.xkv.w [dec_layers * 2d, d] and dec.xkv.b [dec_layers * 2d] (layer L's cross K then V)
+ * wl_mt_translate: B segments of source ids packed at src_off[B+1] (each 1 .. max_positions - 2 tokens, at most
+ * max_src_tokens in all, B <= capacity_segments; opts->max_length <= max_positions + 1); out_ids [B][opts->max_length] receives the best hypothesis of each
+ * segment without the decoder start token (EOS included when it ended on one), out_len its length, out_score its
+ * length-normalised score (beam search) or cumulative log-probability (greedy).  One upload, one download; the token
+ * loop is one CUDA graph whose loop ends on the device.  A segment's result does not depend on the other segments. */
+typedef struct wl_mt_ctx wl_mt_ctx;
+
+typedef struct wl_mt_config {
+  int32_t abi_version;   /* WL_ABI_VERSION */
+  int32_t d_model, n_heads, enc_layers, dec_layers, ffn, vocab, max_positions;
+  int32_t pad_id;        /* padding_idx: the zero row of the position table */
+  float embed_scale;     /* sqrt(d_model) with scale_embedding, else 1 */
+  int32_t max_src_tokens;/* packed source tokens per call */
+} wl_mt_config;
+
+typedef struct wl_mt_opts {
+  int32_t num_beams;     /* 1 = greedy, <= max_beam */
+  int32_t max_length;    /* decoder start token included, <= 448 */
+  float length_penalty;
+  int32_t early_stopping;/* 0 False, 1 True, 2 "never" */
+  int32_t decoder_start, eos, forced_bos, forced_eos; /* -1: no forced token */
+  int32_t use_cuda_graph;
+} wl_mt_opts;
+
+int wl_mt_init(const wl_mt_config* config, int32_t device, int32_t capacity_segments, int32_t max_beam, wl_mt_ctx** out);
+void wl_mt_destroy(wl_mt_ctx* ctx);
+const char* wl_mt_last_error(wl_mt_ctx* ctx);
+int wl_mt_load_tensor(wl_mt_ctx* ctx, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+int wl_mt_finalize(wl_mt_ctx* ctx);
+int wl_mt_device_bytes(wl_mt_ctx* ctx, int64_t* out);
+int wl_mt_translate(wl_mt_ctx* ctx, const int32_t* src_ids, const int32_t* src_off, int32_t B, const wl_mt_opts* opts,
+                    int32_t* out_ids, int32_t* out_len, float* out_score);
+/* Test hook: the encoder self-attention launch.  qkv fp16 [n][3 * 64 H] (q | k | v) of B segments at off[B+1] ->
+ * out fp16 [n][64 H] (uploaded as given, copied back whole). */
+int wl_test_mt_attn(wl_mt_ctx* ctx, const uint16_t* qkv_f16, const int32_t* off, int32_t B, int32_t H, uint16_t* out_f16);
+/* Test hook: the decoder cross-attention launch.  q fp32 [R][64 H], kv fp16 [n][ldkv] with K at column koff and V at
+ * voff, B segments at off[B+1], row r of segment r / rows_per_seg -> out fp16 [R][64 H] (uploaded, copied back whole). */
+int wl_test_mt_cross_attn(wl_mt_ctx* ctx, const float* q, const uint16_t* kv_f16, int32_t ldkv, int32_t koff, int32_t voff,
+                          const int32_t* off, int32_t B, int32_t rows_per_seg, int32_t H, uint16_t* out_f16);
+/* Test hook: teacher-forced logits.  The encoder of wl_mt_translate over B segments, then the decoder (one row per
+ * segment) fed prefix [B][P] token by token (position t at step t) -> out_logits [B][P][vocab], the logits after each
+ * prefix token. */
+int wl_test_mt_logits(wl_mt_ctx* ctx, const int32_t* src_ids, const int32_t* src_off, int32_t B, const int32_t* prefix,
+                      int32_t P, float* out_logits);
+/* Test hook: wl_mt_translate's search launches on scripted logits [opts->max_length - 1][B * num_beams][V] (step t's
+ * logits of row r at [t][r]) in place of the decoder's.  Outputs as wl_mt_translate's; out_steps [B]: the running length
+ * (cur_len) at which each segment stopped. */
+int wl_test_mt_search(wl_mt_ctx* ctx, const float* logits, int32_t V, int32_t B, const wl_mt_opts* opts, int32_t* out_ids,
+                      int32_t* out_len, float* out_score, int32_t* out_steps);
 
 #ifdef __cplusplus
 }

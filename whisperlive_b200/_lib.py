@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 10
+ABI_VERSION = 11
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -44,6 +44,22 @@ class WlStreamSearch(C.Structure):
     _fields_ = [
         ("sample", C.c_int32), ("num_hypotheses", C.c_int32), ("temperature", C.c_float), ("seed", C.c_uint32),
         ("noise_key", C.c_int32),
+    ]
+
+
+class WlMtConfig(C.Structure):
+    _fields_ = [
+        ("abi_version", C.c_int32), ("d_model", C.c_int32), ("n_heads", C.c_int32), ("enc_layers", C.c_int32),
+        ("dec_layers", C.c_int32), ("ffn", C.c_int32), ("vocab", C.c_int32), ("max_positions", C.c_int32),
+        ("pad_id", C.c_int32), ("embed_scale", C.c_float), ("max_src_tokens", C.c_int32),
+    ]
+
+
+class WlMtOpts(C.Structure):
+    _fields_ = [
+        ("num_beams", C.c_int32), ("max_length", C.c_int32), ("length_penalty", C.c_float), ("early_stopping", C.c_int32),
+        ("decoder_start", C.c_int32), ("eos", C.c_int32), ("forced_bos", C.c_int32), ("forced_eos", C.c_int32),
+        ("use_cuda_graph", C.c_int32),
     ]
 
 
@@ -111,6 +127,19 @@ SIGNATURES = {
     "wl_test_spk_fbank": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p]),
     "wl_test_spk_conv": (C.c_int, [C.c_void_p, c_u16p, c_i64p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                    C.c_int32, c_u16p, c_f32p, c_u16p, C.c_int32, c_u16p]),
+    "wl_mt_init": (C.c_int, [C.POINTER(WlMtConfig), C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]),
+    "wl_mt_destroy": (None, [C.c_void_p]),
+    "wl_mt_last_error": (C.c_char_p, [C.c_void_p]),
+    "wl_mt_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
+    "wl_mt_finalize": (C.c_int, [C.c_void_p]),
+    "wl_mt_device_bytes": (C.c_int, [C.c_void_p, c_i64p]),
+    "wl_mt_translate": (C.c_int, [C.c_void_p, c_i32p, c_i32p, C.c_int32, C.POINTER(WlMtOpts), c_i32p, c_i32p, c_f32p]),
+    "wl_test_mt_attn": (C.c_int, [C.c_void_p, c_u16p, c_i32p, C.c_int32, C.c_int32, c_u16p]),
+    "wl_test_mt_cross_attn": (C.c_int, [C.c_void_p, c_f32p, c_u16p, C.c_int32, C.c_int32, C.c_int32, c_i32p, C.c_int32,
+                                        C.c_int32, C.c_int32, c_u16p]),
+    "wl_test_mt_logits": (C.c_int, [C.c_void_p, c_i32p, c_i32p, C.c_int32, c_i32p, C.c_int32, c_f32p]),
+    "wl_test_mt_search": (C.c_int, [C.c_void_p, c_f32p, C.c_int32, C.c_int32, C.POINTER(WlMtOpts), c_i32p, c_i32p, c_f32p,
+                                    c_i32p]),
 }
 
 _lock = threading.Lock()

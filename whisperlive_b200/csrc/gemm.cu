@@ -94,6 +94,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
 #pragma unroll
         for (int i = 0; i < cnt; ++i) x[i] = gelu_erf(x[i]);
       }
+      if (e.relu) {
+#pragma unroll
+        for (int i = 0; i < cnt; ++i) x[i] = fmaxf(x[i], 0.f);
+      }
       if (e.resid) {
         const float* r = e.resid + rbase + n0;
         float4 r4[cnt / 4];
@@ -130,6 +134,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
             float x1 = __uint_as_float(v[i + j]) + bm;
             if (e.bias && !e.bias_on_m) x1 += e.bias[n + j];
             if (e.gelu) x1 = gelu_erf(x1);
+            if (e.relu) x1 = fmaxf(x1, 0.f);
             if (e.resid) x1 += e.resid[rbase + n + j];
             if (e.out_f32) ((float*)e.out)[obase + n + j] = x1;
             else ((__half*)e.out)[obase + n + j] = __float2half_rn(x1);
@@ -148,6 +153,10 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
       if (e.gelu) {
 #pragma unroll
         for (int j = 0; j < 8; ++j) x[j] = gelu_erf(x[j]);
+      }
+      if (e.relu) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) x[j] = fmaxf(x[j], 0.f);
       }
       if (e.resid) {
         const float* r = e.resid + rbase + n;
@@ -176,6 +185,7 @@ __device__ __forceinline__ void epilogue_chunk(const GemmKParams& p, long m, int
     float x = __uint_as_float(v[i]) + bm;
     if (e.bias && !e.bias_on_m) x += e.bias[n];
     if (e.gelu) x = gelu_erf(x);
+    if (e.relu) x = fmaxf(x, 0.f);
     if (e.resid) x += e.resid[rbase + (long)n * e.rldn];
     const long o = obase + (long)n * e.ldn;
     if (e.out_f32) ((float*)e.out)[o] = x;
@@ -630,7 +640,7 @@ static GemmKParams make_params(const GemmOperand& A, const GemmOperand& B, int M
     p.vec_ok = ok ? 1 : 0;
   }
   if (epi.mode == GEMM_HEADSPLIT) {
-    WL_CHECK(!epi.out_f32 && !epi.gelu && !epi.resid && !epi.bias_on_m && N % 64 == 0 && epi.hs_slots, WL_ERR_ARG,
+    WL_CHECK(!epi.out_f32 && !epi.gelu && !epi.relu && !epi.resid && !epi.bias_on_m && N % 64 == 0 && epi.hs_slots, WL_ERR_ARG,
              "gemm_tn: bad head-split epilogue");
   }
   return p;

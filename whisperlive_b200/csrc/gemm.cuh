@@ -31,6 +31,7 @@ struct GemmEpilogue {
   const float* bias = nullptr;
   int bias_on_m = 0;         // bias indexed by m (swap-AB) instead of n
   int gelu = 0;              // exact erf GELU after bias
+  int relu = 0;              // max(x, 0) after bias (M2M100 feed-forward)
   const float* resid = nullptr;  // fp32 residual added last; same indexing scheme as out
   long rldm = 0, rldn = 1, rb1 = 0, rb2 = 0;
   int mode = GEMM_STORE;

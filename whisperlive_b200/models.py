@@ -61,11 +61,14 @@ class ModelRegistry:
     def __init__(self, factory: Callable[[str], object], *, max_streams: int = 8, batch_window_ms: int = 20,
                  resolve: Optional[Callable[[str], str]] = None, footprint: Optional[Callable[[str], Optional[int]]] = None,
                  mem_probe: Optional[Callable[[int], int]] = None, devices: Sequence[int] = (0,),
-                 reserve_bytes: int = 0, clock: Callable[[], float] = time.monotonic):
+                 reserve_bytes: int = 0, clock: Callable[[], float] = time.monotonic,
+                 translator_pending: Optional[Callable[[int], int]] = None):
         """``factory(name)`` builds a transcriber.  ``resolve(name)`` gives the key of a name (default: the name).
         ``footprint(name)`` the device bytes one copy of the model needs (None: unknown, loaded without a check).
         ``mem_probe(device)`` the free bytes of a device (default ``wl_mem_info``).  ``devices``: where every model is
-        placed (one copy per device).  ``reserve_bytes``: kept free beyond the footprint."""
+        placed (one copy per device).  ``reserve_bytes``: kept free beyond the footprint.  ``translator_pending(device)``:
+        the bytes the process-wide translator will still allocate there (default: its footprint while
+        ``WLB200_TRANSLATE=device`` and it is not loaded yet)."""
         self.factory = factory
         self.max_streams = int(max_streams)
         self.batch_window_ms = batch_window_ms
@@ -75,6 +78,9 @@ class ModelRegistry:
         self.devices = [int(d) for d in devices] or [0]
         self.reserve_bytes = int(reserve_bytes)
         self.clock = clock
+        if translator_pending is None:
+            from .translation import pending_translator_bytes as translator_pending
+        self.translator_pending = translator_pending
         self._lock = threading.Lock()          # entries, loads in progress, connection counts
         self._load_lock = threading.Lock()     # one check-evict-load at a time: two loads never count the same free bytes
         self._entries: Dict[str, ModelEntry] = {}
@@ -160,10 +166,11 @@ class ModelRegistry:
             return ModelEntry(key, name, transcriber, scheduler, need)
 
     def _pending_bytes(self, device: int) -> int:
-        """What the resident models will still allocate on ``device``: footprint minus the bytes each holds now."""
+        """What the resident models will still allocate on ``device``: footprint minus the bytes each holds now, and
+        the translator's footprint until it is loaded."""
         with self._lock:
             entries = list(self._entries.values())
-        pending = 0
+        pending = int(self.translator_pending(device))
         for e in entries:
             if e.footprint is None:
                 continue
