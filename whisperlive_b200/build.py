@@ -10,7 +10,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libwlb200.so")
-SOURCES = ["gemm.cu", "dec_gemm.cu", "wgemm.cu", "mel.cu", "elementwise.cu", "attention.cu", "flash_attn.cu", "search.cu", "prefill.cu", "misc.cu", "vad.cu", "spk.cu", "mt.cu", "engine.cu", "mt_engine.cu"]
+SOURCES = ["gemm.cu", "dec_gemm.cu", "wgemm.cu", "mel.cu", "elementwise.cu", "attention.cu", "flash_attn.cu", "search.cu", "prefill.cu", "misc.cu", "vad.cu", "spk.cu", "mt.cu", "engine.cu", "vad_engine.cu", "spk_engine.cu", "hooks.cu", "mt_engine.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "--expt-relaxed-constexpr",
          "-Xcompiler", "-fPIC"]

@@ -1,26 +1,18 @@
-// libwlb200 engine: context, weights, encoder (K2-K7), decoder loop (K8-K13), alignment (K14) and
-// the C ABI declared in include/wlb200.h.
-#include <algorithm>
+// libwlb200 engine: context, weights, encoder (K2-K7), decoder loop (K8-K13), alignment (K14) and their C ABI
+// (include/wlb200.h).  Silero VAD, speaker embeddings and the kernel test hooks are in vad_engine.cu, spk_engine.cu and
+// hooks.cu.
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
-#include <map>
-#include <string>
 #include <thread>
-#include <vector>
 
-#include "../../include/wlb200.h"
-#include "gemm.cuh"
-#include "kernels.cuh"
-
-using namespace wl;
+#include "ctx.cuh"
 
 namespace wl {
 void gemm_prime();
 void attention_prime();
 void search_prime();
 void flash_attn_prime();
-void encoder_attention_fused(cudaStream_t st, const __half* qk, const __half* vt, __half* out, int nb, int H, int d);
 long other_launch_count();
 void gemm_tl_bind(unsigned long long* p);
 void attention_tl_bind(unsigned long long* p);
@@ -30,219 +22,19 @@ void search_tl_bind(unsigned long long* p);
 
 static std::string g_init_error;
 
-struct EncLayer {
-  __half *w_qk, *w_v, *w_o, *w_fc1, *w_fc2;
-  float *b_qk, *b_v, *b_o, *b_fc1, *b_fc2, *ln1_g, *ln1_b, *ln2_g, *ln2_b;
-};
-struct DecLayer {
-  __half *w_qkv, *w_o, *w_qc, *w_kc, *w_vc, *w_oc, *w_fc1, *w_fc2;
-  float *b_qkv, *b_o, *b_qc, *b_vc, *b_oc, *b_fc1, *b_fc2;
-  float *ln1_g, *ln1_b, *ln2_g, *ln2_b, *ln3_g, *ln3_b;
-};
-
-struct GraphEntry {
-  cudaGraphExec_t exec = nullptr;
-  long kernels = 0;  // kernel nodes per replay
-};
-
 // Rows of the per-stream metadata table of a decode call (stream_meta / search_meta -> upload_state_tables):
 // slot, len, sot_index, use_ts, n_new, force_len, pre_n, pre_last, pre_penult, pre_lts, then the stream's search:
 // smode, temperature (float bits), noise seed, noise key, rows
 constexpr int META_ROWS = 15;
 
-struct wl_ctx {
-  wl_config cfg;
-  std::vector<int32_t> align_heads;
-  std::string err;
-  cudaStream_t st = nullptr;
-  cudaEvent_t ev0 = nullptr, ev1 = nullptr;
-  float last_ms[10] = {};   // [0] mel, [1] encode, [2] generate / session run, [5] session admit (prefill),
-                            // [6] / [7] VAD front end / recurrence, [8] / [9] speaker embedding front end / network
-  // per-kernel profiling of the dominant decode kernel (bench.py roofline): events around every cross-attention launch
-  int prof_cross = 0;
-  cudaEvent_t pev0 = nullptr, pev1 = nullptr;
-  double prof_cross_ms = 0.0;
-  long prof_cross_n = 0;
-  int num_sms = 132;
-  int d, H, Le, Ld, n_mels, V, Vld, Bm, Km, Rm, NS;
-  bool finalized = false;
-  // every device buffer the context holds and its size in bytes (dalloc); dev_bytes is their sum plus the weight-load
-  // staging buffer while it exists -- what wl_device_bytes reports
-  std::vector<std::pair<void*, size_t>> allocs;
-  int64_t dev_bytes = 0;
-  std::map<std::string, void*> dev;                 // raw uploaded tensors (fp16 for ndim>=2, f32 for 1-D)
-  std::map<std::string, std::vector<int64_t>> shape;
-  long graph_launched = 0;   // kernels executed through graph replays
-  long capture_counted = 0;  // launcher calls that were captured, not executed
-
-  // weights
-  __half *w_conv1 = nullptr, *w_conv2 = nullptr, *emb = nullptr, *pos_dec = nullptr;
-  float *b_conv1, *b_conv2, *pos_enc, *lnp_g, *lnp_b, *lnf_g, *lnf_b;
-  std::vector<EncLayer> enc;
-  std::vector<DecLayer> dec;
-  // mel
-  float *mel_window, *mel_twiddle, *mel_filt;
-  int* mel_range;
-  float* mel_pcm = nullptr;
-  float* mel_out = nullptr;
-  long *mel_off = nullptr, *mel_ooff = nullptr;
-  unsigned* mel_gmax = nullptr;
-  long mel_pcm_cap = 0, mel_out_cap = 0;
-  int mel_last_B = 0, mel_last_frames = 0;
-  // encoder workspaces
-  int EB, AB;
-  float* feat32;
-  __half *feat16, *conv1o, *xn, *qk, *vt, *probs16, *attn, *hbuf;
-  float *x, *scores;
-  int* enc_slots_dev;
-  // slot pool
-  __half* enc16;   // [NS][1500][d]
-  __half* ckv;     // [Ld][2][NS][H][1500][64]
-  std::vector<int> slot_free;
-  std::vector<char> slot_used;
-  // decoder workspaces
-  float *dx, *part1, *part2, *logits;
-  __half *dxn, *datt, *dh, *kcache, *vcache;
-  long cache_row_stride, cache_layer_stride;
-  CrossAttnWorkspace xws;
-  float* align_probs = nullptr;   // [R][H][1500]
-  float* align_buf = nullptr;     // [B][nh][T_MAX][1500]
-  long align_buf_cap = 0;
-  int* align_heads_dev = nullptr;
-  DecodeState ds;
-  unsigned* suppress_mask;
-  // pinned host staging
-  int* h_int = nullptr;     // generic int staging
-  float* h_flt = nullptr;
-  size_t h_int_cap = 0, h_flt_cap = 0;
-  std::map<std::string, GraphEntry> graphs;
-  // WLB200_TIMELINE: in-graph per-kernel timestamps (common.cuh), dumped after every wl_generate
-  unsigned long long* tl_dev = nullptr;
-  std::string tl_path;
-  // resident log-mel of the last wl_mel_device call (features never leave the GPU between mel and encoder)
-  float *res_pcm = nullptr, *res_mel = nullptr;
-  long res_pcm_cap = 0, res_mel_cap = 0;
-  long *res_off = nullptr, *res_ooff = nullptr;
-  int *res_frames = nullptr, *win_meta = nullptr;
-  std::vector<int> res_frames_h;
-  // K8 batched prefill workspaces (allocated on first use, grown on demand)
-  struct Prefill {
-    long cap_rows = 0;
-    int *tok = nullptr, *pos = nullptr, *active = nullptr, *wrow = nullptr, *vslot = nullptr, *vdone = nullptr, *sel = nullptr;
-    short* src = nullptr;
-    float *x = nullptr, *qkv = nullptr, *qc = nullptr, *xpart = nullptr;
-    __half *xn = nullptr, *att = nullptr, *h = nullptr;
-    long rows_done = 0, calls = 0;   // statistics
-    // K14 (align through the batched pass)
-    int* row_b = nullptr;
-    long row_b_cap = 0;
-    float *aprobs = nullptr, *mat = nullptr, *tokp = nullptr;
-    int *aT = nullptr, *anf = nullptr, *path = nullptr, *path_len = nullptr;
-    long tokp_cap = 0;
-  } pf;
-  // Silero VAD: its own weights (wl_vad_load_tensor, independent of the Whisper weights and of finalize) and workspaces
-  // grown on demand, at least to max_streams x 30 s on first use
-  struct Vad {
-    float* t[15] = {};            // device tensors in VAD_TENSORS order, kernel layout
-    float *pcm = nullptr, *gx = nullptr, *probs = nullptr;
-    long* off = nullptr;          // [2][off_cap]: pcm offsets, frame offsets
-    long pcm_cap = 0, frame_cap = 0, off_cap = 0;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  } vad;
-  // Speaker embedding: its own weights (wl_spk_load_tensor) and workspaces grown on demand, at least to max_streams x 30 s
-  // on first use
-  struct Spk {
-    std::vector<void*> t;         // device tensors in spk_tensors() order: conv weights fp16 [co][taps][ci] (the stem fp32
-                                  // [32][9]), biases fp32, seg_1 fp32 transposed [5120][256]
-    float *melw = nullptr, *pcm = nullptr, *feat = nullptr, *mean = nullptr, *pooled = nullptr, *emb = nullptr;
-    int* mel_range = nullptr;
-    __half *act[3] = {nullptr, nullptr, nullptr};
-    long* off = nullptr;          // [6][off_cap]: pcm, frame and the four stages' position offsets
-    long pcm_cap = 0, frame_cap = 0, act_cap[3] = {0, 0, 0}, stream_cap = 0;
-    cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
-  } spk;
-  float* stage_f32 = nullptr;   // wl_load_tensor staging (freed by wl_finalize_weights)
-  size_t stage_cap = 0;
-  // Decode session (N2, step-level continuous batching): a second decode state + self-attention cache whose stream
-  // indices are admitted, decoded for a bounded number of token steps and collected independently of each other.
-  // One-shot calls (wl_generate / wl_align / wl_detect_language) keep using `ds` / `kcache`, so they may run between two
-  // wl_session_run calls without disturbing the streams in flight.
-  struct Session {
-    bool allocated = false, open = false;
-    int cap = 0, K = 1, Kr = 1, NH = 1, nsplit = 1, use_graph = 1;
-    float length_penalty = 1.f;
-    SearchOpts so;
-    DecodeState ds;
-    __half *kcache = nullptr, *vcache = nullptr;
-    unsigned* mask = nullptr;
-    int* idx_dev = nullptr;
-    int* peek_dev = nullptr;            // wl_session_peek staging [max_streams][PEEK_STRIDE]
-    std::vector<int> hp, meta;          // host shadows: prompts [cap][T_MAX], per-stream metadata [META_ROWS][cap]
-    std::vector<char> used, finished;   // index holds an admitted stream / that stream has finished decoding
-    std::vector<int> nh;                // hypotheses the index's stream returns: N when it samples, else NH
-    int live = 0;                       // admitted and still decoding
-    long steps = 0, runs = 0, admitted = 0;
-  } sess;
-};
-
-#define API_BEGIN(ctx)                                          \
-  if (!(ctx)) return WL_ERR_ARG;                                \
-  try {                                                         \
-    WL_CUDA(cudaSetDevice((ctx)->cfg.device));
-#define API_END(ctx)                                            \
-  }                                                             \
-  catch (const wl::Error& e) {                                  \
-    (ctx)->err = e.msg;                                         \
-    return e.code;                                              \
-  }                                                             \
-  catch (const std::exception& e) {                             \
-    (ctx)->err = e.what();                                      \
-    return WL_ERR_STATE;                                        \
-  }                                                             \
-  return WL_OK;
-
-template <class T>
-static T* dalloc(wl_ctx* c, size_t n, bool zero = true) {
-  void* p = nullptr;
-  const size_t bytes = std::max<size_t>(n, 1) * sizeof(T);
-  cudaError_t e = cudaMalloc(&p, bytes);
-  if (e != cudaSuccess) {
-    cudaGetLastError();   // an out-of-memory cudaMalloc is not sticky: leave no error behind for the next call
-    char b[256];
-    snprintf(b, sizeof(b), "cudaMalloc of %.1f MB failed: %s", n * sizeof(T) / 1048576.0, cudaGetErrorString(e));
-    throw wl::Error{WL_ERR_NOMEM, b};
-  }
-  c->allocs.push_back({p, bytes});
-  c->dev_bytes += (int64_t)bytes;
-  if (zero) WL_CUDA(cudaMemset(p, 0, bytes));
-  return (T*)p;
-}
-
-// Frees the buffers dalloc made after the first `mark` ones (a wl_finalize_weights that failed part-way) and the
-// weight-load staging buffer.
-static void free_allocs_from(wl_ctx* c, size_t mark) {
-  if (c->allocs.size() > mark || c->stage_f32) cudaDeviceSynchronize();
-  while (c->allocs.size() > mark) {
-    cudaFree(c->allocs.back().first);
-    c->dev_bytes -= (int64_t)c->allocs.back().second;
-    c->allocs.pop_back();
-  }
-  if (c->stage_f32) {
-    cudaFree(c->stage_f32);
-    c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
-    c->stage_f32 = nullptr;
-    c->stage_cap = 0;
-  }
-}
-
 // Everything a context owns on the device and the host, and the context itself: wl_destroy, and wl_init when it
 // fails part-way.
 static void free_ctx(wl_ctx* c) {
-  if (c->st || !c->allocs.empty()) cudaSetDevice(c->cfg.device);
+  if (c->st || !c->mem.list.empty()) cudaSetDevice(c->mem.device);
   if (c->st) cudaStreamSynchronize(c->st);
   for (auto& g : c->graphs)
     if (g.second.exec) cudaGraphExecDestroy(g.second.exec);
-  free_allocs_from(c, 0);
+  c->mem.release_from(0);
   if (c->h_int) cudaFreeHost(c->h_int);
   if (c->h_flt) cudaFreeHost(c->h_flt);
   if (c->ev0) cudaEventDestroy(c->ev0);
@@ -273,22 +65,22 @@ static void ensure_host(wl_ctx* c, size_t n_int, size_t n_flt) {
 // device-resident decode state for Bm streams x Km rows (one per context, plus one per decode session)
 static void alloc_decode_state(wl_ctx* c, DecodeState& s) {
   const size_t R = c->Rm, B = c->Bm;
-  s.tok_in = dalloc<int>(c, R); s.pos = dalloc<int>(c, R); s.active = dalloc<int>(c, R); s.cum = dalloc<float>(c, R);
-  s.gen_len = dalloc<int>(c, R); s.last_ts = dalloc<int>(c, R); s.row_done = dalloc<int>(c, R);
-  s.hist = dalloc<int>(c, R * T_MAX); s.src = dalloc<short>(c, R * T_MAX);
-  s.cand_val = dalloc<float>(c, R * MAX_CAND); s.cand_tok = dalloc<int>(c, R * MAX_CAND);
-  s.nospeech_row = dalloc<float>(c, R);
-  s.slot = dalloc<int>(c, B); s.prompt = dalloc<int>(c, B * T_MAX); s.prompt_len = dalloc<int>(c, B);
-  s.fed = dalloc<int>(c, B); s.sot_index = dalloc<int>(c, B); s.use_ts = dalloc<int>(c, B); s.n_new = dalloc<int>(c, B);
-  s.step = dalloc<int>(c, B); s.done = dalloc<int>(c, B); s.n_alive = dalloc<int>(c, B); s.no_speech = dalloc<float>(c, B);
-  s.hyp_count = dalloc<int>(c, B); s.hyp_cum = dalloc<float>(c, B * MAX_HYPS); s.hyp_len = dalloc<int>(c, B * MAX_HYPS);
-  s.hyp_tok = dalloc<int>(c, B * MAX_HYPS * T_MAX); s.steps_run = dalloc<int>(c, B); s.n_done = dalloc<int>(c, 1);
-  s.force_len = dalloc<int>(c, B); s.force_prob = dalloc<float>(c, B * T_MAX);
-  s.steps_left = dalloc<int>(c, 1);
-  s.smode = dalloc<int>(c, B); s.temp = dalloc<float>(c, B); s.nseed = dalloc<unsigned>(c, B); s.nkey = dalloc<int>(c, B);
-  s.nrows = dalloc<int>(c, B);
-  s.pre_n = dalloc<int>(c, B); s.pre_last = dalloc<int>(c, B); s.pre_penult = dalloc<int>(c, B); s.pre_lts = dalloc<int>(c, B);
-  s.brk = dalloc<int>(c, 2);
+  s.tok_in = c->mem.alloc<int>(R); s.pos = c->mem.alloc<int>(R); s.active = c->mem.alloc<int>(R); s.cum = c->mem.alloc<float>(R);
+  s.gen_len = c->mem.alloc<int>(R); s.last_ts = c->mem.alloc<int>(R); s.row_done = c->mem.alloc<int>(R);
+  s.hist = c->mem.alloc<int>(R * T_MAX); s.src = c->mem.alloc<short>(R * T_MAX);
+  s.cand_val = c->mem.alloc<float>(R * MAX_CAND); s.cand_tok = c->mem.alloc<int>(R * MAX_CAND);
+  s.nospeech_row = c->mem.alloc<float>(R);
+  s.slot = c->mem.alloc<int>(B); s.prompt = c->mem.alloc<int>(B * T_MAX); s.prompt_len = c->mem.alloc<int>(B);
+  s.fed = c->mem.alloc<int>(B); s.sot_index = c->mem.alloc<int>(B); s.use_ts = c->mem.alloc<int>(B); s.n_new = c->mem.alloc<int>(B);
+  s.step = c->mem.alloc<int>(B); s.done = c->mem.alloc<int>(B); s.n_alive = c->mem.alloc<int>(B); s.no_speech = c->mem.alloc<float>(B);
+  s.hyp_count = c->mem.alloc<int>(B); s.hyp_cum = c->mem.alloc<float>(B * MAX_HYPS); s.hyp_len = c->mem.alloc<int>(B * MAX_HYPS);
+  s.hyp_tok = c->mem.alloc<int>(B * MAX_HYPS * T_MAX); s.steps_run = c->mem.alloc<int>(B); s.n_done = c->mem.alloc<int>(1);
+  s.force_len = c->mem.alloc<int>(B); s.force_prob = c->mem.alloc<float>(B * T_MAX);
+  s.steps_left = c->mem.alloc<int>(1);
+  s.smode = c->mem.alloc<int>(B); s.temp = c->mem.alloc<float>(B); s.nseed = c->mem.alloc<unsigned>(B); s.nkey = c->mem.alloc<int>(B);
+  s.nrows = c->mem.alloc<int>(B);
+  s.pre_n = c->mem.alloc<int>(B); s.pre_last = c->mem.alloc<int>(B); s.pre_penult = c->mem.alloc<int>(B); s.pre_lts = c->mem.alloc<int>(B);
+  s.brk = c->mem.alloc<int>(2);
 }
 
 // ------------------------------------------------------------------------------------------ init
@@ -307,6 +99,7 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
              cudaGetErrorString(e));
     WL_CHECK(cfg->device >= 0 && cfg->device < ndev, WL_ERR_ARG, "device %d out of range (%d devices)", cfg->device, ndev);
     WL_CUDA(cudaSetDevice(cfg->device));
+    c->mem.device = cfg->device;
     cudaDeviceProp prop;
     WL_CUDA(cudaGetDeviceProperties(&prop, cfg->device));
     WL_CHECK(prop.major == 9 && prop.minor == 0, WL_ERR_CUDA, "libwlb200 is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
@@ -319,6 +112,7 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     WL_CHECK(c->Km >= 1 && c->Km <= MAX_ROWS_PER_STREAM, WL_ERR_ARG, "max_beam %d must be in [1,%d]", c->Km, MAX_ROWS_PER_STREAM);
     WL_CHECK(c->Bm >= 1 && c->NS >= c->Bm, WL_ERR_ARG, "enc_slots %d must be >= max_streams %d", c->NS, c->Bm);
     WL_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
+    c->mem.st = c->st;
     WL_CUDA(cudaEventCreate(&c->ev0));
     WL_CUDA(cudaEventCreate(&c->ev1));
     gemm_prime();
@@ -329,10 +123,7 @@ extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
     flash_attn_prime();
     if (const char* tl = getenv("WLB200_TIMELINE")) {
       c->tl_path = tl;
-      WL_CUDA(cudaMalloc((void**)&c->tl_dev, (size_t)(TL_CAP + 1) * 8));
-      c->allocs.push_back({c->tl_dev, (size_t)(TL_CAP + 1) * 8});
-      c->dev_bytes += (int64_t)(TL_CAP + 1) * 8;
-      WL_CUDA(cudaMemset(c->tl_dev, 0, (size_t)(TL_CAP + 1) * 8));
+      c->tl_dev = c->mem.alloc<unsigned long long>(TL_CAP + 1);
       gemm_tl_bind(c->tl_dev); dec_gemm_tl_bind(c->tl_dev); wgemm_tl_bind(c->tl_dev); attention_tl_bind(c->tl_dev); elementwise_tl_bind(c->tl_dev); search_tl_bind(c->tl_dev);
     }
     c->enc.resize(c->Le);
@@ -356,7 +147,7 @@ extern "C" void wl_destroy(wl_ctx* c) {
 
 extern "C" int wl_device_bytes(wl_ctx* c, int64_t* out) {
   if (!c || !out) return WL_ERR_ARG;
-  *out = c->dev_bytes;
+  *out = c->mem.bytes;
   return WL_OK;
 }
 
@@ -388,12 +179,9 @@ extern "C" int64_t wl_kernel_launches(wl_ctx* c) {
 }
 extern "C" float wl_last_device_ms(wl_ctx* c, int32_t which) {
   if (!c) return -1.f;
-  if (which >= 0 && which < 3) return c->last_ms[which];
   if (which == 3) return c->prof_cross_n > 0 ? (float)(c->prof_cross_ms / (double)c->prof_cross_n) : -1.f;   // avg ms per cross-attention launch
   if (which == 4) return (float)c->prof_cross_n;
-  if (which == 5) return c->last_ms[5];   // last wl_session_admit (upload + batched prefill + init)
-  if (which == 6 || which == 7) return c->last_ms[which];   // last wl_vad: front end / recurrence
-  if (which == 8 || which == 9) return c->last_ms[which];   // last wl_spk_embed: fbank + CMN / network
+  if (which >= 0 && which < 10) return c->last_ms[which];   // the calls wl_ctx::last_ms lists
   return -1.f;
 }
 extern "C" int wl_profile_cross_attn(wl_ctx* c, int32_t enable) {
@@ -419,23 +207,15 @@ extern "C" int wl_load_tensor(wl_ctx* c, const char* name, const float* data, co
   for (auto s : sh) n *= (size_t)s;
   const bool as_f32 = ndim == 1 || nm == "model.encoder.embed_positions.weight" || nm == "mel_filters";
   if (as_f32) {
-    float* p = dalloc<float>(c, n, false);
+    float* p = c->mem.alloc<float>(n, false);
     WL_CUDA(cudaMemcpy(p, data, n * sizeof(float), cudaMemcpyHostToDevice));
     c->dev[nm] = p;
   } else {
     // fp32 -> fp16 (and the conv re-layout) on the device: the host only hands over its buffer.  A large-v3 load
     // is 1.5 G values; converting them on one host thread took longer than everything else in wl_init together.
-    if (n > c->stage_cap) {
-      if (c->stage_f32) cudaFree(c->stage_f32);
-      c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
-      c->stage_f32 = nullptr;
-      c->stage_cap = 0;
-      WL_CUDA(cudaMalloc((void**)&c->stage_f32, n * sizeof(float)));
-      c->stage_cap = n;
-      c->dev_bytes += (int64_t)(n * sizeof(float));
-    }
+    c->mem.grow(c->stage_f32, c->stage_cap, (long)n);
     WL_CUDA(cudaMemcpyAsync(c->stage_f32, data, n * sizeof(float), cudaMemcpyHostToDevice, c->st));
-    __half* p = dalloc<__half>(c, n, false);
+    __half* p = c->mem.alloc<__half>(n, false);
     if (ndim == 3) cast_weight_f16(c->st, c->stage_f32, p, sh[0], sh[1], sh[2]);   // [co][ci][k] -> [co][k][ci]
     else cast_weight_f16(c->st, c->stage_f32, p, (long)n, 1, 1);
     WL_CUDA(cudaStreamSynchronize(c->st));
@@ -456,7 +236,7 @@ static void* need(wl_ctx* c, const std::string& nm, std::initializer_list<int64_
 static __half* concat_h(wl_ctx* c, std::vector<std::pair<__half*, size_t>> parts) {
   size_t tot = 0;
   for (auto& p : parts) tot += p.second;
-  __half* out = dalloc<__half>(c, tot, false);
+  __half* out = c->mem.alloc<__half>(tot, false);
   size_t o = 0;
   for (auto& p : parts) {
     WL_CUDA(cudaMemcpy(out + o, p.first, p.second * sizeof(__half), cudaMemcpyDeviceToDevice));
@@ -467,7 +247,7 @@ static __half* concat_h(wl_ctx* c, std::vector<std::pair<__half*, size_t>> parts
 static float* concat_f(wl_ctx* c, std::vector<std::pair<float*, size_t>> parts) {
   size_t tot = 0;
   for (auto& p : parts) tot += p.second;
-  float* out = dalloc<float>(c, tot, true);
+  float* out = c->mem.alloc<float>(tot, true);
   size_t o = 0;
   for (auto& p : parts) {
     if (p.first) WL_CUDA(cudaMemcpy(out + o, p.first, p.second * sizeof(float), cudaMemcpyDeviceToDevice));
@@ -484,8 +264,8 @@ static void build_mel_tables(wl_ctx* c) {
     tw[2 * i] = (float)cos(2.0 * PI * i / 400.0);
     tw[2 * i + 1] = (float)sin(2.0 * PI * i / 400.0);
   }
-  c->mel_window = dalloc<float>(c, 400);
-  c->mel_twiddle = dalloc<float>(c, 800);
+  c->mel_window = c->mem.alloc<float>(400);
+  c->mel_twiddle = c->mem.alloc<float>(800);
   WL_CUDA(cudaMemcpy(c->mel_window, win.data(), 400 * 4, cudaMemcpyHostToDevice));
   WL_CUDA(cudaMemcpy(c->mel_twiddle, tw.data(), 800 * 4, cudaMemcpyHostToDevice));
   c->mel_filt = (float*)need(c, "mel_filters", {c->n_mels, 201});
@@ -499,32 +279,35 @@ static void build_mel_tables(wl_ctx* c) {
     if (lo > hi) lo = hi = 0;
     rg[2 * m] = lo; rg[2 * m + 1] = hi;
   }
-  c->mel_range = dalloc<int>(c, rg.size());
+  c->mel_range = c->mem.alloc<int>(rg.size());
   WL_CUDA(cudaMemcpy(c->mel_range, rg.data(), rg.size() * 4, cudaMemcpyHostToDevice));
-  c->mel_gmax = dalloc<unsigned>(c, c->Bm);
-  c->res_off = dalloc<long>(c, c->Bm + 1);
-  c->res_ooff = dalloc<long>(c, c->Bm + 1);
-  c->res_frames = dalloc<int>(c, c->Bm);
-  c->win_meta = dalloc<int>(c, 3 * (size_t)c->Bm);
-  c->mel_off = dalloc<long>(c, c->Bm + 1);
-  c->mel_ooff = dalloc<long>(c, c->Bm + 1);
+  c->mel_gmax = c->mem.alloc<unsigned>(c->Bm);
+  c->res_off = c->mem.alloc<long>(c->Bm + 1);
+  c->res_ooff = c->mem.alloc<long>(c->Bm + 1);
+  c->res_frames = c->mem.alloc<int>(c->Bm);
+  c->win_meta = c->mem.alloc<int>(3 * (size_t)c->Bm);
+  c->mel_off = c->mem.alloc<long>(c->Bm + 1);
+  c->mel_ooff = c->mem.alloc<long>(c->Bm + 1);
 }
 
 static void finalize_impl(wl_ctx* c);
 
 // streams per sub-pass of the unfused encoder attention: the fp32 scores of one stream are H x 1500 x 1536 floats
-static int enc_attn_streams(int d) { return d >= 1024 ? 2 : 4; }
+int enc_attn_streams(int d) { return d >= 1024 ? 2 : 4; }
 
-// A finalize that fails part-way (a missing tensor, an out-of-memory workspace) frees every buffer it had allocated and
-// the staging buffer before it returns: only the tensors wl_load_tensor uploaded remain, until wl_destroy.
+// The weight-load staging buffer is freed first.  A finalize that fails part-way (a missing tensor, an out-of-memory
+// workspace) frees every buffer it had allocated before it returns: only the tensors wl_load_tensor uploaded remain,
+// until wl_destroy.
 extern "C" int wl_finalize_weights(wl_ctx* c) {
   API_BEGIN(c)
   WL_CHECK(!c->finalized, WL_ERR_STATE, "weights already finalized");
-  const size_t mark = c->allocs.size();
+  c->mem.release(c->stage_f32);
+  c->stage_cap = 0;
+  const size_t mark = c->mem.list.size();
   try {
     finalize_impl(c);
   } catch (...) {
-    free_allocs_from(c, mark);
+    c->mem.release_from(mark);
     throw;
   }
   API_END(c)
@@ -594,12 +377,6 @@ static void finalize_impl(wl_ctx* c) {
     L.ln3_b = (float*)need(c, p + "final_layer_norm.bias", {d});
   }
   build_mel_tables(c);
-  if (c->stage_f32) {
-    cudaFree(c->stage_f32);
-    c->dev_bytes -= (int64_t)(c->stage_cap * sizeof(float));
-    c->stage_f32 = nullptr;
-    c->stage_cap = 0;
-  }
 
   // ---- encoder workspaces (EB streams per pass, AB streams per attention sub-pass)
   const int H = c->H;
@@ -609,40 +386,40 @@ static void finalize_impl(wl_ctx* c) {
   c->EB = std::min(c->Bm, enc_batch);
   c->AB = std::min(c->EB, enc_attn_streams(d));
   const size_t M = (size_t)c->EB * S_ENC;
-  c->feat32 = dalloc<float>(c, (size_t)c->Bm * nm * 3000);  // all streams of a call stay resident (wl_encode_resident)
-  c->feat16 = dalloc<__half>(c, (size_t)c->EB * 3002 * nm + 4096);
-  c->conv1o = dalloc<__half>(c, (size_t)c->EB * 3002 * d + 4096);
-  c->x = dalloc<float>(c, M * d);
-  c->xn = dalloc<__half>(c, M * d);
-  c->qk = dalloc<__half>(c, M * 2 * d);
-  c->vt = dalloc<__half>(c, (size_t)c->EB * d * S_PAD);
-  c->scores = dalloc<float>(c, (size_t)c->AB * H * S_ENC * S_PAD);
-  c->probs16 = dalloc<__half>(c, (size_t)c->AB * H * S_ENC * S_PAD);
-  c->attn = dalloc<__half>(c, M * d);
-  c->hbuf = dalloc<__half>(c, M * ff);
-  c->enc_slots_dev = dalloc<int>(c, c->Bm);
+  c->feat32 = c->mem.alloc<float>((size_t)c->Bm * nm * 3000);  // all streams of a call stay resident (wl_encode_resident)
+  c->feat16 = c->mem.alloc<__half>((size_t)c->EB * 3002 * nm + 4096);
+  c->conv1o = c->mem.alloc<__half>((size_t)c->EB * 3002 * d + 4096);
+  c->x = c->mem.alloc<float>(M * d);
+  c->xn = c->mem.alloc<__half>(M * d);
+  c->qk = c->mem.alloc<__half>(M * 2 * d);
+  c->vt = c->mem.alloc<__half>((size_t)c->EB * d * S_PAD);
+  c->scores = c->mem.alloc<float>((size_t)c->AB * H * S_ENC * S_PAD);
+  c->probs16 = c->mem.alloc<__half>((size_t)c->AB * H * S_ENC * S_PAD);
+  c->attn = c->mem.alloc<__half>(M * d);
+  c->hbuf = c->mem.alloc<__half>(M * ff);
+  c->enc_slots_dev = c->mem.alloc<int>(c->Bm);
   // ---- slot pool
-  c->enc16 = dalloc<__half>(c, (size_t)c->NS * S_ENC * d, false);
-  c->ckv = dalloc<__half>(c, (size_t)c->Ld * 2 * c->NS * S_ENC * d, false);
+  c->enc16 = c->mem.alloc<__half>((size_t)c->NS * S_ENC * d, false);
+  c->ckv = c->mem.alloc<__half>((size_t)c->Ld * 2 * c->NS * S_ENC * d, false);
   // ---- decoder workspaces
   const size_t R = c->Rm, Rp = (R + 15) / 16 * 16;
-  c->dx = dalloc<float>(c, R * d);
+  c->dx = c->mem.alloc<float>(R * d);
   // split-K partial sums: up to 16 K ranges of a d-wide output, 4 of the 3d-wide QKV, 3 of the 4d-wide MLP
-  c->part1 = dalloc<float>(c, R * 16 * (size_t)d + R * 4 * (size_t)ff);
-  c->part2 = dalloc<float>(c, R * 16 * (size_t)d);
-  c->logits = dalloc<float>(c, R * c->Vld);
-  c->dxn = dalloc<__half>(c, Rp * d);
-  c->datt = dalloc<__half>(c, Rp * d);
-  c->dh = dalloc<__half>(c, Rp * ff);
+  c->part1 = c->mem.alloc<float>(R * 16 * (size_t)d + R * 4 * (size_t)ff);
+  c->part2 = c->mem.alloc<float>(R * 16 * (size_t)d);
+  c->logits = c->mem.alloc<float>(R * c->Vld);
+  c->dxn = c->mem.alloc<__half>(Rp * d);
+  c->datt = c->mem.alloc<__half>(Rp * d);
+  c->dh = c->mem.alloc<__half>(Rp * ff);
   c->cache_row_stride = (long)H * T_MAX * 64;
   c->cache_layer_stride = (long)R * c->cache_row_stride;
-  c->kcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
-  c->vcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
-  c->xws.part = dalloc<float>(c, (size_t)c->Bm * H * 12 * MAX_ROWS_PER_STREAM * 66);
+  c->kcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
+  c->vcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
+  c->xws.part = c->mem.alloc<float>((size_t)c->Bm * H * 12 * MAX_ROWS_PER_STREAM * 66);
   c->xws.probs = nullptr;
-  c->suppress_mask = dalloc<unsigned>(c, (V + 31) / 32 + 1);
+  c->suppress_mask = c->mem.alloc<unsigned>((V + 31) / 32 + 1);
   if (!c->align_heads.empty()) {
-    c->align_heads_dev = dalloc<int>(c, c->align_heads.size());
+    c->align_heads_dev = c->mem.alloc<int>(c->align_heads.size());
     WL_CUDA(cudaMemcpy(c->align_heads_dev, c->align_heads.data(), c->align_heads.size() * 4, cudaMemcpyHostToDevice));
   }
   alloc_decode_state(c, c->ds);
@@ -674,14 +451,8 @@ extern "C" int wl_mel(wl_ctx* c, const float* pcm, const int64_t* offsets, int32
     WL_CHECK(out_offsets[b + 1] - out_offsets[b] == (long)T * c->n_mels, WL_ERR_ARG, "wl_mel: out_offsets do not match frames");
   }
   for (int b = 0; b <= B; ++b) ooff[b] = out_offsets[b] - out_offsets[0];
-  if (total > c->mel_pcm_cap) {
-    c->mel_pcm = dalloc<float>(c, total + total / 4, false);
-    c->mel_pcm_cap = total + total / 4;
-  }
-  if (ooff[B] > c->mel_out_cap) {
-    c->mel_out = dalloc<float>(c, ooff[B] + ooff[B] / 4, false);
-    c->mel_out_cap = ooff[B] + ooff[B] / 4;
-  }
+  c->mem.grow(c->mel_pcm, c->mel_pcm_cap, total, total + total / 4);
+  c->mem.grow(c->mel_out, c->mel_out_cap, ooff[B], ooff[B] + ooff[B] / 4);
   WL_CUDA(cudaMemcpyAsync(c->mel_pcm, pcm + offsets[0], total * sizeof(float), cudaMemcpyHostToDevice, c->st));
   WL_CUDA(cudaMemcpyAsync(c->mel_off, off.data(), (B + 1) * sizeof(long), cudaMemcpyHostToDevice, c->st));
   WL_CUDA(cudaMemcpyAsync(c->mel_ooff, ooff.data(), (B + 1) * sizeof(long), cudaMemcpyHostToDevice, c->st));
@@ -715,14 +486,8 @@ extern "C" int wl_mel_device(wl_ctx* c, const float* pcm, const int64_t* offsets
     frames_out[b] = T;
     ooff[b + 1] = ooff[b] + (long)T * c->n_mels;
   }
-  if (total > c->res_pcm_cap) {
-    c->res_pcm = dalloc<float>(c, total + total / 4, false);
-    c->res_pcm_cap = total + total / 4;
-  }
-  if (ooff[B] > c->res_mel_cap) {
-    c->res_mel = dalloc<float>(c, ooff[B] + ooff[B] / 4, false);
-    c->res_mel_cap = ooff[B] + ooff[B] / 4;
-  }
+  c->mem.grow(c->res_pcm, c->res_pcm_cap, total, total + total / 4);
+  c->mem.grow(c->res_mel, c->res_mel_cap, ooff[B], ooff[B] + ooff[B] / 4);
   cudaStream_t st = c->st;
   WL_CUDA(cudaMemcpyAsync(c->res_pcm, pcm + offsets[0], total * sizeof(float), cudaMemcpyHostToDevice, st));
   WL_CUDA(cudaMemcpyAsync(c->res_off, off.data(), (B + 1) * sizeof(long), cudaMemcpyHostToDevice, st));
@@ -780,439 +545,8 @@ extern "C" int wl_mel_resident(wl_ctx* c) {
   API_END(c)
 }
 
-// ------------------------------------------------------------------------------------------ Silero VAD
-struct VadTensor {
-  const char* name;
-  int ndim;
-  int64_t shape[3];
-  int layout;   // 0 as given, 1 [rows][k] -> [k][rows] (rows = shape[0], k = the rest), 2 conv [co][ci][3] -> [ci][3][co]
-};
-static const VadTensor VAD_TENSORS[15] = {
-    {"vad.stft.basis", 3, {258, 1, 256}, 1},   {"vad.conv0.weight", 3, {128, 129, 3}, 2}, {"vad.conv0.bias", 1, {128}, 0},
-    {"vad.conv1.weight", 3, {64, 128, 3}, 2},  {"vad.conv1.bias", 1, {64}, 0},        {"vad.conv2.weight", 3, {64, 64, 3}, 2},
-    {"vad.conv2.bias", 1, {64}, 0},            {"vad.conv3.weight", 3, {128, 64, 3}, 2}, {"vad.conv3.bias", 1, {128}, 0},
-    {"vad.lstm.weight_ih", 2, {512, 128}, 1},  {"vad.lstm.weight_hh", 2, {512, 128}, 0}, {"vad.lstm.bias_ih", 1, {512}, 0},
-    {"vad.lstm.bias_hh", 1, {512}, 0},         {"vad.out.weight", 3, {1, 128, 1}, 0},  {"vad.out.bias", 1, {1}, 0},
-};
-constexpr long VAD_CHUNK_SAMPLES = 30 * 16000;   // the workspace's first size: max_streams chunks of 30 s
-
-extern "C" int wl_vad_load_tensor(wl_ctx* c, const char* name, const float* data, const int64_t* shape, int32_t ndim) {
-  API_BEGIN(c)
-  WL_CHECK(name && data && shape && ndim >= 1, WL_ERR_ARG, "wl_vad_load_tensor: bad arguments");
-  int i = 0;
-  while (i < 15 && strcmp(VAD_TENSORS[i].name, name) != 0) ++i;
-  WL_CHECK(i < 15, WL_ERR_ARG, "wl_vad_load_tensor: unknown VAD tensor '%s'", name);
-  const VadTensor& T = VAD_TENSORS[i];
-  bool ok = ndim == T.ndim;
-  for (int k = 0; ok && k < ndim; ++k) ok = shape[k] == T.shape[k];
-  WL_CHECK(ok, WL_ERR_ARG, "wl_vad_load_tensor: '%s' must have shape [%lld%s%lld%s%lld]", name, (long long)T.shape[0],
-           T.ndim > 1 ? ", " : "", (long long)(T.ndim > 1 ? T.shape[1] : 0), T.ndim > 2 ? ", " : "",
-           (long long)(T.ndim > 2 ? T.shape[2] : 0));
-  size_t n = 1;
-  for (int k = 0; k < ndim; ++k) n *= (size_t)shape[k];
-  std::vector<float> h(n);
-  if (T.layout == 1) {
-    const size_t rows = (size_t)shape[0], kk = n / rows;
-    for (size_t r = 0; r < rows; ++r)
-      for (size_t k = 0; k < kk; ++k) h[k * rows + r] = data[r * kk + k];
-  } else if (T.layout == 2) {
-    const size_t co_n = (size_t)shape[0], ci_n = (size_t)shape[1];
-    for (size_t co = 0; co < co_n; ++co)
-      for (size_t ci = 0; ci < ci_n; ++ci)
-        for (size_t k = 0; k < 3; ++k) h[(ci * 3 + k) * co_n + co] = data[(co * ci_n + ci) * 3 + k];
-  } else {
-    std::copy(data, data + n, h.begin());
-  }
-  if (!c->vad.t[i]) c->vad.t[i] = dalloc<float>(c, n, false);
-  WL_CUDA(cudaMemcpy(c->vad.t[i], h.data(), n * sizeof(float), cudaMemcpyHostToDevice));
-  API_END(c)
-}
-
-extern "C" int wl_vad(wl_ctx* c, const float* pcm, const int64_t* offsets, int32_t B, float* probs_out, const int64_t* prob_off) {
-  API_BEGIN(c)
-  WL_CHECK(pcm && offsets && probs_out && prob_off && B >= 1, WL_ERR_ARG, "wl_vad: bad arguments (B=%d)", B);
-  for (int i = 0; i < 15; ++i)
-    WL_CHECK(c->vad.t[i], WL_ERR_STATE, "wl_vad: VAD weights not loaded: '%s' is missing (wl_vad_load_tensor)", VAD_TENSORS[i].name);
-  std::vector<long> off(2 * (B + 1));
-  long* poff = off.data();
-  long* foff = off.data() + B + 1;
-  for (int b = 0; b <= B; ++b) poff[b] = offsets[b] - offsets[0];
-  foff[0] = 0;
-  for (int b = 0; b < B; ++b) {
-    const long n = poff[b + 1] - poff[b];
-    WL_CHECK(n >= 0, WL_ERR_ARG, "wl_vad: offsets decrease at stream %d", b);
-    const long frames = n > 0 ? n / 512 + 1 : 0;
-    WL_CHECK(prob_off[b + 1] - prob_off[b] == frames, WL_ERR_ARG,
-             "wl_vad: prob_off gives stream %d %lld frames; its %ld samples have %ld", b,
-             (long long)(prob_off[b + 1] - prob_off[b]), n, frames);
-    foff[b + 1] = foff[b] + frames;
-  }
-  const long total = poff[B], frames = foff[B];
-  auto& v = c->vad;
-  if (total > v.pcm_cap) {
-    const long cap = std::max(total, (long)c->Bm * VAD_CHUNK_SAMPLES);
-    v.pcm = dalloc<float>(c, cap, false);
-    v.pcm_cap = cap;
-  }
-  if (frames > v.frame_cap) {
-    const long cap = std::max(frames, (long)c->Bm * (VAD_CHUNK_SAMPLES / 512 + 1));
-    v.gx = dalloc<float>(c, (size_t)cap * 512, false);
-    v.probs = dalloc<float>(c, cap, false);
-    v.frame_cap = cap;
-  }
-  if (2L * (B + 1) > v.off_cap) {
-    const long cap = 2L * (std::max(B, c->Bm) + 1);
-    v.off = dalloc<long>(c, cap, false);
-    v.off_cap = cap;
-  }
-  if (!v.ev[0])
-    for (auto& e : v.ev) WL_CUDA(cudaEventCreate(&e));
-  cudaStream_t st = c->st;
-  const VadWeights w{v.t[0], v.t[1], v.t[2], v.t[3], v.t[4], v.t[5], v.t[6], v.t[7], v.t[8], v.t[9], v.t[10], v.t[11],
-                     v.t[12], v.t[13], v.t[14]};
-  if (total > 0) WL_CUDA(cudaMemcpyAsync(v.pcm, pcm + offsets[0], total * sizeof(float), cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaMemcpyAsync(v.off, off.data(), off.size() * sizeof(long), cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaEventRecord(v.ev[0], st));
-  vad_front(st, w, v.pcm, v.off, v.off + B + 1, B, frames, v.gx);
-  WL_CUDA(cudaEventRecord(v.ev[1], st));
-  if (frames > 0) vad_lstm(st, w, v.gx, v.off + B + 1, B, v.probs);
-  WL_CUDA(cudaEventRecord(v.ev[2], st));
-  if (frames > 0)
-    WL_CUDA(cudaMemcpyAsync(probs_out + prob_off[0], v.probs, frames * sizeof(float), cudaMemcpyDeviceToHost, st));
-  WL_CUDA(cudaStreamSynchronize(st));
-  WL_CUDA(cudaEventElapsedTime(&c->last_ms[6], v.ev[0], v.ev[1]));
-  WL_CUDA(cudaEventElapsedTime(&c->last_ms[7], v.ev[1], v.ev[2]));
-  API_END(c)
-}
-
-// ------------------------------------------------------------------------------------------ speaker embedding
-struct SpkTensor {
-  std::string name;
-  int co, ci, k;   // a conv weight [co][ci][k][k]; a bias has k = 0 (shape [co]); seg_1.weight has k = -1 ([co][ci])
-};
-constexpr int SPK_MEL_BINS = 80, SPK_EMB = 256, SPK_POOL = 2 * 256 * 10;
-constexpr long SPK_CHUNK_SAMPLES = 30 * 16000;   // the workspace's first size: max_streams segments of 30 s
-static const int SPK_STAGE_C[4] = {32, 64, 128, 256}, SPK_STAGE_N[4] = {3, 4, 6, 3};
-
-static const std::vector<SpkTensor>& spk_tensors() {
-  static const std::vector<SpkTensor> t = [] {
-    std::vector<SpkTensor> v;
-    auto conv = [&](const std::string& n, int co, int ci, int k) {
-      v.push_back({n + ".weight", co, ci, k});
-      v.push_back({n + ".bias", co, 0, 0});
-    };
-    conv("spk.conv1", 32, 1, 3);
-    int cin = 32;
-    for (int L = 0; L < 4; ++L)
-      for (int i = 0; i < SPK_STAGE_N[L]; ++i) {
-        const std::string b = "spk.layer" + std::to_string(L + 1) + "." + std::to_string(i);
-        const int c = SPK_STAGE_C[L];
-        conv(b + ".conv1", c, cin, 3);
-        conv(b + ".conv2", c, c, 3);
-        if (i == 0 && L > 0) conv(b + ".shortcut", c, cin, 1);
-        cin = c;
-      }
-    v.push_back({"spk.seg_1.weight", SPK_EMB, SPK_POOL, -1});
-    v.push_back({"spk.seg_1.bias", SPK_EMB, 0, 0});
-    return v;
-  }();
-  return t;
-}
-
-static int spk_index(const std::string& name) {
-  const auto& T = spk_tensors();
-  for (size_t i = 0; i < T.size(); ++i)
-    if (T[i].name == name) return (int)i;
-  return -1;
-}
-
-extern "C" int wl_spk_load_tensor(wl_ctx* c, const char* name, const float* data, const int64_t* shape, int32_t ndim) {
-  API_BEGIN(c)
-  WL_CHECK(name && data && shape && ndim >= 1, WL_ERR_ARG, "wl_spk_load_tensor: bad arguments");
-  const int i = spk_index(name);
-  WL_CHECK(i >= 0, WL_ERR_ARG, "wl_spk_load_tensor: unknown speaker-embedding tensor '%s'", name);
-  const SpkTensor& T = spk_tensors()[i];
-  std::vector<int64_t> want;
-  if (T.k > 0) want = {T.co, T.ci, T.k, T.k};
-  else if (T.k == 0) want = {T.co};
-  else want = {T.co, T.ci};
-  bool ok = ndim == (int)want.size();
-  for (int k = 0; ok && k < ndim; ++k) ok = shape[k] == want[k];
-  std::string ws;
-  for (size_t k = 0; k < want.size(); ++k) ws += (k ? ", " : "") + std::to_string(want[k]);
-  WL_CHECK(ok, WL_ERR_ARG, "wl_spk_load_tensor: '%s' must have shape [%s]", name, ws.c_str());
-  auto& s = c->spk;
-  if (s.t.empty()) s.t.assign(spk_tensors().size(), nullptr);
-  if (T.k > 0 && T.ci > 1) {   // tensor-core conv: fp16 [co][kh * k + kw][ci]
-    const int taps = T.k * T.k;
-    std::vector<__half> h((size_t)T.co * taps * T.ci);
-    for (int co = 0; co < T.co; ++co)
-      for (int ci = 0; ci < T.ci; ++ci)
-        for (int tap = 0; tap < taps; ++tap)
-          h[((size_t)co * taps + tap) * T.ci + ci] = __float2half_rn(data[((size_t)co * T.ci + ci) * taps + tap]);
-    if (!s.t[i]) s.t[i] = dalloc<__half>(c, h.size(), false);
-    WL_CUDA(cudaMemcpyAsync(s.t[i], h.data(), h.size() * sizeof(__half), cudaMemcpyHostToDevice, c->st));
-  } else {
-    size_t n = 1;
-    for (int k = 0; k < ndim; ++k) n *= (size_t)shape[k];
-    std::vector<float> h(data, data + n);
-    if (T.k < 0)   // seg_1: [256][5120] -> [5120][256]
-      for (int r = 0; r < T.co; ++r)
-        for (int k = 0; k < T.ci; ++k) h[(size_t)k * T.co + r] = data[(size_t)r * T.ci + k];
-    if (!s.t[i]) s.t[i] = dalloc<float>(c, n, false);
-    WL_CUDA(cudaMemcpyAsync(s.t[i], h.data(), n * sizeof(float), cudaMemcpyHostToDevice, c->st));
-  }
-  API_END(c)
-}
-
-// Kaldi mel banks [80][257] (20 Hz .. Nyquist, mel = 1127 ln(1 + f / 700)) and each bin's non-zero FFT-bin range
-static void spk_mel_tables(std::vector<float>& w, std::vector<int>& range) {
-  const int nb = SPK_MEL_BINS, half = 256;
-  auto mel = [](double f) { return 1127.0 * std::log(1.0 + f / 700.0); };
-  const double lo = mel(20.0), hi = mel(8000.0), delta = (hi - lo) / (nb + 1), width = 16000.0 / 512;
-  w.assign((size_t)nb * (half + 1), 0.f);
-  range.assign(2 * nb, 0);
-  for (int b = 0; b < nb; ++b) {
-    const double l = lo + b * delta, ce = lo + (b + 1) * delta, r = lo + (b + 2) * delta;
-    int k0 = half, k1 = 0;
-    for (int k = 0; k < half; ++k) {
-      const double m = mel(width * k);
-      const double v = std::max(0.0, std::min((m - l) / (ce - l), (r - m) / (r - ce)));
-      w[(size_t)b * (half + 1) + k] = (float)v;
-      if (v > 0) { k0 = std::min(k0, k); k1 = k + 1; }
-    }
-    range[2 * b] = k0 < k1 ? k0 : 0;
-    range[2 * b + 1] = k1;
-  }
-}
-
-// Position offsets of every stage, shared by wl_spk_embed and wl_test_spk_conv: a stream of T frames has H x T positions
-// at the stem (H = 80) and ceil-halved H and T after each stride-2 stage.
-static void spk_positions(const std::vector<long>& T, int H, std::vector<long>& off) {
-  off.assign(T.size() + 1, 0);
-  for (size_t b = 0; b < T.size(); ++b) off[b + 1] = off[b] + (long)H * T[b];
-}
-static std::vector<long> spk_halve(const std::vector<long>& T) {
-  std::vector<long> o(T.size());
-  for (size_t b = 0; b < T.size(); ++b) o[b] = (T[b] + 1) / 2;
-  return o;
-}
-
-static SpkConvParams spk_conv_params(const __half* x, const __half* w, const float* bias, const __half* res, __half* out,
-                                     const long* in_off, const long* out_off, long M, int B, int H_in, int C_in, int C_out,
-                                     int k, int stride, int relu) {
-  SpkConvParams p;
-  p.x = x; p.w = w; p.bias = bias; p.res = res; p.out = out; p.in_off = in_off; p.out_off = out_off; p.M = M; p.B = B;
-  p.H_in = H_in; p.H_out = stride == 2 ? (H_in + 1) / 2 : H_in; p.C_in = C_in; p.C_out = C_out; p.taps = k * k;
-  p.stride = stride; p.relu = relu;
-  return p;
-}
-
-static void spk_grow(wl_ctx* c, __half*& p, long& cap, long need, long first) {
-  if (need <= cap) return;
-  cap = std::max(need, first);
-  p = dalloc<__half>(c, cap, false);
-}
-
-extern "C" int wl_spk_embed(wl_ctx* c, const float* pcm, const int64_t* offsets, int32_t B, float* emb_out) {
-  API_BEGIN(c)
-  WL_CHECK(pcm && offsets && emb_out && B >= 1, WL_ERR_ARG, "wl_spk_embed: bad arguments (B=%d)", B);
-  auto& s = c->spk;
-  const auto& TT = spk_tensors();
-  for (size_t i = 0; i < TT.size(); ++i)
-    WL_CHECK(!s.t.empty() && s.t[i], WL_ERR_STATE, "wl_spk_embed: speaker weights not loaded: '%s' is missing (wl_spk_load_tensor)",
-             TT[i].name.c_str());
-  std::vector<long> T(B), poff(B + 1);
-  for (int b = 0; b <= B; ++b) poff[b] = offsets[b] - offsets[0];
-  for (int b = 0; b < B; ++b) {
-    const long n = poff[b + 1] - poff[b];
-    WL_CHECK(n >= 400, WL_ERR_ARG, "wl_spk_embed: stream %d has %ld samples; the fbank needs at least 400 (one 25 ms frame)", b, n);
-    T[b] = 1 + (n - 400) / 160;
-  }
-  // the tables: pcm offsets, frame offsets, the position offsets of the four stages
-  std::vector<long> tab(6 * (size_t)(B + 1)), st_off;
-  std::copy(poff.begin(), poff.end(), tab.begin());
-  spk_positions(T, 1, st_off);
-  std::copy(st_off.begin(), st_off.end(), tab.begin() + (B + 1));
-  std::vector<long> Ts = T;
-  long elems[4];
-  for (int L = 0; L < 4; ++L) {
-    if (L > 0) Ts = spk_halve(Ts);
-    spk_positions(Ts, SPK_MEL_BINS >> L, st_off);
-    std::copy(st_off.begin(), st_off.end(), tab.begin() + (2 + L) * (B + 1));
-    elems[L] = st_off[B] * SPK_STAGE_C[L];
-  }
-  // first size: max_streams segments of 30 s
-  long first[4], first_frames = (SPK_CHUNK_SAMPLES - 400) / 160 + 1;
-  {
-    long t = first_frames;
-    for (int L = 0; L < 4; ++L) {
-      if (L > 0) t = (t + 1) / 2;
-      first[L] = (long)c->Bm * (SPK_MEL_BINS >> L) * t * SPK_STAGE_C[L];
-    }
-  }
-  const long total = poff[B], frames = tab[(B + 1) + B];
-  if (total > s.pcm_cap) {
-    s.pcm_cap = std::max(total, (long)c->Bm * SPK_CHUNK_SAMPLES);
-    s.pcm = dalloc<float>(c, s.pcm_cap, false);
-  }
-  if (frames > s.frame_cap) {
-    s.frame_cap = std::max(frames, (long)c->Bm * first_frames);
-    s.feat = dalloc<float>(c, (size_t)s.frame_cap * SPK_MEL_BINS, false);
-  }
-  if (B > s.stream_cap) {
-    s.stream_cap = std::max(B, c->Bm);
-    s.mean = dalloc<float>(c, (size_t)s.stream_cap * SPK_MEL_BINS, false);
-    s.pooled = dalloc<float>(c, (size_t)s.stream_cap * SPK_POOL, false);
-    s.emb = dalloc<float>(c, (size_t)s.stream_cap * SPK_EMB, false);
-    s.off = dalloc<long>(c, 6 * (size_t)(s.stream_cap + 1), false);
-  }
-  // act[0]: stage input / output of stages 1 and 3; act[1]: each block's first conv; act[2]: stages 2 and 4
-  spk_grow(c, s.act[0], s.act_cap[0], std::max(elems[0], elems[2]), std::max(first[0], first[2]));
-  spk_grow(c, s.act[1], s.act_cap[1], std::max(std::max(elems[0], elems[1]), std::max(elems[2], elems[3])),
-           std::max(std::max(first[0], first[1]), std::max(first[2], first[3])));
-  spk_grow(c, s.act[2], s.act_cap[2], std::max(elems[1], elems[3]), std::max(first[1], first[3]));
-  if (!s.melw) {
-    std::vector<float> w;
-    std::vector<int> r;
-    spk_mel_tables(w, r);
-    s.melw = dalloc<float>(c, w.size(), false);
-    s.mel_range = dalloc<int>(c, r.size(), false);
-    WL_CUDA(cudaMemcpyAsync(s.melw, w.data(), w.size() * sizeof(float), cudaMemcpyHostToDevice, c->st));
-    WL_CUDA(cudaMemcpyAsync(s.mel_range, r.data(), r.size() * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  }
-  if (!s.ev[0])
-    for (auto& e : s.ev) WL_CUDA(cudaEventCreate(&e));
-  cudaStream_t st = c->st;
-  const long* d_pcm_off = s.off;
-  const long* d_frame_off = s.off + (B + 1);
-  auto d_pos = [&](int L) { return s.off + (2 + L) * (B + 1); };
-  WL_CUDA(cudaMemcpyAsync(s.pcm, pcm + offsets[0], total * sizeof(float), cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaMemcpyAsync(s.off, tab.data(), tab.size() * sizeof(long), cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaEventRecord(s.ev[0], st));
-  spk_fbank(st, s.pcm, d_pcm_off, d_frame_off, B, frames, s.melw, s.mel_range, s.feat, s.mean);
-  WL_CUDA(cudaEventRecord(s.ev[1], st));
-  size_t ti = 0;
-  auto wgt = [&]() { return s.t[ti++]; };
-  {
-    const float* w = (const float*)wgt();
-    const float* b = (const float*)wgt();
-    spk_stem(st, s.feat, s.mean, d_frame_off, B, frames, w, b, s.act[0]);
-  }
-  __half* cur = s.act[0];
-  int cin = 32;
-  for (int L = 0; L < 4; ++L) {
-    const int C = SPK_STAGE_C[L], H_in = L == 0 ? SPK_MEL_BINS : (SPK_MEL_BINS >> (L - 1)), H = SPK_MEL_BINS >> L;
-    const long M = elems[L] / C;
-    __half* y = s.act[1];
-    for (int i = 0; i < SPK_STAGE_N[L]; ++i) {
-      const bool down = i == 0 && L > 0;
-      const long* in_off = down ? d_pos(L - 1) : d_pos(L);
-      const int hin = down ? H_in : H, stride = down ? 2 : 1;
-      const __half* w1 = (const __half*)wgt(); const float* b1 = (const float*)wgt();
-      const __half* w2 = (const __half*)wgt(); const float* b2 = (const float*)wgt();
-      __half* out = cur;
-      if (down) {   // the shortcut goes to the buffer the block's output then replaces in place
-        const __half* ws = (const __half*)wgt(); const float* bs = (const float*)wgt();
-        out = cur == s.act[0] ? s.act[2] : s.act[0];
-        spk_conv(st, spk_conv_params(cur, ws, bs, nullptr, out, in_off, d_pos(L), M, B, hin, cin, C, 1, 2, 0));
-      }
-      spk_conv(st, spk_conv_params(cur, w1, b1, nullptr, y, in_off, d_pos(L), M, B, hin, cin, C, 3, stride, 1));
-      spk_conv(st, spk_conv_params(y, w2, b2, out, out, d_pos(L), d_pos(L), M, B, H, C, C, 3, 1, 1));
-      cur = out;
-      cin = C;
-    }
-  }
-  {
-    const float* w = (const float*)wgt();
-    const float* b = (const float*)wgt();
-    spk_pool_embed(st, cur, d_pos(3), B, SPK_MEL_BINS >> 3, w, b, s.pooled, s.emb);
-  }
-  WL_CUDA(cudaEventRecord(s.ev[2], st));
-  WL_CUDA(cudaMemcpyAsync(emb_out, s.emb, (size_t)B * SPK_EMB * sizeof(float), cudaMemcpyDeviceToHost, st));
-  WL_CUDA(cudaStreamSynchronize(st));
-  WL_CUDA(cudaEventElapsedTime(&c->last_ms[8], s.ev[0], s.ev[1]));
-  WL_CUDA(cudaEventElapsedTime(&c->last_ms[9], s.ev[1], s.ev[2]));
-  API_END(c)
-}
-
-extern "C" int wl_test_spk_fbank(wl_ctx* c, const float* pcm, const int64_t* offsets, int32_t B, float* feat_out) {
-  API_BEGIN(c)
-  WL_CHECK(pcm && offsets && feat_out && B >= 1, WL_ERR_ARG, "wl_test_spk_fbank: bad arguments");
-  std::vector<long> tab(2 * (size_t)(B + 1), 0);
-  for (int b = 0; b <= B; ++b) tab[b] = offsets[b] - offsets[0];
-  for (int b = 0; b < B; ++b) {
-    const long n = tab[b + 1] - tab[b];
-    WL_CHECK(n >= 400, WL_ERR_ARG, "wl_test_spk_fbank: stream %d has %ld samples (< 400)", b, n);
-    tab[B + 2 + b] = tab[B + 1 + b] + 1 + (n - 400) / 160;
-  }
-  const long total = tab[B], frames = tab[2 * B + 1];
-  std::vector<float> w;
-  std::vector<int> r;
-  spk_mel_tables(w, r);
-  float *dp = nullptr, *dw = nullptr, *df = nullptr, *dm = nullptr;
-  int* dr = nullptr;
-  long* doff = nullptr;
-  WL_CUDA(cudaMalloc(&dp, total * 4));
-  WL_CUDA(cudaMalloc(&dw, w.size() * 4));
-  WL_CUDA(cudaMalloc(&dr, r.size() * 4));
-  WL_CUDA(cudaMalloc(&df, frames * SPK_MEL_BINS * 4));
-  WL_CUDA(cudaMalloc(&dm, (size_t)B * SPK_MEL_BINS * 4));
-  WL_CUDA(cudaMalloc(&doff, tab.size() * sizeof(long)));
-  WL_CUDA(cudaMemcpyAsync(dp, pcm + offsets[0], total * 4, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(dw, w.data(), w.size() * 4, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(dr, r.data(), r.size() * 4, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(doff, tab.data(), tab.size() * sizeof(long), cudaMemcpyHostToDevice, c->st));
-  spk_fbank(c->st, dp, doff, doff + B + 1, B, frames, dw, dr, df, dm);
-  WL_CUDA(cudaMemcpyAsync(feat_out, df, frames * SPK_MEL_BINS * 4, cudaMemcpyDeviceToHost, c->st));
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  for (void* p : {(void*)dp, (void*)dw, (void*)dr, (void*)df, (void*)dm, (void*)doff}) cudaFree(p);
-  API_END(c)
-}
-
-extern "C" int wl_test_spk_conv(wl_ctx* c, const uint16_t* x_f16, const int64_t* frames, int32_t B, int32_t H_in, int32_t C_in,
-                                int32_t C_out, int32_t ksize, int32_t stride, const uint16_t* w_f16, const float* bias,
-                                const uint16_t* res_f16, int32_t relu, uint16_t* out_f16) {
-  API_BEGIN(c)
-  WL_CHECK(x_f16 && frames && B >= 1 && w_f16 && bias && out_f16 && (ksize == 1 || ksize == 3), WL_ERR_ARG,
-           "wl_test_spk_conv: bad arguments");
-  WL_CHECK(spk_conv_supported(C_in, C_out, ksize * ksize, stride), WL_ERR_ARG, "wl_test_spk_conv: unsupported shape");
-  std::vector<long> T(frames, frames + B), in_off, out_off;
-  for (long t : T) WL_CHECK(t >= 1, WL_ERR_ARG, "wl_test_spk_conv: every stream needs a frame");
-  spk_positions(T, H_in, in_off);
-  const int H_out = stride == 2 ? (H_in + 1) / 2 : H_in;
-  spk_positions(stride == 2 ? spk_halve(T) : T, H_out, out_off);
-  const long Min = in_off[B], M = out_off[B];
-  const size_t nw = (size_t)C_out * ksize * ksize * C_in;
-  std::vector<long> tab(in_off);
-  tab.insert(tab.end(), out_off.begin(), out_off.end());
-  __half *dx = nullptr, *dw = nullptr, *dr = nullptr, *dout = nullptr;
-  float* db = nullptr;
-  long* doff = nullptr;
-  WL_CUDA(cudaMalloc(&dx, Min * C_in * 2));
-  WL_CUDA(cudaMalloc(&dw, nw * 2));
-  WL_CUDA(cudaMalloc(&db, C_out * 4));
-  WL_CUDA(cudaMalloc(&dout, M * C_out * 2));
-  WL_CUDA(cudaMalloc(&doff, tab.size() * sizeof(long)));
-  WL_CUDA(cudaMemcpyAsync(dx, x_f16, Min * C_in * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(dw, w_f16, nw * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(db, bias, C_out * 4, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(dout, out_f16, M * C_out * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(doff, tab.data(), tab.size() * sizeof(long), cudaMemcpyHostToDevice, c->st));
-  if (res_f16) {
-    WL_CUDA(cudaMalloc(&dr, M * C_out * 2));
-    WL_CUDA(cudaMemcpyAsync(dr, res_f16, M * C_out * 2, cudaMemcpyHostToDevice, c->st));
-  }
-  spk_conv(c->st, spk_conv_params(dx, dw, db, dr, dout, doff, doff + B + 1, M, B, H_in, C_in, C_out, ksize, stride, relu));
-  WL_CUDA(cudaMemcpyAsync(out_f16, dout, M * C_out * 2, cudaMemcpyDeviceToHost, c->st));
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  for (void* p : {(void*)dx, (void*)dw, (void*)db, (void*)dout, (void*)doff, (void*)dr})
-    if (p) cudaFree(p);
-  API_END(c)
-}
-
 // ------------------------------------------------------------------------------------------ K2-K7 encoder
-static GemmOperand opnd(const __half* p, long rows, long k, long ld, int n1 = 1, long s1 = 0, int n2 = 1, long s2 = 0) {
+GemmOperand opnd(const __half* p, long rows, long k, long ld, int n1, long s1, int n2, long s2) {
   GemmOperand o;
   o.ptr = p; o.rows = rows; o.k = k; o.ld = ld; o.n1 = n1; o.s1 = s1; o.n2 = n2; o.s2 = s2;
   return o;
@@ -1221,7 +555,7 @@ static GemmOperand opnd(const __half* p, long rows, long k, long ld, int n1 = 1,
 // The conv stem: features [nb][n_mels][3000] f32 -> x [nb][1500][d] f32 (conv1 + GELU, conv2 (stride 2) + GELU + the
 // positional table).  feat16 [nb][3002][n_mels] and conv1o [nb][3002][d] are workspaces whose rows 0 and 3001 of every
 // stream must be zero (the conv padding): nothing here writes them.
-static void encoder_stem(wl_ctx* c, cudaStream_t st, int nb, const float* feat_dev, __half* feat16, __half* conv1o, float* x) {
+void encoder_stem(wl_ctx* c, cudaStream_t st, int nb, const float* feat_dev, __half* feat16, __half* conv1o, float* x) {
   const int d = c->d, nm = c->n_mels;
   prep_features(st, feat_dev, feat16, nb, nm);
   {  // conv1 + GELU -> conv1o rows 1..3000 (rows 0 / 3001 stay zero)
@@ -1240,8 +574,8 @@ static void encoder_stem(wl_ctx* c, cudaStream_t st, int nb, const float* feat_d
 // Encoder self-attention without the fused kernel (WLB200_FUSED_ATTN=0), AB streams at a time: the scores GEMM into
 // scores [AB][H][1500][S_PAD] f32, softmax_rows into probs16 (same shape, fp16, the pad columns written as 0), the P V
 // GEMM into attn.  qk [nb][1500][2d], vt [nb][d][S_PAD], attn [nb * 1500][d].
-static void encoder_attention_unfused(cudaStream_t st, const __half* qk, const __half* vt, __half* attn, float* scores,
-                                      __half* probs16, int nb, int H, int AB) {
+void encoder_attention_unfused(cudaStream_t st, const __half* qk, const __half* vt, __half* attn, float* scores,
+                               __half* probs16, int nb, int H, int AB) {
   const int d = H * 64;
   for (int b0 = 0; b0 < nb; b0 += AB) {
     const int ab = std::min(AB, nb - b0);
@@ -1494,14 +828,15 @@ static void prefill_reserve(wl_ctx* c, long rows) {
   if (rows <= f.cap_rows) return;
   const long cap = (rows + 1023) / 1024 * 1024;
   const int d = c->d, ff = 4 * c->d;
-  // (earlier, smaller buffers stay in c->allocs until wl_destroy: growth happens a handful of times per process)
-  f.tok = dalloc<int>(c, cap); f.pos = dalloc<int>(c, cap); f.active = dalloc<int>(c, cap); f.wrow = dalloc<int>(c, cap);
-  f.vslot = dalloc<int>(c, cap / 8 + PF_VCHUNK); f.vdone = dalloc<int>(c, cap / 8 + PF_VCHUNK);
-  if (!f.sel) f.sel = dalloc<int>(c, 3 * (size_t)c->Rm + 16);
-  f.src = dalloc<short>(c, cap * T_MAX, false);
-  f.x = dalloc<float>(c, cap * d, false); f.qkv = dalloc<float>(c, cap * 3 * d, false); f.qc = dalloc<float>(c, cap * d, false);
-  f.xn = dalloc<__half>(c, cap * d, false); f.att = dalloc<__half>(c, cap * d, false); f.h = dalloc<__half>(c, cap * ff, false);
-  if (!f.xpart) f.xpart = dalloc<float>(c, (size_t)PF_VCHUNK * c->H * 12 * MAX_ROWS_PER_STREAM * 66, false);
+  DeviceMem& m = c->mem;
+  f.cap_rows = 0;   // until every buffer of the set has its new size
+  m.replace(f.tok, cap, true); m.replace(f.pos, cap, true); m.replace(f.active, cap, true); m.replace(f.wrow, cap, true);
+  m.replace(f.vslot, cap / 8 + PF_VCHUNK, true); m.replace(f.vdone, cap / 8 + PF_VCHUNK, true);
+  if (!f.sel) f.sel = m.alloc<int>(3 * (size_t)c->Rm + 16);
+  m.replace(f.src, cap * T_MAX);
+  m.replace(f.x, cap * d); m.replace(f.qkv, cap * 3 * d); m.replace(f.qc, cap * d);
+  m.replace(f.xn, cap * d); m.replace(f.att, cap * d); m.replace(f.h, cap * ff);
+  if (!f.xpart) f.xpart = m.alloc<float>((size_t)PF_VCHUNK * c->H * 12 * MAX_ROWS_PER_STREAM * 66, false);
   f.cap_rows = cap;
 }
 
@@ -1562,9 +897,9 @@ static void pf_stack(wl_ctx* c, const PfRows& r, bool align) {
   WL_CUDA(cudaMemsetAsync(f.vdone, 0, NV * 4, st));
   const int nh = (int)c->align_heads.size() / 2;
   if (align) {
-    if (!f.row_b_cap || f.row_b_cap < f.cap_rows) { f.row_b = dalloc<int>(c, f.cap_rows); f.row_b_cap = f.cap_rows; }
+    c->mem.grow(f.row_b, f.row_b_cap, f.cap_rows, 0, true);
     WL_CUDA(cudaMemcpyAsync(f.row_b, r.row_b.data(), M * 4, cudaMemcpyHostToDevice, st));
-    if (!f.aprobs) f.aprobs = dalloc<float>(c, (size_t)PF_VCHUNK * 8 * H * S_ENC, false);
+    if (!f.aprobs) f.aprobs = c->mem.alloc<float>((size_t)PF_VCHUNK * 8 * H * S_ENC, false);
   }
   prefill_embed(st, f.tok, f.pos, f.active, f.wrow, c->emb, c->pos_dec, f.x, f.src, (int)M, d);
   DecodeState sv = c->ds;
@@ -2046,11 +1381,11 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
            "wl_session_open: sampling is chosen per stream at admission (wl_session_admit_ex), not for the session");
   if (!ss.allocated) {
     alloc_decode_state(c, ss.ds);
-    ss.kcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
-    ss.vcache = dalloc<__half>(c, (size_t)c->Ld * c->cache_layer_stride, false);
-    ss.mask = dalloc<unsigned>(c, (c->V + 31) / 32 + 1);
-    ss.idx_dev = dalloc<int>(c, c->Bm);
-    ss.peek_dev = dalloc<int>(c, (size_t)c->Bm * PEEK_STRIDE);
+    ss.kcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
+    ss.vcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
+    ss.mask = c->mem.alloc<unsigned>((c->V + 31) / 32 + 1);
+    ss.idx_dev = c->mem.alloc<int>(c->Bm);
+    ss.peek_dev = c->mem.alloc<int>((size_t)c->Bm * PEEK_STRIDE);
     ss.allocated = true;
   }
   ss.cap = capacity; ss.K = K; ss.Kr = Kr; ss.NH = o->num_hypotheses; ss.length_penalty = o->length_penalty;
@@ -2365,16 +1700,10 @@ extern "C" int wl_decode_logits(wl_ctx* c, const int32_t* slots, int32_t B, cons
   std::vector<long> base(B);
   long tot = 0;
   for (int b = 0; b < B; ++b) { base[b] = tot; tot += tok_off[b + 1] - tok_off[b]; }
-  float* dev = nullptr;
-  WL_CUDA(cudaMalloc((void**)&dev, (size_t)tot * c->V * 4));
-  try {
-    forced_run(c, slots, B, tokens, tok_off, false, dev, base);
-    WL_CUDA(cudaMemcpy(logits_out, dev, (size_t)tot * c->V * 4, cudaMemcpyDeviceToHost));
-  } catch (...) {
-    cudaFree(dev);
-    throw;
-  }
-  cudaFree(dev);
+  Scratch sc(c->st);
+  float* dev = sc.alloc<float>((size_t)tot * c->V);
+  forced_run(c, slots, B, tokens, tok_off, false, dev, base);
+  sc.download(logits_out, dev, (size_t)tot * c->V);
   API_END(c)
 }
 
@@ -2424,10 +1753,7 @@ extern "C" int wl_align(wl_ctx* c, const int32_t* slots, int32_t B, const int32_
   }
   WL_CHECK(maxT <= T_MAX, WL_ERR_ARG, "wl_align: sequence of %d tokens exceeds %d", maxT, T_MAX);
   const long need_buf = (long)B * nh * T_MAX * S_ENC;
-  if (need_buf > c->align_buf_cap) {
-    c->align_buf = dalloc<float>(c, need_buf, false);
-    c->align_buf_cap = need_buf;
-  }
+  c->mem.grow(c->align_buf, c->align_buf_cap, need_buf);
   for (int b = 0; b < B; ++b)
     WL_CHECK(slots[b] >= 0 && slots[b] < c->NS && c->slot_used[slots[b]], WL_ERR_ARG, "wl_align: stream %d: bad encoder slot %d", b, slots[b]);
   // ---- teacher-forced pass: every position of every stream at once (the K8 machinery), attention probabilities of
@@ -2441,7 +1767,7 @@ extern "C" int wl_align(wl_ctx* c, const int32_t* slots, int32_t B, const int32_
   // ---- P(text token | prefix): the logits row that predicts it
   const int n_text = text_off[B] - text_off[0];
   if (n_text > 0) {
-    if (n_text > f.tokp_cap) { f.tokp = dalloc<float>(c, (size_t)n_text + 256); f.tokp_cap = n_text + 256; }
+    c->mem.grow(f.tokp, f.tokp_cap, n_text, n_text + 256, true);
     std::vector<int> sel, tgt, oidx;
     for (int b = 0; b < B; ++b)
       for (int i = 0; i < text_off[b + 1] - text_off[b]; ++i) {
@@ -2454,10 +1780,10 @@ extern "C" int wl_align(wl_ctx* c, const int32_t* slots, int32_t B, const int32_
   }
   // ---- standardise / median filter / mean over heads / DTW on the device
   if (!f.mat) {
-    f.mat = dalloc<float>(c, (size_t)c->Bm * T_MAX * S_ENC, false);
-    f.aT = dalloc<int>(c, c->Bm); f.anf = dalloc<int>(c, c->Bm);
-    f.path = dalloc<int>(c, (size_t)c->Bm * (T_MAX + S_ENC + 2) * 2, false);
-    f.path_len = dalloc<int>(c, c->Bm);
+    f.mat = c->mem.alloc<float>((size_t)c->Bm * T_MAX * S_ENC, false);
+    f.aT = c->mem.alloc<int>(c->Bm); f.anf = c->mem.alloc<int>(c->Bm);
+    f.path = c->mem.alloc<int>((size_t)c->Bm * (T_MAX + S_ENC + 2) * 2, false);
+    f.path_len = c->mem.alloc<int>(c->Bm);
   }
   const int path_cap = T_MAX + S_ENC + 2;
   std::vector<int> hT(B), hnf(B);
@@ -2485,419 +1811,5 @@ extern "C" int wl_align(wl_ctx* c, const int32_t* slots, int32_t B, const int32_
     }
     pair_off[b + 1] = np_total;
   }
-  API_END(c)
-}
-
-// ------------------------------------------------------------------------------------------ test hook
-extern "C" int wl_test_gemm(wl_ctx* c, const uint16_t* a_f16, const uint16_t* b_f16, const float* bias, float* cc, int32_t M,
-                            int32_t N, int32_t K, int32_t batch, int32_t transposed_store, int32_t gelu, int32_t use_simt,
-                            int32_t opts) {
-  API_BEGIN(c)
-  const int out_kind = opts & 3, variant = (opts >> 4) & 3, hs_S = opts >> 8;
-  const bool a_shared = opts & 4, b_shared = opts & 8, bias_on_m = transposed_store || (opts & 64);
-  const bool f16_out = out_kind == 2 || out_kind == 3;
-  WL_CHECK(variant <= GEMM_PINGPONG && (out_kind != 3 || (hs_S > 0 && M % hs_S == 0 && N % 64 == 0 && batch == 1)), WL_ERR_ARG,
-           "wl_test_gemm: bad opts %d", opts);
-  __half *da = nullptr, *db = nullptr, *dh = nullptr;
-  float *dbias = nullptr, *dc = nullptr;
-  int* dslots = nullptr;
-  const size_t na = (size_t)(a_shared ? 1 : batch) * M * K, nb = (size_t)(b_shared ? 1 : batch) * N * K, nc = (size_t)batch * M * N;
-  WL_CUDA(cudaMalloc((void**)&da, na * 2));
-  WL_CUDA(cudaMalloc((void**)&db, nb * 2));
-  WL_CUDA(cudaMalloc((void**)&dc, nc * 4));
-  WL_CUDA(cudaMalloc((void**)&dh, nc * 2));
-  WL_CUDA(cudaMemcpy(da, a_f16, na * 2, cudaMemcpyHostToDevice));
-  WL_CUDA(cudaMemcpy(db, b_f16, nb * 2, cudaMemcpyHostToDevice));
-  if (out_kind == 1) WL_CUDA(cudaMemcpy(dc, cc, nc * 4, cudaMemcpyHostToDevice));   // the residual, updated in place
-  else WL_CUDA(cudaMemset(dc, 0, nc * 4));
-  WL_CUDA(cudaMemset(dh, 0, nc * 2));
-  if (bias) {
-    WL_CUDA(cudaMalloc((void**)&dbias, (size_t)std::max(M, N) * 4));
-    WL_CUDA(cudaMemcpy(dbias, bias, (size_t)(bias_on_m ? M : N) * 4, cudaMemcpyHostToDevice));
-  }
-  if (out_kind == 3) {   // head-split into slots in reverse stream order: out[slot][h][s][64], s-swizzled 16-byte pieces
-    const int ns = M / hs_S;
-    std::vector<int> slots(ns);
-    for (int b = 0; b < ns; ++b) slots[b] = ns - 1 - b;
-    WL_CUDA(cudaMalloc((void**)&dslots, ns * sizeof(int)));
-    WL_CUDA(cudaMemcpy(dslots, slots.data(), ns * sizeof(int), cudaMemcpyHostToDevice));
-  }
-  // the copies / memset above ran on the legacy default stream, the GEMM runs on the library's non-blocking stream:
-  // without this the kernel may overtake the memset of its own output buffer
-  WL_CUDA(cudaDeviceSynchronize());
-  GemmEpilogue e;
-  e.out = f16_out ? (void*)dh : (void*)dc; e.out_f32 = f16_out ? 0 : 1; e.gelu = gelu; e.bias = dbias;
-  if (transposed_store) { e.ldm = 1; e.ldn = M; }   // C^T stored: [N][M]
-  else { e.ldm = N; e.ldn = 1; }
-  e.bias_on_m = bias_on_m;
-  e.ob1 = (long)M * N;
-  if (out_kind == 1) { e.resid = dc; e.rldm = e.ldm; e.rldn = e.ldn; e.rb1 = e.ob1; }
-  if (out_kind == 3) {
-    e.mode = GEMM_HEADSPLIT; e.hs_S = hs_S; e.hs_H = N / 64; e.hs_slot_stride = (long)hs_S * N; e.hs_slots = dslots;
-  }
-  try {
-    GemmOperand A = opnd(da, M, K, K, batch, a_shared ? 0 : (long)M * K), Bo = opnd(db, N, K, K, batch, b_shared ? 0 : (long)N * K);
-    if (a_shared) A.n1 = 1;
-    if (b_shared) Bo.n1 = 1;
-    if (use_simt) gemm_tn_simt(c->st, A, Bo, M, N, K, e);
-    else gemm_tn(c->st, A, Bo, M, N, K, e, (GemmVariant)variant);
-    WL_CUDA(cudaStreamSynchronize(c->st));
-    if (f16_out) {
-      std::vector<__half> h(nc);
-      WL_CUDA(cudaMemcpy(h.data(), dh, nc * 2, cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < nc; ++i) cc[i] = __half2float(h[i]);
-    } else {
-      WL_CUDA(cudaMemcpy(cc, dc, nc * 4, cudaMemcpyDeviceToHost));
-    }
-  } catch (...) {
-    cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dh); if (dbias) cudaFree(dbias); if (dslots) cudaFree(dslots);
-    throw;
-  }
-  cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dh); if (dbias) cudaFree(dbias); if (dslots) cudaFree(dslots);
-  API_END(c)
-}
-
-extern "C" int wl_gemm_variant(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t* variant_out) {
-  API_BEGIN(c)
-  WL_CHECK(variant_out && M > 0 && N > 0 && K > 0 && batch > 0, WL_ERR_ARG, "wl_gemm_variant: bad arguments");
-  *variant_out = (int32_t)gemm_tn_variant(M, N, K, batch);
-  API_END(c)
-}
-
-// mode 0/1/2/3 of wgemm (see gemm.cuh); out holds [R][n_out] floats (mode 1: the residual on input, the sum on output;
-// mode 2: gelu as fp32; mode 3: the K ranges summed on the host side of this hook)
-extern "C" int wl_test_wgemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x_f16, const float* bias, float* out, int32_t R,
-                             int32_t n_out, int32_t K, int32_t mode) {
-  API_BEGIN(c)
-  WL_CHECK(w_f16 && x_f16 && out && mode >= 0 && mode <= 3, WL_ERR_ARG, "wl_test_wgemm: bad arguments");
-  WL_CHECK(wgemm_supported(R, K), WL_ERR_ARG, "wl_test_wgemm: unsupported shape R=%d K=%d", R, K);
-  __half *dw = nullptr, *dx = nullptr, *dh = nullptr;
-  float *db = nullptr, *dout = nullptr;
-  const size_t nw = (size_t)n_out * K, nx = (size_t)R * K, no = (size_t)R * n_out;
-  const int ks = wgemm_ksplit(K);
-  WL_CUDA(cudaMalloc((void**)&dw, nw * 2));
-  WL_CUDA(cudaMalloc((void**)&dx, nx * 2));
-  WL_CUDA(cudaMalloc((void**)&dh, no * 2));
-  WL_CUDA(cudaMalloc((void**)&dout, no * 4 * (size_t)std::max(1, ks)));
-  WL_CUDA(cudaMalloc((void**)&db, (size_t)n_out * 4));
-  try {
-    WL_CUDA(cudaMemcpy(dw, w_f16, nw * 2, cudaMemcpyHostToDevice));
-    WL_CUDA(cudaMemcpy(dx, x_f16, nx * 2, cudaMemcpyHostToDevice));
-    WL_CUDA(cudaMemset(dout, 0, no * 4 * (size_t)std::max(1, ks)));
-    if (mode == 1) WL_CUDA(cudaMemcpy(dout, out, no * 4, cudaMemcpyHostToDevice));
-    if (bias) WL_CUDA(cudaMemcpy(db, bias, (size_t)n_out * 4, cudaMemcpyHostToDevice));
-    WL_CUDA(cudaDeviceSynchronize());
-    wgemm(c->st, dw, n_out, K, dx, R, bias ? db : nullptr, mode, dout, dh, (long)no);
-    WL_CUDA(cudaStreamSynchronize(c->st));
-    if (mode == 2) {
-      std::vector<__half> h(no);
-      WL_CUDA(cudaMemcpy(h.data(), dh, no * 2, cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < no; ++i) out[i] = __half2float(h[i]);
-    } else if (mode == 3) {
-      std::vector<float> h(no * ks);
-      WL_CUDA(cudaMemcpy(h.data(), dout, h.size() * 4, cudaMemcpyDeviceToHost));
-      for (size_t i = 0; i < no; ++i) { float a = 0.f; for (int q = 0; q < ks; ++q) a += h[(size_t)q * no + i]; out[i] = a; }
-    } else {
-      WL_CUDA(cudaMemcpy(out, dout, no * 4, cudaMemcpyDeviceToHost));
-    }
-  } catch (...) {
-    cudaFree(dw); cudaFree(dx); cudaFree(dh); cudaFree(dout); cudaFree(db);
-    throw;
-  }
-  cudaFree(dw); cudaFree(dx); cudaFree(dh); cudaFree(dout); cudaFree(db);
-  API_END(c)
-}
-
-// Device buffers of one decode-kernel test hook: freed when the hook returns, whether it returns normally or through an
-// exception (a failed check or launch).
-struct HookBufs {
-  std::vector<void*> p;
-  template <class T>
-  T* alloc(size_t n) {
-    void* q = nullptr;
-    WL_CUDA(cudaMalloc(&q, std::max<size_t>(n, 1) * sizeof(T)));
-    p.push_back(q);
-    return (T*)q;
-  }
-  template <class T>
-  T* upload(const T* h, size_t n) {
-    T* d = alloc<T>(n);
-    WL_CUDA(cudaMemcpy(d, h, n * sizeof(T), cudaMemcpyHostToDevice));
-    return d;
-  }
-  ~HookBufs() {
-    for (void* q : p) cudaFree(q);
-  }
-};
-
-static void fill_f16(__half* d, size_t n, float v) {
-  std::vector<__half> h(n, __float2half_rn(v));
-  WL_CUDA(cudaMemcpy(d, h.data(), n * 2, cudaMemcpyHostToDevice));
-}
-static void download_f16(const __half* d, float* out, size_t n) {
-  std::vector<__half> h(n);
-  WL_CUDA(cudaMemcpy(h.data(), d, n * 2, cudaMemcpyDeviceToHost));
-  for (size_t i = 0; i < n; ++i) out[i] = __half2float(h[i]);
-}
-
-extern "C" int wl_test_dec_gemm(wl_ctx* c, const uint16_t* w_f16, const uint16_t* x_f16, float* out, int32_t R, int32_t n_out,
-                                int32_t K, int32_t nsplit, int32_t* nsplit_out) {
-  API_BEGIN(c)
-  PdlScope pdl(false);
-  WL_CHECK(w_f16 && x_f16 && nsplit_out && R > 0 && n_out > 0 && K > 0 && K % 8 == 0 && nsplit >= 0, WL_ERR_ARG,
-           "wl_test_dec_gemm: bad arguments");
-  const int ns = nsplit == 0 ? dec_gemm_split_plan(n_out, R, K, 8) : nsplit;
-  const int kb = cdiv(K, 64);
-  WL_CHECK(cdiv(kb, cdiv(kb, ns)) == ns, WL_ERR_ARG, "wl_test_dec_gemm: %d K ranges cannot be formed from %d k-blocks", ns, kb);
-  *nsplit_out = ns;
-  if (!out) return WL_OK;   // split query only
-  HookBufs hb;
-  const long part = (long)R * n_out;
-  const __half* dw = hb.upload(reinterpret_cast<const __half*>(w_f16), (size_t)n_out * K);
-  const __half* dx = hb.upload(reinterpret_cast<const __half*>(x_f16), (size_t)R * K);
-  float* dout = hb.alloc<float>((size_t)ns * part);
-  WL_CUDA(cudaMemset(dout, 0xff, (size_t)ns * part * 4));   // NaN: an element no K range wrote cannot pass as a value
-  WL_CUDA(cudaDeviceSynchronize());
-  dec_gemm(c->st, dw, n_out, K, dx, R, dout, n_out, part, ns);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  WL_CUDA(cudaMemcpy(out, dout, (size_t)ns * part * 4, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_test_cross_attn(wl_ctx* c, const float* q_part, const float* q_bias, int32_t q_nsplit, const uint16_t* k_pool,
-                                  const uint16_t* v_pool, int32_t n_slots, const int32_t* slot, const int32_t* done, int32_t B,
-                                  int32_t rows_per_stream, int32_t H, int32_t nsplit, int32_t* nsplit_out, float sentinel,
-                                  float* out, float* probs) {
-  API_BEGIN(c)
-  PdlScope pdl(false);
-  WL_CHECK(q_part && k_pool && v_pool && slot && done && out && nsplit_out && B > 0 && H > 0 && n_slots > 0 && nsplit >= 0 &&
-               rows_per_stream >= 1 && rows_per_stream <= MAX_ROWS_PER_STREAM,
-           WL_ERR_ARG, "wl_test_cross_attn: bad arguments");
-  for (int b = 0; b < B; ++b) WL_CHECK(slot[b] >= 0 && slot[b] < n_slots, WL_ERR_ARG, "wl_test_cross_attn: slot %d out of range", slot[b]);
-  const int nchunk = cdiv(S_ENC, 128);
-  const int ns = nsplit == 0 ? cross_attn_pick_nsplit(B, H, c->num_sms, rows_per_stream) : nsplit;
-  WL_CHECK(ns >= 1 && ns <= nchunk && cdiv(nchunk, cdiv(nchunk, ns)) == ns, WL_ERR_ARG,
-           "wl_test_cross_attn: %d key ranges cannot be formed from %d chunks", ns, nchunk);
-  WL_CHECK(!probs || ns == 1, WL_ERR_ARG, "wl_test_cross_attn: the probabilities need the whole key range (nsplit 1)");
-  *nsplit_out = ns;
-  const int d = H * 64, R = B * rows_per_stream;
-  const long slot_sz = (long)S_ENC * d;
-  HookBufs hb;
-  DecodeState s;
-  memset(&s, 0, sizeof(s));   // the two kernels read only slot and done
-  s.slot = hb.upload(slot, B);
-  s.done = hb.upload(done, B);
-  PartialSrc q;
-  q.nsplit = q_nsplit;
-  q.stride = (long)R * d;
-  q.ptr = hb.upload(q_part, (size_t)std::max(q_nsplit, 1) * R * d);
-  q.bias = q_bias ? hb.upload(q_bias, d) : nullptr;
-  const __half* kc = hb.upload(reinterpret_cast<const __half*>(k_pool), (size_t)n_slots * slot_sz);
-  const __half* vc = hb.upload(reinterpret_cast<const __half*>(v_pool), (size_t)n_slots * slot_sz);
-  CrossAttnWorkspace ws;
-  ws.part = hb.alloc<float>((size_t)B * H * ns * MAX_ROWS_PER_STREAM * 66);
-  ws.probs = probs ? hb.alloc<float>((size_t)R * H * S_ENC) : nullptr;
-  if (ws.probs) WL_CUDA(cudaMemset(ws.probs, 0, (size_t)R * H * S_ENC * 4));
-  __half* dout = hb.alloc<__half>((size_t)R * d);
-  fill_f16(dout, (size_t)R * d, sentinel);
-  WL_CUDA(cudaDeviceSynchronize());
-  decoder_cross_attn(c->st, s, q, kc, vc, slot_sz, ws, dout, B, rows_per_stream, H, d, ns);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  download_f16(dout, out, (size_t)R * d);
-  if (probs) WL_CUDA(cudaMemcpy(probs, ws.probs, (size_t)R * H * S_ENC * 4, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_test_self_attn(wl_ctx* c, const float* qkv_part, const float* qkv_bias, int32_t nsplit, uint16_t* k_cache,
-                                 uint16_t* v_cache, int32_t n_rows, const int16_t* src, const int32_t* pos, const int32_t* active,
-                                 const int32_t* wrow, int32_t R, int32_t H, float sentinel, float* out) {
-  API_BEGIN(c)
-  PdlScope pdl(false);
-  WL_CHECK(qkv_part && k_cache && v_cache && src && pos && active && out && R > 0 && H > 0 && n_rows > 0 && nsplit >= 1 &&
-               nsplit <= 8,
-           WL_ERR_ARG, "wl_test_self_attn: bad arguments");
-  for (int r = 0; r < R; ++r) {
-    WL_CHECK(pos[r] >= 0 && pos[r] < T_MAX && (wrow ? wrow[r] : r) >= 0 && (wrow ? wrow[r] : r) < n_rows, WL_ERR_ARG,
-             "wl_test_self_attn: row %d: position or write row out of range", r);
-    for (int p = 0; active[r] && p < pos[r]; ++p)
-      WL_CHECK(src[(long)r * T_MAX + p] >= 0 && src[(long)r * T_MAX + p] < n_rows, WL_ERR_ARG, "wl_test_self_attn: src out of range");
-  }
-  const int d = H * 64;
-  const long row_stride = (long)H * T_MAX * 64;
-  HookBufs hb;
-  DecodeState s;
-  memset(&s, 0, sizeof(s));   // the kernel reads only src, pos, active and wrow
-  s.src = hb.upload(src, (size_t)R * T_MAX);
-  s.pos = hb.upload(pos, R);
-  s.active = hb.upload(active, R);
-  s.wrow = wrow ? hb.upload(wrow, R) : nullptr;
-  PartialSrc qkv;
-  qkv.nsplit = nsplit;
-  qkv.stride = (long)R * 3 * d;
-  qkv.ptr = hb.upload(qkv_part, (size_t)nsplit * R * 3 * d);
-  qkv.bias = qkv_bias ? hb.upload(qkv_bias, 3 * d) : nullptr;
-  __half* kc = hb.upload(reinterpret_cast<__half*>(k_cache), (size_t)n_rows * row_stride);
-  __half* vc = hb.upload(reinterpret_cast<__half*>(v_cache), (size_t)n_rows * row_stride);
-  __half* dout = hb.alloc<__half>((size_t)R * d);
-  fill_f16(dout, (size_t)R * d, sentinel);
-  WL_CUDA(cudaDeviceSynchronize());
-  decoder_self_attn(c->st, s, qkv, kc, vc, row_stride, dout, R, H, d);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  download_f16(dout, out, (size_t)R * d);
-  WL_CUDA(cudaMemcpy(k_cache, kc, (size_t)n_rows * row_stride * 2, cudaMemcpyDeviceToHost));
-  WL_CUDA(cudaMemcpy(v_cache, vc, (size_t)n_rows * row_stride * 2, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_test_fold(wl_ctx* c, int32_t mode, float* x, const float* part, int32_t nsplit, const float* bias,
-                            const float* gamma, const float* beta, float* y, int32_t rows, int32_t cols) {
-  API_BEGIN(c)
-  PdlScope pdl(false);
-  WL_CHECK(y && rows > 0 && cols > 0 && (mode == 0 || mode == 1) && nsplit >= 0 && nsplit <= 8 && (nsplit == 0 || part),
-           WL_ERR_ARG, "wl_test_fold: bad arguments");
-  WL_CHECK(mode == 1 || (x && gamma && beta), WL_ERR_ARG, "wl_test_fold: layernorm_update needs x, gamma and beta");
-  WL_CHECK(mode == 0 || nsplit >= 1, WL_ERR_ARG, "wl_test_fold: gelu_cast needs at least one K range");
-  const size_t n = (size_t)rows * cols;
-  HookBufs hb;
-  PartialSrc upd;
-  upd.nsplit = nsplit;
-  upd.stride = (long)n;
-  upd.ptr = nsplit ? hb.upload(part, (size_t)nsplit * n) : nullptr;
-  upd.bias = bias ? hb.upload(bias, cols) : nullptr;
-  __half* dy = hb.alloc<__half>(n);
-  WL_CUDA(cudaMemset(dy, 0, n * 2));
-  float* dx = mode == 0 ? hb.upload(x, n) : nullptr;
-  const float* dg = mode == 0 ? hb.upload(gamma, cols) : nullptr;
-  const float* db = mode == 0 ? hb.upload(beta, cols) : nullptr;
-  WL_CUDA(cudaDeviceSynchronize());
-  if (mode == 0) layernorm_update_rows(c->st, dx, upd, dg, db, dy, rows, cols);
-  else gelu_cast(c->st, upd, dy, rows, cols);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  download_f16(dy, y, n);
-  if (mode == 0) WL_CUDA(cudaMemcpy(x, dx, n * 4, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-// Test hooks of the encoder-pass kernels: each runs the code encoder_pass runs, on its own device copies of the inputs.
-extern "C" int wl_test_enc_attn(wl_ctx* c, const uint16_t* qk_f16, const uint16_t* vt_f16, uint16_t* out_f16, int32_t nb,
-                                int32_t H, int32_t path, int32_t ab) {
-  API_BEGIN(c)
-  WL_CHECK(qk_f16 && vt_f16 && out_f16 && nb >= 1 && H >= 1 && H <= 32 && (path == 0 || path == 1) && ab >= 0, WL_ERR_ARG,
-           "wl_test_enc_attn: bad arguments");
-  const int d = H * 64;
-  const size_t n_qk = (size_t)nb * S_ENC * 2 * d, n_vt = (size_t)nb * d * S_PAD, n_out = ((size_t)nb * S_ENC + 128) * d;
-  HookBufs hb;
-  const __half* dqk = hb.upload(reinterpret_cast<const __half*>(qk_f16), n_qk);
-  const __half* dvt = hb.upload(reinterpret_cast<const __half*>(vt_f16), n_vt);
-  __half* dout = hb.upload(reinterpret_cast<const __half*>(out_f16), n_out);
-  if (path == 0) {
-    WL_CUDA(cudaDeviceSynchronize());
-    encoder_attention_fused(c->st, dqk, dvt, dout, nb, H, d);
-  } else {
-    const int AB = ab ? ab : std::min(nb, enc_attn_streams(d));
-    float* scores = hb.alloc<float>((size_t)AB * H * S_ENC * S_PAD);
-    __half* probs16 = hb.alloc<__half>((size_t)AB * H * S_ENC * S_PAD);
-    // zeroed like the engine's workspaces: the scores GEMM never writes the pad columns, softmax_rows writes all of P
-    WL_CUDA(cudaMemset(scores, 0, (size_t)AB * H * S_ENC * S_PAD * 4));
-    WL_CUDA(cudaMemset(probs16, 0, (size_t)AB * H * S_ENC * S_PAD * 2));
-    WL_CUDA(cudaDeviceSynchronize());
-    encoder_attention_unfused(c->st, dqk, dvt, dout, scores, probs16, nb, H, AB);
-  }
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  WL_CUDA(cudaMemcpy(out_f16, dout, n_out * 2, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_test_enc_stem(wl_ctx* c, const float* feats_f32, float* x_out_f32, int32_t nb) {
-  API_BEGIN(c)
-  WL_CHECK(c->finalized, WL_ERR_STATE, "weights not finalized");
-  WL_CHECK(feats_f32 && x_out_f32 && nb >= 1, WL_ERR_ARG, "wl_test_enc_stem: bad arguments");
-  const int d = c->d, nm = c->n_mels;
-  HookBufs hb;
-  const float* dfeat = hb.upload(feats_f32, (size_t)nb * nm * 3000);
-  // the engine's shapes, slack included; zeroed: rows 0 and 3001 of every stream are the conv padding
-  const size_t n16 = (size_t)nb * 3002 * nm + 4096, n1 = (size_t)nb * 3002 * d + 4096, nx = (size_t)nb * S_ENC * d;
-  __half* feat16 = hb.alloc<__half>(n16);
-  __half* conv1o = hb.alloc<__half>(n1);
-  float* x = hb.alloc<float>(nx);
-  WL_CUDA(cudaMemset(feat16, 0, n16 * 2));
-  WL_CUDA(cudaMemset(conv1o, 0, n1 * 2));
-  WL_CUDA(cudaMemset(x, 0xff, nx * 4));   // NaN: an element the stem did not write cannot pass as a value
-  WL_CUDA(cudaDeviceSynchronize());
-  encoder_stem(c, c->st, nb, dfeat, feat16, conv1o, x);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  WL_CUDA(cudaMemcpy(x_out_f32, x, nx * 4, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_test_layernorm(wl_ctx* c, const float* x_f32, const float* gamma, const float* beta, float* y16_as_f32,
-                                 float* y32, int32_t rows, int32_t d) {
-  API_BEGIN(c)
-  WL_CHECK(x_f32 && gamma && beta && rows >= 1 && d >= 4, WL_ERR_ARG, "wl_test_layernorm: bad arguments");
-  // the outputs carry 8 guard rows after the last one: the grid covers whole blocks of 8 rows
-  const size_t n = (size_t)rows * d, ng = (size_t)(rows + 8) * d;
-  HookBufs hb;
-  const float* dx = hb.upload(x_f32, n);
-  const float* dg = hb.upload(gamma, d);
-  const float* db = hb.upload(beta, d);
-  __half* dy = nullptr;
-  float* dy32 = nullptr;
-  if (y16_as_f32) {
-    std::vector<__half> h(ng);
-    for (size_t i = 0; i < ng; ++i) h[i] = __float2half_rn(y16_as_f32[i]);
-    dy = hb.upload(h.data(), ng);
-  }
-  if (y32) dy32 = hb.upload(y32, ng);
-  WL_CUDA(cudaDeviceSynchronize());
-  layernorm_rows(c->st, dx, dg, db, dy, dy32, rows, d);
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  if (y16_as_f32) download_f16(dy, y16_as_f32, ng);
-  if (y32) WL_CUDA(cudaMemcpy(y32, dy32, ng * 4, cudaMemcpyDeviceToHost));
-  API_END(c)
-}
-
-extern "C" int wl_bench_gemm(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,
-                             float* ms_out) {
-  // flags: 1 transposed (swap-AB) store, 2 bias, 4 GELU, 8 fp32 output with fp32 residual (in place), 16 bias on m,
-  // 32 A shared by the batch, 64 output rows padded to a multiple of 64 elements (V^T: S_PAD)
-  API_BEGIN(c)
-  WL_CHECK(ms_out && M > 0 && N > 0 && K > 0 && batch > 0 && iters > 0, WL_ERR_ARG, "wl_bench_gemm: bad arguments");
-  __half *da = nullptr, *db = nullptr;
-  void* dc = nullptr;
-  float* dbias = nullptr;
-  const bool tr = flags & 1, f32 = flags & 8, a_shared = flags & 32;
-  const long ld = (flags & 64) ? (N + 63) / 64 * 64 : N;
-  const size_t na = (size_t)(a_shared ? 1 : batch) * M * K, nb = (size_t)batch * N * K, nc = (size_t)batch * M * ld;
-  WL_CUDA(cudaMalloc((void**)&da, na * 2));
-  WL_CUDA(cudaMalloc((void**)&db, nb * 2));
-  WL_CUDA(cudaMalloc(&dc, nc * (f32 ? 4 : 2)));
-  WL_CUDA(cudaMalloc((void**)&dbias, (size_t)std::max(M, N) * 4));
-  WL_CUDA(cudaMemset(da, 0x11, na * 2));
-  WL_CUDA(cudaMemset(db, 0x11, nb * 2));
-  WL_CUDA(cudaMemset(dc, 0, nc * (f32 ? 4 : 2)));
-  WL_CUDA(cudaMemset(dbias, 0, (size_t)std::max(M, N) * 4));
-  WL_CUDA(cudaDeviceSynchronize());
-  GemmEpilogue e;
-  e.out = dc; e.out_f32 = f32 ? 1 : 0;
-  if (tr) { e.ldm = 1; e.ldn = M; } else { e.ldm = ld; e.ldn = 1; }
-  e.ob1 = (long)M * ld;
-  if (flags & 2) { e.bias = dbias; e.bias_on_m = (tr || (flags & 16)) ? 1 : 0; }
-  if (flags & 4) e.gelu = 1;
-  if (f32) { e.resid = (const float*)dc; e.rldm = e.ldm; e.rldn = e.ldn; e.rb1 = e.ob1; }
-  try {
-    GemmOperand A = opnd(da, M, K, K, a_shared ? 1 : batch, a_shared ? 0 : (long)M * K), Bo = opnd(db, N, K, K, batch, (long)N * K);
-    for (int i = 0; i < 3; ++i) gemm_tn(c->st, A, Bo, M, N, K, e);
-    WL_CUDA(cudaEventRecord(c->ev0, c->st));
-    for (int i = 0; i < iters; ++i) gemm_tn(c->st, A, Bo, M, N, K, e);
-    WL_CUDA(cudaEventRecord(c->ev1, c->st));
-    WL_CUDA(cudaStreamSynchronize(c->st));
-    float ms;
-    WL_CUDA(cudaEventElapsedTime(&ms, c->ev0, c->ev1));
-    *ms_out = ms / iters;
-  } catch (...) {
-    cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dbias);
-    throw;
-  }
-  cudaFree(da); cudaFree(db); cudaFree(dc); cudaFree(dbias);
   API_END(c)
 }

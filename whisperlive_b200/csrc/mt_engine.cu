@@ -1,17 +1,11 @@
 // Translation context and C ABI (include/wlb200.h, wl_mt_*): M2M100 encoder over the packed source tokens of a call, the
 // decoder's cross K/V once per call, then the token loop (decoder step + beam-search step) as one CUDA graph with a
 // conditional WHILE node, so no host synchronisation happens per token.
-#include <algorithm>
 #include <cmath>
-#include <map>
-#include <string>
-#include <vector>
+#include <cstring>
 
-#include "../../include/wlb200.h"
-#include "gemm.cuh"
+#include "ctx.cuh"
 #include "mt.cuh"
-
-using namespace wl;
 
 namespace wl {
 void gemm_prime();
@@ -25,14 +19,13 @@ struct MtTensor {
 
 struct wl_mt_ctx {
   wl_mt_config cfg;
-  int device = 0, Bc = 0, Km = 0, Ns = 0, Rm = 0, Vld = 0;
+  int Bc = 0, Km = 0, Ns = 0, Rm = 0, Vld = 0;
   int d = 0, H = 0, ff = 0, Le = 0, Ld = 0, V = 0;
   cudaStream_t st = nullptr;
   std::string err;
   std::map<std::string, MtTensor> w;
   bool finalized = false;
-  int64_t bytes = 0;
-  std::vector<void*> allocs;
+  DeviceMem mem;
   // encoder
   float* ex = nullptr;
   __half *eh = nullptr, *eqkv = nullptr, *eattn = nullptr, *eff = nullptr, *xkv = nullptr;
@@ -45,38 +38,11 @@ struct wl_mt_ctx {
   std::map<std::string, cudaGraphExec_t> graphs;
 };
 
-#define MT_BEGIN(ctx)                                           \
-  if (!(ctx)) return WL_ERR_ARG;                                \
-  try {                                                         \
-    WL_CUDA(cudaSetDevice((ctx)->device));
-#define MT_END(ctx)                                             \
-  }                                                             \
-  catch (const wl::Error& e) {                                  \
-    (ctx)->err = e.msg;                                         \
-    return e.code;                                              \
-  }                                                             \
-  catch (const std::exception& e) {                             \
-    (ctx)->err = e.what();                                      \
-    return WL_ERR_STATE;                                        \
-  }                                                             \
-  return WL_OK;
-
 static std::string g_mt_init_error;
-
-template <class T>
-static T* mt_alloc(wl_mt_ctx* c, size_t n) {
-  void* p = nullptr;
-  const size_t bytes = std::max<size_t>(n, 1) * sizeof(T);
-  WL_CHECK(cudaMalloc(&p, bytes) == cudaSuccess, WL_ERR_NOMEM, "wl_mt: out of device memory allocating %zu bytes", bytes);
-  WL_CUDA(cudaMemsetAsync(p, 0, bytes, c->st));
-  c->allocs.push_back(p);
-  c->bytes += (int64_t)bytes;
-  return (T*)p;
-}
 
 static void mt_free(wl_mt_ctx* c) {
   for (auto& kv : c->graphs) cudaGraphExecDestroy(kv.second);
-  for (void* p : c->allocs) cudaFree(p);
+  c->mem.release_from(0);
   if (c->st) cudaStreamDestroy(c->st);
 }
 
@@ -122,7 +88,7 @@ extern "C" int wl_mt_init(const wl_mt_config* cfg, int32_t device, int32_t capac
     WL_CUDA(cudaGetDeviceProperties(&prop, device));
     WL_CHECK(prop.major == 9 && prop.minor == 0, WL_ERR_CUDA, "libwlb200 is built for sm_90a only; device is sm_%d%d", prop.major, prop.minor);
     c->cfg = *cfg;
-    c->device = device;
+    c->mem.device = device;
     c->d = cfg->d_model; c->H = cfg->n_heads; c->ff = cfg->ffn; c->Le = cfg->enc_layers; c->Ld = cfg->dec_layers; c->V = cfg->vocab;
     WL_CHECK(c->H >= 1 && c->d == 64 * c->H && c->d <= 1280, WL_ERR_ARG, "wl_mt_init: d_model %d / heads %d unsupported (head dim 64)", c->d, c->H);
     WL_CHECK(c->ff >= 64 && c->ff % 64 == 0 && c->Le >= 1 && c->Ld >= 1 && c->V >= 16, WL_ERR_ARG, "wl_mt_init: bad shape");
@@ -133,47 +99,48 @@ extern "C" int wl_mt_init(const wl_mt_config* cfg, int32_t device, int32_t capac
     c->Bc = capacity_segments; c->Km = max_beam; c->Ns = cfg->max_src_tokens; c->Rm = c->Bc * c->Km;
     c->Vld = (c->V + 7) / 8 * 8;
     WL_CUDA(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
+    c->mem.st = c->st;
     gemm_prime();
     mt_table(c);
     const long d = c->d, Ns = c->Ns, Rm = c->Rm;
-    c->ex = mt_alloc<float>(c, Ns * d);
-    c->eh = mt_alloc<__half>(c, Ns * d);
-    c->eqkv = mt_alloc<__half>(c, Ns * 3 * d);
-    c->eattn = mt_alloc<__half>(c, Ns * d);
-    c->eff = mt_alloc<__half>(c, Ns * c->ff);
-    c->xkv = mt_alloc<__half>(c, Ns * 2 * d * c->Ld);
-    c->etok = mt_alloc<int>(c, Ns);
-    c->etpos = mt_alloc<int>(c, Ns);
-    c->eoff = mt_alloc<int>(c, c->Bc + 1);
-    c->etiles = mt_alloc<int2>(c, Ns / 64 + c->Bc);
-    c->dx = mt_alloc<float>(c, Rm * d);
-    c->dqkv = mt_alloc<float>(c, Rm * 3 * d);
-    c->dq = mt_alloc<float>(c, Rm * d);
-    c->logits = mt_alloc<float>(c, Rm * c->Vld);
-    c->dh = mt_alloc<__half>(c, Rm * d);
-    c->dattn = mt_alloc<__half>(c, Rm * d);
-    c->dff = mt_alloc<__half>(c, Rm * c->ff);
-    c->kc = mt_alloc<__half>(c, (long)c->Ld * Rm * d * T_MAX);
-    c->vc = mt_alloc<__half>(c, (long)c->Ld * Rm * d * T_MAX);
+    c->ex = c->mem.alloc<float>(Ns * d);
+    c->eh = c->mem.alloc<__half>(Ns * d);
+    c->eqkv = c->mem.alloc<__half>(Ns * 3 * d);
+    c->eattn = c->mem.alloc<__half>(Ns * d);
+    c->eff = c->mem.alloc<__half>(Ns * c->ff);
+    c->xkv = c->mem.alloc<__half>(Ns * 2 * d * c->Ld);
+    c->etok = c->mem.alloc<int>(Ns);
+    c->etpos = c->mem.alloc<int>(Ns);
+    c->eoff = c->mem.alloc<int>(c->Bc + 1);
+    c->etiles = c->mem.alloc<int2>(Ns / 64 + c->Bc);
+    c->dx = c->mem.alloc<float>(Rm * d);
+    c->dqkv = c->mem.alloc<float>(Rm * 3 * d);
+    c->dq = c->mem.alloc<float>(Rm * d);
+    c->logits = c->mem.alloc<float>(Rm * c->Vld);
+    c->dh = c->mem.alloc<__half>(Rm * d);
+    c->dattn = c->mem.alloc<__half>(Rm * d);
+    c->dff = c->mem.alloc<__half>(Rm * c->ff);
+    c->kc = c->mem.alloc<__half>((long)c->Ld * Rm * d * T_MAX);
+    c->vc = c->mem.alloc<__half>((long)c->Ld * Rm * d * T_MAX);
     MtState& s = c->s;
-    s.tok_in = mt_alloc<int>(c, Rm);
-    s.pos = mt_alloc<int>(c, Rm);
-    s.active = mt_alloc<int>(c, Rm);
-    s.src = mt_alloc<short>(c, Rm * T_MAX);
-    s.hist = mt_alloc<int>(c, Rm * T_MAX);
-    s.run_score = mt_alloc<float>(c, Rm);
-    s.run_next = mt_alloc<float>(c, Rm);
-    s.cand_val = mt_alloc<float>(c, Rm * MT_MAX_CAND);
-    s.cand_tok = mt_alloc<int>(c, Rm * MT_MAX_CAND);
-    s.fin_score = mt_alloc<float>(c, Rm);
-    s.fin_flag = mt_alloc<int>(c, Rm);
-    s.fin_len = mt_alloc<int>(c, Rm);
-    s.fin_tok = mt_alloc<int>(c, (long)c->Bc * MT_MAX_BEAM * T_MAX);
-    s.done = mt_alloc<int>(c, c->Bc);
-    s.unsat = mt_alloc<int>(c, c->Bc);
-    s.steps = mt_alloc<int>(c, c->Bc);
-    s.n_done = mt_alloc<int>(c, 1);
-    s.steps_left = mt_alloc<int>(c, 1);
+    s.tok_in = c->mem.alloc<int>(Rm);
+    s.pos = c->mem.alloc<int>(Rm);
+    s.active = c->mem.alloc<int>(Rm);
+    s.src = c->mem.alloc<short>(Rm * T_MAX);
+    s.hist = c->mem.alloc<int>(Rm * T_MAX);
+    s.run_score = c->mem.alloc<float>(Rm);
+    s.run_next = c->mem.alloc<float>(Rm);
+    s.cand_val = c->mem.alloc<float>(Rm * MT_MAX_CAND);
+    s.cand_tok = c->mem.alloc<int>(Rm * MT_MAX_CAND);
+    s.fin_score = c->mem.alloc<float>(Rm);
+    s.fin_flag = c->mem.alloc<int>(Rm);
+    s.fin_len = c->mem.alloc<int>(Rm);
+    s.fin_tok = c->mem.alloc<int>((long)c->Bc * MT_MAX_BEAM * T_MAX);
+    s.done = c->mem.alloc<int>(c->Bc);
+    s.unsat = c->mem.alloc<int>(c->Bc);
+    s.steps = c->mem.alloc<int>(c->Bc);
+    s.n_done = c->mem.alloc<int>(1);
+    s.steps_left = c->mem.alloc<int>(1);
     s.forced_bos = s.forced_eos = -1;
     WL_CUDA(cudaStreamSynchronize(c->st));
   } catch (const wl::Error& e) {
@@ -188,7 +155,7 @@ extern "C" int wl_mt_init(const wl_mt_config* cfg, int32_t device, int32_t capac
 
 extern "C" void wl_mt_destroy(wl_mt_ctx* c) {
   if (!c) return;
-  cudaSetDevice(c->device);
+  cudaSetDevice(c->mem.device);
   if (c->st) cudaStreamSynchronize(c->st);
   mt_free(c);
   delete c;
@@ -197,14 +164,14 @@ extern "C" void wl_mt_destroy(wl_mt_ctx* c) {
 extern "C" const char* wl_mt_last_error(wl_mt_ctx* c) { return c ? c->err.c_str() : g_mt_init_error.c_str(); }
 
 extern "C" int wl_mt_device_bytes(wl_mt_ctx* c, int64_t* out) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(out, WL_ERR_ARG, "wl_mt_device_bytes: null output");
-  *out = c->bytes;
-  MT_END(c)
+  *out = c->mem.bytes;
+  API_END(c)
 }
 
 extern "C" int wl_mt_load_tensor(wl_mt_ctx* c, const char* name, const float* data, const int64_t* shape, int32_t ndim) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(name && data && shape && ndim >= 1, WL_ERR_ARG, "wl_mt_load_tensor: bad arguments");
   auto it = c->w.find(name);
   WL_CHECK(it != c->w.end(), WL_ERR_ARG, "wl_mt_load_tensor: unknown tensor '%s'", name);
@@ -212,27 +179,20 @@ extern "C" int wl_mt_load_tensor(wl_mt_ctx* c, const char* name, const float* da
   WL_CHECK(std::vector<int64_t>(shape, shape + ndim) == t.shape, WL_ERR_ARG, "wl_mt_load_tensor: '%s' has the wrong shape", name);
   long n = 1;
   for (int64_t s : t.shape) n *= s;
-  float* tmp = nullptr;
-  WL_CUDA(cudaMalloc(&tmp, n * sizeof(float)));
-  try {
-    WL_CUDA(cudaMemcpyAsync(tmp, data, n * sizeof(float), cudaMemcpyHostToDevice, c->st));
-    if (!t.p) t.p = t.f16 ? (void*)mt_alloc<__half>(c, n) : (void*)mt_alloc<float>(c, n);
-    if (t.f16) cast_weight_f16(c->st, tmp, (__half*)t.p, n, 1, 1);
-    else WL_CUDA(cudaMemcpyAsync(t.p, tmp, n * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
-    WL_CUDA(cudaStreamSynchronize(c->st));
-  } catch (...) {
-    cudaFree(tmp);
-    throw;
-  }
-  cudaFree(tmp);
-  MT_END(c)
+  if (!t.p) t.p = t.f16 ? (void*)c->mem.alloc<__half>(n) : (void*)c->mem.alloc<float>(n);
+  Scratch sc(c->st);
+  const float* tmp = sc.upload(data, n);
+  if (t.f16) cast_weight_f16(c->st, tmp, (__half*)t.p, n, 1, 1);
+  else WL_CUDA(cudaMemcpyAsync(t.p, tmp, n * sizeof(float), cudaMemcpyDeviceToDevice, c->st));
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  API_END(c)
 }
 
 extern "C" int wl_mt_finalize(wl_mt_ctx* c) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   for (auto& kv : c->w) WL_CHECK(kv.second.p, WL_ERR_STATE, "wl_mt_finalize: missing tensor '%s'", kv.first.c_str());
   c->finalized = true;
-  MT_END(c)
+  API_END(c)
 }
 
 // ---------------------------------------------------------------------------------------------- building blocks
@@ -388,7 +348,7 @@ static void upload_and_encode(wl_mt_ctx* c, const int32_t* src_ids, const int32_
 
 extern "C" int wl_mt_translate(wl_mt_ctx* c, const int32_t* src_ids, const int32_t* src_off, int32_t B, const wl_mt_opts* o,
                                int32_t* out_ids, int32_t* out_len, float* out_score) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(c->finalized, WL_ERR_STATE, "wl_mt_translate: weights not finalized");
   WL_CHECK(src_ids && out_ids && out_len && out_score, WL_ERR_ARG, "wl_mt_translate: bad arguments");
   const MtSearch so = search_opts(c, o, B, "wl_mt_translate");
@@ -440,79 +400,66 @@ extern "C" int wl_mt_translate(wl_mt_ctx* c, const int32_t* src_ids, const int32
     }
   }
   collect(c, B, so, out_ids, out_len, out_score, nullptr);
-  MT_END(c)
+  API_END(c)
 }
 
 // ---------------------------------------------------------------------------------------------- test hooks
-template <class T>
-struct DevBuf {
-  T* p = nullptr;
-  explicit DevBuf(size_t n) { WL_CUDA(cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T))); }
-  ~DevBuf() { cudaFree(p); }
-};
-
 extern "C" int wl_test_mt_attn(wl_mt_ctx* c, const uint16_t* qkv_f16, const int32_t* off, int32_t B, int32_t H, uint16_t* out_f16) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(qkv_f16 && out_f16 && B >= 1 && H >= 1 && H <= 20, WL_ERR_ARG, "wl_test_mt_attn: bad arguments");
   check_off(off, B, MT_MAX_SRC, 1L << 30, "wl_test_mt_attn");
   const int d = 64 * H, n = off[B];
   std::vector<int> tpos;
   std::vector<int2> tiles;
   const int n_tiles = enc_tables(nullptr, off, B, 0, tpos, tiles);
-  DevBuf<__half> qkv((size_t)n * 3 * d), out((size_t)n * d);
-  DevBuf<int> doff(B + 1);
-  DevBuf<int2> dtiles(n_tiles);
-  WL_CUDA(cudaMemcpyAsync(qkv.p, qkv_f16, (size_t)n * 3 * d * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(out.p, out_f16, (size_t)n * d * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(doff.p, off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(dtiles.p, tiles.data(), n_tiles * sizeof(int2), cudaMemcpyHostToDevice, c->st));
-  mt_enc_attn(c->st, qkv.p, doff.p, dtiles.p, n_tiles, out.p, H, d);
-  WL_CUDA(cudaMemcpyAsync(out_f16, out.p, (size_t)n * d * 2, cudaMemcpyDeviceToHost, c->st));
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  MT_END(c)
+  Scratch sc(c->st);
+  const __half* qkv = sc.upload(reinterpret_cast<const __half*>(qkv_f16), (size_t)n * 3 * d);
+  __half* out = sc.upload(reinterpret_cast<const __half*>(out_f16), (size_t)n * d);
+  const int* doff = sc.upload(off, B + 1);
+  const int2* dtiles = sc.upload(tiles.data(), n_tiles);
+  mt_enc_attn(c->st, qkv, doff, dtiles, n_tiles, out, H, d);
+  sc.download(reinterpret_cast<__half*>(out_f16), out, (size_t)n * d);
+  API_END(c)
 }
 
 extern "C" int wl_test_mt_cross_attn(wl_mt_ctx* c, const float* q, const uint16_t* kv_f16, int32_t ldkv, int32_t koff, int32_t voff,
                                      const int32_t* off, int32_t B, int32_t rows_per_seg, int32_t H, uint16_t* out_f16) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(q && kv_f16 && out_f16 && B >= 1 && rows_per_seg >= 1 && H >= 1 && H <= 20, WL_ERR_ARG, "wl_test_mt_cross_attn: bad arguments");
   const int d = 64 * H, R = B * rows_per_seg;
   WL_CHECK(ldkv % 8 == 0 && koff % 8 == 0 && voff % 8 == 0 && koff + d <= ldkv && voff + d <= ldkv, WL_ERR_ARG,
            "wl_test_mt_cross_attn: bad K/V layout");
   check_off(off, B, MT_MAX_SRC, 1L << 30, "wl_test_mt_cross_attn");
   const int n = off[B];
-  DevBuf<float> dq((size_t)R * d);
-  DevBuf<__half> kv((size_t)n * ldkv), out((size_t)R * d);
-  DevBuf<int> doff(B + 1);
-  WL_CUDA(cudaMemcpyAsync(dq.p, q, (size_t)R * d * 4, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(kv.p, kv_f16, (size_t)n * ldkv * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(out.p, out_f16, (size_t)R * d * 2, cudaMemcpyHostToDevice, c->st));
-  WL_CUDA(cudaMemcpyAsync(doff.p, off, (B + 1) * sizeof(int), cudaMemcpyHostToDevice, c->st));
+  Scratch sc(c->st);
+  const float* dq = sc.upload(q, (size_t)R * d);
+  const __half* kv = sc.upload(reinterpret_cast<const __half*>(kv_f16), (size_t)n * ldkv);
+  __half* out = sc.upload(reinterpret_cast<const __half*>(out_f16), (size_t)R * d);
+  const int* doff = sc.upload(off, B + 1);
   MtState s;
   memset(&s, 0, sizeof(s));   // no active table: every row
-  mt_cross_attn(c->st, s, dq.p, kv.p, ldkv, koff, voff, doff.p, rows_per_seg, out.p, R, H, d);
-  WL_CUDA(cudaMemcpyAsync(out_f16, out.p, (size_t)R * d * 2, cudaMemcpyDeviceToHost, c->st));
-  WL_CUDA(cudaStreamSynchronize(c->st));
-  MT_END(c)
+  mt_cross_attn(c->st, s, dq, kv, ldkv, koff, voff, doff, rows_per_seg, out, R, H, d);
+  sc.download(reinterpret_cast<__half*>(out_f16), out, (size_t)R * d);
+  API_END(c)
 }
 
 extern "C" int wl_test_mt_search(wl_mt_ctx* c, const float* logits, int32_t V, int32_t B, const wl_mt_opts* o, int32_t* out_ids,
                                  int32_t* out_len, float* out_score, int32_t* out_steps) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(logits && out_ids && out_len && out_score && out_steps && V >= 16, WL_ERR_ARG, "wl_test_mt_search: bad arguments");
   const MtSearch so = search_opts(c, o, B, "wl_test_mt_search");
   const int R = B * so.beam, steps = so.max_length - 1;
-  DevBuf<float> dl((size_t)steps * R * V);
-  WL_CUDA(cudaMemcpyAsync(dl.p, logits, (size_t)steps * R * V * 4, cudaMemcpyHostToDevice, c->st));
+  Scratch sc(c->st);
+  const float* dl = sc.upload(logits, (size_t)steps * R * V);
   mt_search_init(c->st, c->s, B, so.beam, o->decoder_start, steps);
-  for (int t = 0; t < steps; ++t) mt_search_step(c->st, c->s, so, dl.p + (size_t)t * R * V, V, V, B);
+  for (int t = 0; t < steps; ++t) mt_search_step(c->st, c->s, so, dl + (size_t)t * R * V, V, V, B);
   collect(c, B, so, out_ids, out_len, out_score, out_steps);
-  MT_END(c)
+  API_END(c)
 }
 
 extern "C" int wl_test_mt_logits(wl_mt_ctx* c, const int32_t* src_ids, const int32_t* src_off, int32_t B, const int32_t* prefix,
                                  int32_t P, float* out_logits) {
-  MT_BEGIN(c)
+  API_BEGIN(c)
   WL_CHECK(c->finalized, WL_ERR_STATE, "wl_test_mt_logits: weights not finalized");
   WL_CHECK(src_ids && prefix && out_logits && B >= 1 && B <= c->Bc && P >= 1 && P <= T_MAX && P <= c->cfg.max_positions,
            WL_ERR_ARG, "wl_test_mt_logits: bad arguments");
@@ -532,5 +479,5 @@ extern "C" int wl_test_mt_logits(wl_mt_ctx* c, const int32_t* src_ids, const int
     for (int b = 0; b < B; ++b)
       memcpy(out_logits + ((long)b * P + t) * c->V, lg.data() + (size_t)b * c->Vld, c->V * sizeof(float));
   }
-  MT_END(c)
+  API_END(c)
 }

@@ -107,7 +107,8 @@ def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 
     before a load.  ``vad=True`` adds the Silero VAD weights and the VAD workspace of ``max_streams`` 30-second chunks
     (``wl_vad_load_tensor``, ``wl_vad``); ``diarize=True`` the speaker-embedding weights and the workspace of its first
     call, ``max_streams`` segments of 30 s (``wl_spk_load_tensor``, ``wl_spk_embed``).  Not included: the CUDA context of the process, CUDA graph executables, workspaces grown later (longer
-    chunks, more prompt rows, the word-alignment buffers) and the allocator's rounding."""
+    chunks, more prompt rows, the word-alignment buffers; a grown workspace replaces the one before it, so it adds only
+    the difference) and the allocator's rounding."""
     B, K = int(max_streams), int(max_beam)
     NS = int(enc_slots) if enc_slots is not None else 2 * B
     d, H, Le, Ld, nm, V = dims.d_model, dims.n_heads, dims.enc_layers, dims.dec_layers, dims.n_mels, dims.vocab
@@ -323,7 +324,8 @@ class B200Whisper:
     @property
     def device_bytes(self) -> int:
         """Device memory this context holds right now (``wl_device_bytes``): weights, workspaces, slot pool, caches,
-        decode states and the workspaces grown so far; 0 once the context is destroyed."""
+        decode states and the grown workspaces at their current sizes (a grown workspace replaces the one before it);
+        0 once the context is destroyed."""
         out = C.c_int64(0)
         with self._lock:     # destroy() frees the context under the same lock
             if not self._fin.alive:
