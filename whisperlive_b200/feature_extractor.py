@@ -48,9 +48,14 @@ class ResidentFeatures:
         a, b, _ = sl.indices(self.stop - self.start)
         return ResidentFeatures(self.engine, self.stream, self.n_mels, self.start + a, self.start + max(a, b), self.epoch)
 
+    @property
+    def resident(self) -> bool:
+        """False once a later mel_device call on the engine has replaced these features."""
+        return getattr(self.engine, "_resident_epoch", None) == self.epoch
+
     def window(self, max_frames: int = 3000):
         """(stream, seek, length) for engine.encode_windows."""
-        if getattr(self.engine, "_resident_epoch", None) != self.epoch:
+        if not self.resident:
             raise RuntimeError("these features are no longer resident: a later mel_device call replaced them")
         return (self.stream, self.start, min(self.stop - self.start, max_frames))
 

@@ -27,6 +27,7 @@ import time
 import logging
 import os
 import zlib
+from math import ceil
 from dataclasses import asdict, dataclass, field, replace
 from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
@@ -275,6 +276,14 @@ class _StreamJob:
             self.temp_idx, self.tried, self.below_cr = 0, [], []
             return self.features[:, self.seek:self.seek + min(self.segment_size, fe.nb_max_frames)]
         return None
+
+    def prepare_decode(self) -> None:
+        """The window is encoded (``self.enc``): language id when ``multilingual``, then the prompt."""
+        if self.opt.multilingual:
+            tok_s, _p = self.m.model.detect_language(self.enc)[0][0]
+            self.tok.language = self.tok.tokenizer.token_to_id(tok_s)
+            self.tok.language_code = tok_s[2:-2]
+        self.build_prompt()
 
     def build_prompt(self) -> List[int]:
         self.prompt = self.m.get_prompt(
@@ -797,15 +806,11 @@ class TranscribeSession:
             tm["encode"] = tm.get("encode", 0.0) + time.perf_counter() - t0
             parent = _EncGroup(enc, len(grp))
             for k, e in enumerate(grp):
-                j = e.job
                 e.parent, e.index, e.window = parent, k, None
-                j.enc = enc.select([k]) if hasattr(enc, "select") else _EncoderSlice(enc, k)
+                e.job.enc = enc.select([k]) if hasattr(enc, "select") else _EncoderSlice(enc, k)
+            for e in grp:
                 try:
-                    if j.opt.multilingual:
-                        tok_s, _p = m.model.detect_language(j.enc)[0][0]
-                        j.tok.language = j.tok.tokenizer.token_to_id(tok_s)
-                        j.tok.language_code = tok_s[2:-2]
-                    j.build_prompt()
+                    e.job.prepare_decode()
                     e.state = "decode"
                 except Exception as ex:
                     self._fail(e, ex)
@@ -1301,9 +1306,11 @@ class B200WhisperModel:
         return out, seek, single_ending
 
     # -- word timestamps (K14 host part; reference :1515-1714) ------------------------------------
-    def add_word_timestamps(self, segments: List[List[dict]], tokenizer: Tokenizer, encoder_output, num_frames: int,
-                            prepend_punctuations: str, append_punctuations: str, last_speech_timestamp: float,
-                            precomputed=None):
+    def add_word_timestamps(self, segments: List[List[dict]], tokenizer: Tokenizer, encoder_output,
+                            num_frames: Union[int, Sequence[int]], prepend_punctuations: str, append_punctuations: str,
+                            last_speech_timestamp: float, precomputed=None):
+        """``num_frames``: one count for every window, or one per window (``BatchedInferencePipeline``, reference
+        :163-172, whose chunks differ in length)."""
         if len(segments) == 0:
             return
         per_seg_tokens = [[[t for t in sub["tokens"] if t < tokenizer.eot] for sub in seg] for seg in segments]
@@ -1362,8 +1369,9 @@ class B200WhisperModel:
                 sub["words"] = words
         return last_speech_timestamp
 
-    def find_alignment(self, tokenizer: Tokenizer, text_tokens: List[List[int]], encoder_output, num_frames: int,
-                       median_filter_width: int = 7, results=None) -> List[List[dict]]:
+    def find_alignment(self, tokenizer: Tokenizer, text_tokens: List[List[int]], encoder_output,
+                       num_frames: Union[int, Sequence[int]], median_filter_width: int = 7,
+                       results=None) -> List[List[dict]]:
         if len(text_tokens) == 0:
             return []
         if results is None:   # (the batched scheduler path hands in the engine results of its one align call)
@@ -1421,3 +1429,283 @@ class _EncoderSlice:
 
     def __init__(self, enc, index):
         self.enc, self.index = enc, index
+
+
+# --------------------------------------------------------------------------- batched long-file transcription
+class _ChunkRun:
+    """What the chunks of one ``BatchedInferencePipeline.transcribe`` call share: options, tokenizer, prompt, the
+    features, the word-timestamp carry-over from chunk to chunk, and the group being decoded."""
+
+    def __init__(self, model: "B200WhisperModel", tok: Tokenizer, options: TranscriptionOptions, audio_chunks,
+                 metadata: List[dict], features: List[Any], clips: List[dict]):
+        self.m, self.tok, self.opt = model, tok, options
+        self.audio_chunks, self.metadata, self.features, self.clips = audio_chunks, metadata, features, clips
+        self.last_speech_timestamp = 0.0
+        self.jobs: List["_ChunkJob"] = []
+        ip = options.initial_prompt
+        previous = [] if ip is None else (tok.encode(ip) if isinstance(ip, str) else list(ip))   # reference :184-193
+        self.prompt = model.get_prompt(tok, previous_tokens=previous, without_timestamps=options.without_timestamps,
+                                       hotwords=options.hotwords)
+        self.language_index = self.prompt.index(tok.language) if options.multilingual else -1
+
+    def max_length(self) -> int:
+        """Reference :195-209."""
+        o, m, n = self.opt, self.m, len(self.prompt)
+        max_length = m.max_length if o.max_new_tokens is None else n + o.max_new_tokens
+        if max_length > m.max_length:
+            raise ValueError(
+                f"The length of the prompt is {n}, and the `max_new_tokens` {max_length - n}. Thus, the combined length "
+                f"of the prompt and `max_new_tokens` is: {max_length}. This exceeds the `max_length` of the Whisper "
+                f"model: {m.max_length}. You should either reduce the length of your prompt, or reduce the value of "
+                f"`max_new_tokens`, so that their combined length is less that {m.max_length}.")
+        return max_length
+
+    def refresh_resident(self) -> None:
+        """Features kept in HBM are valid until the next mel call on the engine; if one ran while the caller held the
+        generator, compute them again (the same mel call, so the same values)."""
+        if self.features and not getattr(self.features[0], "resident", True):
+            fe = self.m.feature_extractor
+            self.features = [pad_or_trim(f[..., :-1]) for f in fe.batch_resident(self.audio_chunks)]
+
+    def chunk_language(self, job: "_ChunkJob") -> int:
+        """Language token of ``job``'s chunk: the top language of ONE ``detect_language`` call over every chunk of the
+        group whose encoder output is ready (reference :214-222)."""
+        if job.language is None:
+            todo = [j for j in self.jobs if j.enc is not None and j.language is None]
+            for j, langs in zip(todo, self.m.model.detect_language(_join_encoded([j.enc for j in todo]))):
+                j.language = self.tok.tokenizer.token_to_id(langs[0][0])
+        return job.language
+
+
+class _ChunkJob:
+    """One speech chunk of ``BatchedInferencePipeline``, driven by ``TranscribeSession`` rounds like a ``_StreamJob``
+    but with the reference's chunk rules (:121-254): one window, no previous text, no temperature ladder, no skipping
+    for silence, every sub-segment emitted."""
+
+    single_window = False
+
+    def __init__(self, run: _ChunkRun, index: int):
+        self.run, self.index = run, index
+        self.m, self.tok, self.opt = run.m, run.tok, run.opt
+        meta = run.metadata[index]
+        # the reference reads start_time / end_time; faster-whisper 1.2.0's collect_chunks gives offset / duration
+        # (start_time = offset, end_time = offset + duration), and the duration is taken back from the two the same way
+        start_time, end_time = meta["offset"], meta["offset"] + meta["duration"]
+        self.time_offset = start_time
+        self.segment_duration = end_time - start_time
+        self.segment_size = int(ceil(self.segment_duration) * self.m.frames_per_second)
+        self.seek = int(start_time * self.m.frames_per_second)
+        self.enc = None
+        self.prompt: List[int] = []
+        self.language: Optional[int] = None
+        self.segments: List[Segment] = []
+        self.current: Optional[List[dict]] = None
+        self.steps = 0
+        self._align_result = None
+        self._started = False
+
+    def advance_window(self):
+        if self._started:
+            return None
+        self._started = True
+        return self.run.features[self.index]
+
+    def prepare_decode(self) -> None:
+        self.prompt = list(self.run.prompt)
+        if self.opt.multilingual:
+            self.prompt[self.run.language_index] = self.run.chunk_language(self)
+
+    def generate_kwargs(self) -> dict:
+        """The reference's generate arguments (:224-238); what it leaves out stays at the engine's default
+        (``max_initial_timestamp_index`` 50, ``sampling_topk`` 1, so ``sampling_temperature`` does not sample)."""
+        o = self.opt
+        return dict(beam_size=o.beam_size, patience=o.patience, length_penalty=o.length_penalty,
+                    max_length=self.run.max_length(), suppress_blank=o.suppress_blank, suppress_tokens=o.suppress_tokens,
+                    return_scores=True, return_no_speech_prob=True, sampling_temperature=o.temperatures[0],
+                    repetition_penalty=o.repetition_penalty, no_repeat_ngram_size=o.no_repeat_ngram_size)
+
+    def accept(self, result) -> bool:
+        n = len(result.sequences_ids[0])
+        self.result = result
+        self.avg_logprob = result.scores[0] * (n ** self.opt.length_penalty) / (n + 1)
+        self.steps = int(getattr(result, "steps", n))
+        return True
+
+    def split(self) -> None:
+        pieces, _seek, _single = self.m._split_segments_by_timestamps(
+            tokenizer=self.tok, tokens=self.result.sequences_ids[0], time_offset=self.time_offset,
+            segment_size=self.segment_size, segment_duration=self.segment_duration, seek=0)
+        self.current = [dict(seek=self.seek, start=p["start"], end=p["end"], tokens=p["tokens"]) for p in pieces]
+
+    def alignment_request(self) -> List[int]:
+        self.split()
+        return [t for sub in self.current for t in sub["tokens"] if t < self.tok.eot]
+
+    def finish_window(self) -> None:
+        """Sub-segments (reference :128-162), words (:163-172; chunks settle in order, so the carry-over
+        ``last_speech_timestamp`` runs through them as through the reference's one call per batch), records (:547-566)."""
+        o, tok, run = self.opt, self.tok, self.run
+        if self.current is None:
+            self.split()
+        if o.word_timestamps:
+            pre = self._align_result
+            run.last_speech_timestamp = self.m.add_word_timestamps(
+                [self.current], tok, self.enc, [self.segment_size], o.prepend_punctuations, o.append_punctuations,
+                run.last_speech_timestamp, precomputed=None if pre is None else [pre])
+        for p in self.current:
+            text = tok.decode(p["tokens"])
+            self.segments.append(Segment(
+                id=0, seek=p["seek"], start=round(p["start"], 3), end=round(p["end"], 3), text=text, tokens=p["tokens"],
+                avg_logprob=self.avg_logprob, compression_ratio=get_compression_ratio(text),
+                no_speech_prob=self.result.no_speech_prob, temperature=o.temperatures[0],
+                words=[Word(**w) for w in p["words"]] if o.word_timestamps else None))
+
+
+class BatchedInferencePipeline:
+    """faster-whisper's batched long-file transcription (the reference vendors it: transcriber_faster_whisper.py
+    :113-571): VAD cuts the file into speech chunks of at most ``chunk_length`` seconds, and every chunk is decoded on
+    its own -- no previous-text prompt, no temperature ladder -- ``batch_size`` chunks per encode and ``generate``.
+
+    Two things differ from the vendored code, both as faster-whisper 1.2.0 has them: the chunks come from
+    ``collect_chunks(..., max_duration=chunk_length)`` (its ``offset`` / ``duration`` on the speech-only axis), and
+    ``restore_speech_timestamps`` maps the segments and words back to the original time axis.
+
+    On this engine one group is ``min(batch_size, max_streams)`` chunks: one mel call for the whole file, then per
+    group one encode, one ``detect_language`` (``multilingual``), one ``generate`` and one ``align``
+    (``word_timestamps``), driven by ``TranscribeSession`` rounds.  The calls are one-shot, so a ``TranscribeSession``
+    with an open step-level decode session on the same model keeps its streams."""
+
+    def __init__(self, model: "B200WhisperModel"):
+        self.model = model
+        self.resident_features = True        # False: features always go through the host (tests compare the paths)
+        self.group_steps: List[List[int]] = []   # token steps of every chunk, per group of the last transcribe call
+
+    def transcribe(self, audio, language: Optional[str] = None, task: str = "transcribe", log_progress: bool = False,
+                   beam_size: int = 5, best_of: int = 5, patience: float = 1, length_penalty: float = 1,
+                   repetition_penalty: float = 1, no_repeat_ngram_size: int = 0,
+                   temperature: Union[float, List[float], Tuple[float, ...]] = [0.0, 0.2, 0.4, 0.6, 0.8, 1.0],
+                   compression_ratio_threshold: Optional[float] = 2.4, log_prob_threshold: Optional[float] = -1.0,
+                   no_speech_threshold: Optional[float] = 0.6, condition_on_previous_text: bool = True,
+                   prompt_reset_on_temperature: float = 0.5, initial_prompt=None, prefix: Optional[str] = None,
+                   suppress_blank: bool = True, suppress_tokens: Optional[List[int]] = [-1],
+                   without_timestamps: bool = True, max_initial_timestamp: float = 1.0, word_timestamps: bool = False,
+                   prepend_punctuations: str = PUNCT_PREPEND, append_punctuations: str = PUNCT_APPEND,
+                   multilingual: bool = False, vad_filter: bool = True, vad_parameters=None,
+                   max_new_tokens: Optional[int] = None, chunk_length: Optional[int] = None,
+                   clip_timestamps: Optional[List[dict]] = None, hallucination_silence_threshold: Optional[float] = None,
+                   batch_size: int = 8, hotwords: Optional[str] = None,
+                   language_detection_threshold: Optional[float] = 0.5, language_detection_segments: int = 1):
+        """Reference :256-532: ``(generator of Segment, TranscriptionInfo)``.  The generator decodes group by group as
+        it is consumed.  ``compression_ratio_threshold``, ``log_prob_threshold``, ``no_speech_threshold``,
+        ``condition_on_previous_text``, ``prompt_reset_on_temperature``, ``prefix``, ``max_initial_timestamp`` and
+        ``hallucination_silence_threshold`` are accepted and unused, as in the reference; of ``temperature`` only the
+        first value is kept."""
+        if repetition_penalty != 1:
+            raise NotImplementedError(f"repetition_penalty={repetition_penalty}: the engine implements only 1")
+        if no_repeat_ngram_size != 0:
+            raise NotImplementedError(f"no_repeat_ngram_size={no_repeat_ngram_size}: the engine implements only 0")
+        m = self.model
+        fe = m.feature_extractor
+        sr = fe.sampling_rate
+        if multilingual and not m.model.is_multilingual:
+            m.logger.warning("The current model is English-only but the multilingual parameter is set to True; "
+                             "setting to False instead.")
+            multilingual = False
+        if not isinstance(audio, np.ndarray):
+            from .audio import decode_audio
+            audio = decode_audio(audio, sampling_rate=sr)
+        duration = audio.shape[0] / sr
+        chunk_length = chunk_length or fe.chunk_length
+        if not clip_timestamps:                                    # reference :393-417
+            if vad_filter:
+                vad = m._vad or _load_vad()
+                if vad_parameters is None:
+                    vad_parameters = vad.VadOptions(max_speech_duration_s=chunk_length, min_silence_duration_ms=160)
+                elif isinstance(vad_parameters, dict):
+                    params = {k: v for k, v in vad_parameters.items() if k != "max_speech_duration_s"}
+                    vad_parameters = vad.VadOptions(**params, max_speech_duration_s=chunk_length)
+                clip_timestamps = vad.get_speech_timestamps(audio, vad_parameters)
+            elif duration < chunk_length:
+                clip_timestamps = [{"start": 0, "end": audio.shape[0]}]
+            else:
+                raise RuntimeError("No clip timestamps found. Set 'vad_filter' to True or provide 'clip_timestamps'.")
+        duration_after_vad = sum(c["end"] - c["start"] for c in clip_timestamps) / sr
+
+        from . import vad as vad_mod
+        audio_chunks, metadata = vad_mod.collect_chunks(audio, clip_timestamps, sr, max_duration=chunk_length)
+        detect = language is None and m.model.is_multilingual
+        features: List[Any] = []
+        if duration_after_vad:
+            # ONE mel call for every chunk; resident in HBM when the chunks fit one call and nothing needs host values
+            cap = int(getattr(m.model, "max_streams", 0) or 0)
+            resident = (self.resident_features and hasattr(fe, "batch_resident") and len(audio_chunks) <= cap
+                        and not detect)
+            feats = fe.batch_resident(audio_chunks) if resident else fe.batch(audio_chunks)
+            features = [f[..., :-1] for f in feats]
+
+        all_language_probs = None
+        if language is None:                                       # reference :431-467
+            if not m.model.is_multilingual:
+                language, language_probability = "en", 1
+            else:
+                language, language_probability, all_language_probs = m.detect_language(
+                    features=np.concatenate(features + [np.full((m.model.n_mels, 1), -1.5, dtype="float32")], axis=1),
+                    language_detection_segments=language_detection_segments,
+                    language_detection_threshold=language_detection_threshold)
+                m.logger.info("Detected language '%s' with probability %.2f", language, language_probability)
+        else:
+            if not m.model.is_multilingual and language != "en":
+                m.logger.warning("The current model is English-only but the language parameter is set to '%s'; "
+                                 "using 'en' instead." % language)
+                language = "en"
+            language_probability = 1
+        tokenizer = Tokenizer(m.hf_tokenizer, m.model.is_multilingual, task=task, language=language)
+        features = [pad_or_trim(f) for f in features]
+
+        options = TranscriptionOptions(
+            beam_size=beam_size, best_of=best_of, patience=patience, length_penalty=length_penalty,
+            repetition_penalty=repetition_penalty, no_repeat_ngram_size=no_repeat_ngram_size,
+            log_prob_threshold=log_prob_threshold, no_speech_threshold=no_speech_threshold,
+            compression_ratio_threshold=compression_ratio_threshold,
+            temperatures=temperature[:1] if isinstance(temperature, (list, tuple)) else [temperature],
+            initial_prompt=initial_prompt, prefix=prefix, suppress_blank=suppress_blank,
+            suppress_tokens=get_suppressed_tokens(tokenizer, suppress_tokens),
+            prepend_punctuations=prepend_punctuations, append_punctuations=append_punctuations,
+            max_new_tokens=max_new_tokens, hotwords=hotwords, word_timestamps=word_timestamps,
+            hallucination_silence_threshold=None, condition_on_previous_text=False, clip_timestamps=clip_timestamps,
+            prompt_reset_on_temperature=0.5, multilingual=multilingual, without_timestamps=without_timestamps,
+            max_initial_timestamp=0.0)
+        info = TranscriptionInfo(language=language, language_probability=language_probability, duration=duration,
+                                 duration_after_vad=duration_after_vad, transcription_options=options,
+                                 vad_options=vad_parameters, all_language_probs=all_language_probs)
+        run = _ChunkRun(m, tokenizer, options, audio_chunks, metadata, features, clip_timestamps)
+        self.group_steps = []
+        return self._segments(run, batch_size), info
+
+    def _segments(self, run: _ChunkRun, batch_size: int):
+        """Reference :534-571, one ``TranscribeSession`` run per group; ids count on across groups."""
+        m = self.model
+        from . import vad as vad_mod
+        cap = int(getattr(m.model, "max_streams", 0) or 0)
+        group = max(1, min(batch_size, cap) if cap else batch_size)
+        free = getattr(m.model, "free_slots", None)
+        seg_idx = 0
+        for g0 in range(0, len(run.features), group):
+            run.refresh_resident()
+            run.jobs = [_ChunkJob(run, k) for k in range(g0, min(g0 + group, len(run.features)))]
+            sess = TranscribeSession(m)
+            for j in run.jobs:
+                sess.add_job(j)
+            while sess.pending():
+                if callable(free) and free() == 0:
+                    raise RuntimeError("no free encoder slot: release encoder outputs held elsewhere on this model")
+                sess.round()
+            for e in sess.entries:
+                if e.error is not None:
+                    raise e.error
+            self.group_steps.append([j.steps for j in run.jobs])
+            segs = [s for j in run.jobs for s in j.segments]
+            for s in segs:
+                seg_idx += 1
+                s.id = seg_idx
+            yield from restore_speech_timestamps(segs, run.clips, m.feature_extractor.sampling_rate, vad_mod)
