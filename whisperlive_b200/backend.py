@@ -91,13 +91,7 @@ if ServeClientBase is not None:
             try:
                 cls = ServeClientB200
                 if single_model:
-                    with cls.SINGLE_MODEL_LOCK:
-                        if cls.SINGLE_MODEL is None:
-                            cls.SINGLE_MODEL = self.create_model()
-                            cls.BATCH_WORKER = StreamScheduler(cls.SINGLE_MODEL, max_batch_size=cls.MAX_STREAMS,
-                                                               batch_window_ms=cls.BATCH_WINDOW_MS)
-                            cls.BATCH_WORKER.start()
-                    self.transcriber = cls.SINGLE_MODEL
+                    self.transcriber, _worker = cls.shared_model(self.create_model)
                 else:
                     self.registry = cls.model_registry()
                     self.model_entry = self.registry.acquire(self.model_size_or_path)
@@ -135,6 +129,18 @@ if ServeClientBase is not None:
                                                compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS, vad=vad)
             return B200WhisperModel(model_size_or_path, device="cuda", device_index=devices[0],
                                     compute_type=compute_type, max_streams=ServeClientB200.MAX_STREAMS, vad=vad)
+
+        @classmethod
+        def shared_model(cls, create):
+            """``(SINGLE_MODEL, BATCH_WORKER)``, the model every ``single_model=True`` connection shares and its
+            scheduler; ``create()`` builds the model on first use."""
+            with cls.SINGLE_MODEL_LOCK:
+                if cls.SINGLE_MODEL is None:
+                    cls.SINGLE_MODEL = create()
+                    cls.BATCH_WORKER = StreamScheduler(cls.SINGLE_MODEL, max_batch_size=cls.MAX_STREAMS,
+                                                       batch_window_ms=cls.BATCH_WINDOW_MS)
+                    cls.BATCH_WORKER.start()
+                return cls.SINGLE_MODEL, cls.BATCH_WORKER
 
         @classmethod
         def model_registry(cls) -> ModelRegistry:

@@ -192,6 +192,19 @@ class MultiDeviceSession:
                     out[loc[lo]] = segs
         return out
 
+    def settled(self, cursors: dict) -> dict:
+        """``TranscribeSession.settled`` on the device that owns each handle."""
+        out = {}
+        for g, loc in enumerate(self._locate(list(cursors))):
+            if loc:
+                for lo, segs in self.sessions[g].settled({lo: cursors[h] for lo, h in loc.items()}).items():
+                    out[loc[lo]] = segs
+        return out
+
+    def info(self, handle: int):
+        g, lo = next((g, lo) for g, loc in enumerate(self._locate([handle])) for lo in loc)
+        return self.sessions[g].info(lo)
+
     def cancel(self, handle: int) -> None:
         for g, loc in enumerate(self._locate([handle])):
             for lo in loc:

@@ -18,7 +18,9 @@ the drop-in schema a client thread fills in and waits on); the control flow is d
 * between step rounds the owner thread publishes interim segments for the requests that want them (one batched peek of
   the decode session) and drops cancelled requests, freeing their decode index and encoder slots;
 * speaker-embedding requests (``embed``, the device diarizer's) are answered at every round boundary, all that are
-  pending in one ``speaker_embeddings`` call, and right away when nothing is in flight.
+  pending in one ``speaker_embeddings`` call, and right away when nothing is in flight;
+* a request that wants its segments window by window (``want_segments``, the REST route's file jobs) gets the segments
+  that settled published after every round: host state only, no peek of the decode session.
 
 ``linger_ms`` (default 0) optionally waits for more requests when the engine is idle and a single request arrived --
 the latency / batching trade the reference hard-codes as its 50 ms window.
@@ -35,6 +37,8 @@ from typing import Any, Deque, Dict, List, Optional
 import numpy as np
 
 log = logging.getLogger("whisperlive_b200.scheduler")
+
+EMBED_CALL_SAMPLES = 30 * 16000     # per stream of capacity: one 30 s segment each, the first wl_spk_embed workspace
 
 
 class RequestCancelled(RuntimeError):
@@ -68,11 +72,38 @@ class Partial:
             return self.version, list(self.segments)
 
 
+class Settled:
+    """The segments of a request's settled windows, appended by the owner thread as windows settle; ``event`` is set on
+    each append and when the request finishes."""
+
+    def __init__(self):
+        self._lock = threading.Lock()
+        self._segments: List[Any] = []
+        self.event = threading.Event()
+
+    def __len__(self) -> int:
+        with self._lock:
+            return len(self._segments)
+
+    def extend(self, segments: List[Any]) -> None:
+        with self._lock:
+            self._segments.extend(segments)
+        self.event.set()
+
+    def since(self, n: int) -> List[Any]:
+        """The segments after the first ``n``."""
+        with self._lock:
+            return self._segments[n:]
+
+
 @dataclass
 class BatchRequest:
     """What a client thread submits and waits on (same fields as the reference's request record,
     whisper_live/batch_inference.py:51-84, so ``ServeClient*`` code can fill either).  ``want_partials``: publish interim
-    segments in ``partial`` after each step round; ``cancel()``: nobody waits for the result any more."""
+    segments in ``partial`` after each step round; ``cancel()``: nobody waits for the result any more.
+    ``temperature``: the ladder (a float is a one-rung ladder); None keeps the transcriber's default.  ``want_segments``:
+    append the segments of each window that settles to ``settled``, after the round it settled in.  ``admitted`` is set once the request is in the
+    session, with ``info`` (language resolved) -- or once it failed or was cancelled before that."""
     audio: np.ndarray
     language: Optional[str] = None
     task: str = "transcribe"
@@ -91,6 +122,10 @@ class BatchRequest:
     want_partials: bool = False
     partial: Partial = field(default_factory=Partial)
     cancelled: bool = False
+    temperature: Optional[Any] = None
+    want_segments: bool = False
+    settled: Settled = field(default_factory=Settled)
+    admitted: threading.Event = field(default_factory=threading.Event)
 
     def cancel(self) -> None:
         """The scheduler drops this request at its next round boundary (its decode index and encoder slots go back) and
@@ -98,9 +133,12 @@ class BatchRequest:
         self.cancelled = True
 
     def kwargs(self) -> dict:
-        return dict(language=self.language, task=self.task, initial_prompt=self.initial_prompt, vad_filter=self.use_vad,
-                    vad_parameters=self.vad_parameters if self.use_vad else None, hotwords=self.hotwords,
-                    word_timestamps=self.word_timestamps)
+        kw = dict(language=self.language, task=self.task, initial_prompt=self.initial_prompt, vad_filter=self.use_vad,
+                  vad_parameters=self.vad_parameters if self.use_vad else None, hotwords=self.hotwords,
+                  word_timestamps=self.word_timestamps)
+        if self.temperature is not None:
+            kw["temperature"] = self.temperature
+        return kw
 
 
 class EmbeddingRequest:
@@ -155,11 +193,15 @@ class RoundScheduler:
     def embed(self, audio: np.ndarray) -> EmbeddingRequest:
         """Queue one segment for a speaker embedding; the owner thread answers it with every other pending one at the
         next round boundary, or at once when the engine is idle."""
-        request = EmbeddingRequest(np.asarray(audio, dtype=np.float32).reshape(-1))
+        return self.embed_many([audio])[0]
+
+    def embed_many(self, audios) -> List[EmbeddingRequest]:
+        """Queue several segments at once: they are answered together, by one ``speaker_embeddings`` call."""
+        requests = [EmbeddingRequest(np.asarray(a, dtype=np.float32).reshape(-1)) for a in audios]
         with self._cv:
-            self._embeds.append(request)
+            self._embeds.extend(requests)
             self._cv.notify()
-        return request
+        return requests
 
     def start(self) -> None:
         self._thread = threading.Thread(target=self._owner_loop, daemon=True, name="wlb200-rounds")
@@ -216,6 +258,8 @@ class RoundScheduler:
                     log.error("admission failed: %s", e)
                     for r in new:
                         self._finish(r, None, None, e)
+                else:
+                    self._announce_admitted(session, zip(handles, new))
             self._answer_embeddings()
             self.max_in_flight = max(self.max_in_flight, len(in_flight))
             self._drop_cancelled(session, in_flight)
@@ -246,13 +290,37 @@ class RoundScheduler:
                     self._finish(r, None, None, e)
             if step:
                 self._publish_partials(session, in_flight)
+            self._publish_settled(session, in_flight)
+
+    def _announce_admitted(self, session, admitted) -> None:
+        """``info`` (language resolved) for the admitted requests that want segments, then their ``admitted`` event.  A
+        failing ``info`` leaves ``info`` unset; the stream keeps decoding and its result carries the info."""
+        for h, r in admitted:
+            if r.want_segments:
+                try:
+                    r.info = session.info(h)
+                except Exception as e:
+                    log.error("info of an admitted request failed: %s", e)
+            r.admitted.set()
 
     def _answer_embeddings(self) -> None:
-        """Every pending embedding request in one ``speaker_embeddings`` call; an error fails only these requests."""
+        """Every pending embedding request, in calls of at most ``capacity`` x 30 s of audio -- the workspace
+        ``footprint_estimate`` budgets for the speaker embedding -- so a long file's segments cannot grow it further
+        (a longer segment goes alone); an error fails only the requests of its call."""
         with self._cv:
             batch, self._embeds = self._embeds, []
-        if not batch:
-            return
+        limit = self.capacity * EMBED_CALL_SAMPLES
+        group, samples = [], 0
+        for r in batch:
+            if group and samples + len(r.audio) > limit:
+                self._embed_call(group)
+                group, samples = [], 0
+            group.append(r)
+            samples += len(r.audio)
+        if group:
+            self._embed_call(group)
+
+    def _embed_call(self, batch: List[EmbeddingRequest]) -> None:
         try:
             out = self.transcriber.speaker_embeddings([r.audio for r in batch])
             self.embedding_calls += 1
@@ -288,6 +356,20 @@ class RoundScheduler:
         for h, segs in got.items():
             in_flight[h].partial.publish(segs)
 
+    def _publish_settled(self, session, in_flight: Dict[int, BatchRequest]) -> None:
+        """Append the newly settled segments of the in-flight requests that want them (host state of the session, read
+        past each request's cursor only); an error here loses interim segments, never the final result."""
+        want = {h: len(r.settled) for h, r in in_flight.items() if r.want_segments and not r.cancelled}
+        if not want:
+            return
+        try:
+            got = session.settled(want)
+        except Exception as e:
+            log.error("settled segments failed: %s", e)
+            return
+        for h, segs in got.items():
+            in_flight[h].settled.extend(segs)
+
     def _finish(self, r: BatchRequest, segments, info, error) -> None:
         r.result = list(segments) if segments is not None else None
         r.info = info
@@ -296,6 +378,8 @@ class RoundScheduler:
         self.streams_done += 1
         r.future.set()
         r.partial.event.set()
+        r.settled.event.set()
+        r.admitted.set()
 
 
 class _OneShotSession:
@@ -332,6 +416,12 @@ class _OneShotSession:
     def pop_finished(self):
         d, self._done = self._done, []
         return d
+
+    def info(self, handle):
+        return None                 # known once the call returns
+
+    def settled(self, cursors):
+        return {}
 
     def result_of(self, entry):
         if entry.error is not None:

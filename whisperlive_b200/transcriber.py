@@ -609,10 +609,39 @@ class TranscribeSession:
             return (segs, None)
         if p["speech_chunks"]:
             segs = restore_speech_timestamps(segs, p["speech_chunks"], m.feature_extractor.sampling_rate, m._vad)
-        info = TranscriptionInfo(language=p["language"], language_probability=p["language_probability"], duration=p["duration"],
+        return (segs, self._info(p))
+
+    @staticmethod
+    def _info(p: dict) -> TranscriptionInfo:
+        return TranscriptionInfo(language=p["language"], language_probability=p["language_probability"], duration=p["duration"],
                                  duration_after_vad=p["duration_after_vad"], transcription_options=p["options"],
                                  vad_options=p["vad_parameters"], all_language_probs=p["all_language_probs"])
-        return (segs, info)
+
+    def info(self, handle: int) -> Optional[TranscriptionInfo]:
+        """The ``TranscriptionInfo`` of an admitted stream (its language is resolved at admission); None for a stream
+        that VAD left empty."""
+        e = next(x for x in self.entries if x.handle == handle)
+        return None if e.job is None or e.prepared is None else self._info(e.prepared)
+
+    def settled(self, cursors: Dict[int, int]) -> Dict[int, List[Segment]]:
+        """``handle -> cursor``: the segments each live stream settled past its cursor (streams with none are left
+        out).  Copies, with the timestamps of the final result; host state only, no device call.  A settled segment
+        does not change afterwards, so a caller that advances its cursor reads each one once."""
+        out = {}
+        for e in self.entries:
+            n = cursors.get(e.handle)
+            if n is not None and e.job is not None and len(e.job.segments) > n:
+                out[e.handle] = self._settled_copy(e, e.job.segments[n:])
+        return out
+
+    def _settled_copy(self, e: _Entry, segments: List[Segment]) -> List[Segment]:
+        # copies down to the words: restore_speech_timestamps maps them in place, and result_of maps the stream's own
+        # segments and words once, when it finishes
+        segs = [replace(s, words=None if s.words is None else [replace(w) for w in s.words]) for s in segments]
+        p = e.prepared
+        if p is not None and p.get("speech_chunks"):
+            segs = restore_speech_timestamps(segs, p["speech_chunks"], self.m.feature_extractor.sampling_rate, self.m._vad)
+        return segs
 
     def pending(self) -> int:
         return sum(1 for e in self.entries if e.state != "done")
