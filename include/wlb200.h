@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 11
+#define WL_ABI_VERSION 12
 
 typedef struct wl_ctx wl_ctx;
 
@@ -91,6 +91,18 @@ int wl_mem_info(int32_t device, int64_t* free_bytes, int64_t* total_bytes);
 /* Weights: float32 host tensors under HF WhisperForConditionalGeneration names
  * ("model.encoder.conv1.weight", ...), plus "mel_filters" [n_mels, 201]. */
 int wl_load_tensor(wl_ctx* ctx, const char* name, const float* data, const int64_t* shape, int32_t ndim);
+/* The same upload from the bytes as a checkpoint stores them (ABI 12): data is `dtype` (WL_DT_*).  For WL_DT_I8,
+ * scale holds one value per leading-dimension row, of type scale_dtype (F32, F16 or BF16), and the weight is
+ * (float)q / scale[row]; scale is ignored otherwise.  The device keeps exactly what wl_load_tensor keeps for the same
+ * values (fp32 vectors, encoder position table and mel filters; fp16 with the conv re-layout for the rest), rounded
+ * with __float2half_rn.  A finite value that would become +-inf in fp16 fails the call with WL_ERR_ARG, naming the
+ * tensor and the count; nothing of that tensor stays on the device. */
+#define WL_DT_F32 0
+#define WL_DT_F16 1
+#define WL_DT_BF16 2
+#define WL_DT_I8 3
+int wl_load_tensor_typed(wl_ctx* ctx, const char* name, const void* data, int32_t dtype, const int64_t* shape, int32_t ndim,
+                         const void* scale, int32_t scale_dtype);
 int wl_finalize_weights(wl_ctx* ctx);
 
 /* K1. pcm: B waveforms concatenated, offsets[B+1] in samples.  out: per stream [n_mels, n_b/160 + 1]
@@ -247,6 +259,9 @@ int wl_test_enc_attn(wl_ctx* ctx, const uint16_t* qk_f16, const uint16_t* vt_f16
 /* The conv stem with the loaded conv weights, biases and positional table: feats [nb][n_mels][3000] f32 -> x_out
  * [nb][1500][d] f32, the residual stream after conv2 + GELU + positions. */
 int wl_test_enc_stem(wl_ctx* ctx, const float* feats_f32, float* x_out_f32, int32_t nb);
+/* A tensor uploaded by wl_load_tensor / wl_load_tensor_typed as the device holds it, before wl_finalize_weights: fp32
+ * (vectors, encoder position table, mel filters) or fp16 bits after the conv re-layout, into out. */
+int wl_test_read_weight(wl_ctx* ctx, const char* name, void* out);
 /* layernorm_rows over x [rows][d] (d a multiple of 4, at most 1280).  y16_as_f32 (the fp16 output as float) and y32
  * (the fp32 output), either may be NULL: [rows + 8][d], uploaded as the caller filled them (y16 rounded to fp16) and
  * copied back whole, so the 8 guard rows after the last one show what the kernel wrote past it. */

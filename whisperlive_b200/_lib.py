@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 11
+ABI_VERSION = 12
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -75,6 +75,8 @@ SIGNATURES = {
     "wl_device_bytes": (C.c_int, [C.c_void_p, c_i64p]),
     "wl_mem_info": (C.c_int, [C.c_int32, c_i64p, c_i64p]),
     "wl_load_tensor": (C.c_int, [C.c_void_p, C.c_char_p, c_f32p, c_i64p, C.c_int32]),
+    "wl_load_tensor_typed": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int32, c_i64p, C.c_int32, C.c_void_p,
+                                       C.c_int32]),
     "wl_finalize_weights": (C.c_int, [C.c_void_p]),
     "wl_mel": (C.c_int, [C.c_void_p, c_f32p, c_i64p, C.c_int32, c_f32p, c_i64p]),
     "wl_encode": (C.c_int, [C.c_void_p, c_f32p, C.c_int32, c_i32p]),
@@ -109,6 +111,7 @@ SIGNATURES = {
                                C.c_int32, C.c_int32]),
     "wl_test_enc_attn": (C.c_int, [C.c_void_p, c_u16p, c_u16p, c_u16p, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "wl_test_enc_stem": (C.c_int, [C.c_void_p, c_f32p, c_f32p, C.c_int32]),
+    "wl_test_read_weight": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p]),
     "wl_test_layernorm": (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_int32, C.c_int32]),
     "wl_test_search": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, C.POINTER(WlGenOpts), C.POINTER(WlSearchScript),
                                  c_i32p, c_i32p, c_f32p, c_f32p, c_i32p, c_i32p, c_f32p]),

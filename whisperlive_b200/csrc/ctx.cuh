@@ -261,6 +261,8 @@ struct wl_ctx {
   } spk;
   float* stage_f32 = nullptr;   // wl_load_tensor staging (freed by wl_finalize_weights)
   long stage_cap = 0;
+  unsigned char* stage_bytes = nullptr;   // wl_load_tensor_typed staging: overflow count, payload, scales (freed likewise)
+  long stage_bytes_cap = 0;
   // Decode session (N2, step-level continuous batching): a second decode state + self-attention cache whose stream
   // indices are admitted, decoded for a bounded number of token steps and collected independently of each other.
   // One-shot calls (wl_generate / wl_align / wl_detect_language) keep using `ds` / `kcache`, so they may run between two

@@ -1,6 +1,8 @@
 // Row-wise helper kernels: feature layout prep, LayerNorm, softmax, decoder token embedding.
 #include <algorithm>
 
+#include <cuda_bf16.h>
+
 #include "kernels.cuh"
 
 namespace wl {
@@ -21,6 +23,91 @@ void cast_weight_f16(cudaStream_t st, const float* in, __half* out, long a, long
   const int grid = (int)std::min<long>((n + 255) / 256, 132L * 16);
   cast_weight_kernel<<<grid, 256, 0, st>>>(in, out, n, b, k);
   WL_CUDA(cudaGetLastError());
+}
+
+// ---------------------------------------------------------------------------- convert_weight (typed upload)
+// One 16-byte load per thread and iteration: V source values.  Value j of the source becomes fp32 exactly (fp16 and
+// bf16 widen exactly, int8 is (float)q / scale[row] with IEEE division), then __float2half_rn for fp16 targets.  The
+// write goes to the relayout index of cast_weight_kernel ([a][b][k] -> [a][k][b]; b = k = 1 is the identity).
+__device__ __forceinline__ float widen(float x) { return x; }
+__device__ __forceinline__ float widen(__half x) { return __half2float(x); }
+__device__ __forceinline__ float widen(__nv_bfloat16 x) { return __bfloat162float(x); }
+
+__device__ __forceinline__ float load_scale(const void* s, int dt, long row) {
+  if (dt == WDT_F16) return __half2float(((const __half*)s)[row]);
+  if (dt == WDT_BF16) return __bfloat162float(((const __nv_bfloat16*)s)[row]);
+  return ((const float*)s)[row];
+}
+
+template <class S>
+__device__ __forceinline__ float src_value(S x, const void*, int, long) { return widen(x); }
+template <>
+__device__ __forceinline__ float src_value<int8_t>(int8_t q, const void* scale, int sdt, long row) {
+  return __fdiv_rn((float)q, load_scale(scale, sdt, row));
+}
+
+__device__ __forceinline__ void store_out(float* out, long i, float v, int&) { out[i] = v; }
+__device__ __forceinline__ void store_out(__half* out, long i, float v, int& bad) {
+  const __half h = __float2half_rn(v);
+  bad += __hisinf(h) && !isinf(v);   // a finite value beyond the fp16 range
+  out[i] = h;
+}
+
+template <class S, class O>
+__global__ void __launch_bounds__(256) convert_weight_kernel(const S* __restrict__ in, const void* __restrict__ scale, int sdt,
+                                                             O* __restrict__ out, long n, long cols, long b, long k,
+                                                             int* __restrict__ overflow) {
+  constexpr int V = 16 / sizeof(S);
+  const long stride = (long)gridDim.x * blockDim.x, nvec = n / V;
+  const bool plain = b == 1 && k == 1;
+  int bad = 0;
+  for (long v = blockIdx.x * (long)blockDim.x + threadIdx.x; v < nvec; v += stride) {
+    union { uint4 u; S s[V]; } x;
+    x.u = __ldg(reinterpret_cast<const uint4*>(in) + v);
+#pragma unroll
+    for (int j = 0; j < V; ++j) {
+      const long i = v * V + j;   // source index (a, bb, kk)
+      const float f = src_value<S>(x.s[j], scale, sdt, i / cols);
+      long o = i;
+      if (!plain) {
+        const long kk = i % k, bb = (i / k) % b, a = i / (b * k);
+        o = (a * k + kk) * b + bb;
+      }
+      store_out(out, o, f, bad);
+    }
+  }
+  // the ragged tail, fewer than V values
+  for (long i = nvec * V + blockIdx.x * (long)blockDim.x + threadIdx.x; i < n; i += stride) {
+    const float f = src_value<S>(in[i], scale, sdt, i / cols);
+    long o = i;
+    if (!plain) {
+      const long kk = i % k, bb = (i / k) % b, a = i / (b * k);
+      o = (a * k + kk) * b + bb;
+    }
+    store_out(out, o, f, bad);
+  }
+  if (bad) atomicAdd(overflow, bad);
+}
+
+template <class O>
+static void convert_weight_t(cudaStream_t st, const void* in, int dt, const void* scale, int sdt, O* out, long a, long b, long k,
+                             long cols, int* overflow, int num_sms) {
+  const long n = a * b * k;
+  const int V = dt == WDT_F32 ? 4 : dt == WDT_I8 ? 16 : 8;
+  const int grid = (int)std::max<long>(1, std::min<long>((n / V + 255) / 256, (long)num_sms * 8));
+  if (dt == WDT_F32) convert_weight_kernel<<<grid, 256, 0, st>>>((const float*)in, scale, sdt, out, n, cols, b, k, overflow);
+  else if (dt == WDT_F16) convert_weight_kernel<<<grid, 256, 0, st>>>((const __half*)in, scale, sdt, out, n, cols, b, k, overflow);
+  else if (dt == WDT_BF16) convert_weight_kernel<<<grid, 256, 0, st>>>((const __nv_bfloat16*)in, scale, sdt, out, n, cols, b, k, overflow);
+  else convert_weight_kernel<<<grid, 256, 0, st>>>((const int8_t*)in, scale, sdt, out, n, cols, b, k, overflow);
+  WL_CUDA(cudaGetLastError());
+}
+void convert_weight_f16(cudaStream_t st, const void* in, int dt, const void* scale, int sdt, __half* out, long a, long b, long k,
+                        long cols, int* overflow, int num_sms) {
+  convert_weight_t(st, in, dt, scale, sdt, out, a, b, k, cols, overflow, num_sms);
+}
+void convert_weight_f32(cudaStream_t st, const void* in, int dt, const void* scale, int sdt, float* out, long n, long cols,
+                        int* overflow, int num_sms) {
+  convert_weight_t(st, in, dt, scale, sdt, out, n, 1, 1, cols, overflow, num_sms);
 }
 
 // ---------------------------------------------------------------------------- gather_windows

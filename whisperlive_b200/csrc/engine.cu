@@ -225,6 +225,63 @@ extern "C" int wl_load_tensor(wl_ctx* c, const char* name, const float* data, co
   API_END(c)
 }
 
+static_assert(WL_DT_F32 == WDT_F32 && WL_DT_F16 == WDT_F16 && WL_DT_BF16 == WDT_BF16 && WL_DT_I8 == WDT_I8,
+              "wlb200.h and kernels.cuh disagree on the weight dtypes");
+
+// The bytes go to the device as stored (half the PCIe traffic of wl_load_tensor for an fp16 checkpoint, a quarter
+// for int8) and are converted there.  One byte staging buffer holds [overflow count | payload | scales], each part
+// 256-byte aligned so the conversion kernels read it 16 bytes at a time.
+extern "C" int wl_load_tensor_typed(wl_ctx* c, const char* name, const void* data, int32_t dtype, const int64_t* shape,
+                                    int32_t ndim, const void* scale, int32_t scale_dtype) {
+  API_BEGIN(c)
+  WL_CHECK(name && data && shape && ndim >= 1 && ndim <= 3, WL_ERR_ARG, "wl_load_tensor_typed: bad arguments");
+  WL_CHECK(dtype >= WL_DT_F32 && dtype <= WL_DT_I8, WL_ERR_ARG, "wl_load_tensor_typed(%s): unknown dtype %d", name, dtype);
+  WL_CHECK(dtype != WL_DT_I8 || (scale && scale_dtype >= WL_DT_F32 && scale_dtype <= WL_DT_BF16), WL_ERR_ARG,
+           "wl_load_tensor_typed(%s): int8 needs a float32 / float16 / bfloat16 scale per row", name);
+  WL_CHECK(!c->finalized, WL_ERR_STATE, "weights already finalized");
+  std::string nm(name);
+  size_t n = 1;
+  std::vector<int64_t> sh(shape, shape + ndim);
+  for (auto s : sh) {
+    WL_CHECK(s > 0, WL_ERR_ARG, "wl_load_tensor_typed(%s): empty dimension", name);
+    n *= (size_t)s;
+  }
+  static const size_t esize[4] = {4, 2, 2, 1};
+  const size_t rows = (size_t)sh[0], cols = n / rows;
+  const size_t pay = esize[dtype] * n, sc = dtype == WL_DT_I8 ? esize[scale_dtype] * rows : 0;
+  auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+  const size_t off_data = 256, off_scale = off_data + up(pay), total = off_scale + up(sc);
+  c->mem.grow(c->stage_bytes, c->stage_bytes_cap, (long)total);
+  unsigned char* s = c->stage_bytes;
+  int* overflow = (int*)s;
+  WL_CUDA(cudaMemsetAsync(overflow, 0, sizeof(int), c->st));
+  WL_CUDA(cudaMemcpyAsync(s + off_data, data, pay, cudaMemcpyHostToDevice, c->st));
+  if (sc) WL_CUDA(cudaMemcpyAsync(s + off_scale, scale, sc, cudaMemcpyHostToDevice, c->st));
+  const void* dscale = sc ? (const void*)(s + off_scale) : nullptr;
+  const bool as_f32 = ndim == 1 || nm == "model.encoder.embed_positions.weight" || nm == "mel_filters";
+  void* p;
+  if (as_f32) {
+    float* q = c->mem.alloc<float>(n, false);
+    convert_weight_f32(c->st, s + off_data, dtype, dscale, scale_dtype, q, (long)n, (long)cols, overflow, c->num_sms);
+    p = q;
+  } else {
+    __half* q = c->mem.alloc<__half>(n, false);
+    if (ndim == 3) convert_weight_f16(c->st, s + off_data, dtype, dscale, scale_dtype, q, sh[0], sh[1], sh[2], (long)cols, overflow, c->num_sms);
+    else convert_weight_f16(c->st, s + off_data, dtype, dscale, scale_dtype, q, (long)n, 1, 1, (long)cols, overflow, c->num_sms);
+    p = q;
+  }
+  int n_over = 0;
+  WL_CUDA(cudaMemcpyAsync(&n_over, overflow, sizeof(int), cudaMemcpyDeviceToHost, c->st));
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  if (n_over) {
+    c->mem.release(p);
+    WL_CHECK(false, WL_ERR_ARG, "weight '%s': %d finite values exceed the float16 range (|x| > 65504)", name, n_over);
+  }
+  c->dev[nm] = p;
+  c->shape[nm] = sh;
+  API_END(c)
+}
+
 static void* need(wl_ctx* c, const std::string& nm, std::initializer_list<int64_t> want) {
   auto it = c->dev.find(nm);
   WL_CHECK(it != c->dev.end(), WL_ERR_STATE, "missing weight tensor '%s'", nm.c_str());
@@ -303,6 +360,8 @@ extern "C" int wl_finalize_weights(wl_ctx* c) {
   WL_CHECK(!c->finalized, WL_ERR_STATE, "weights already finalized");
   c->mem.release(c->stage_f32);
   c->stage_cap = 0;
+  c->mem.release(c->stage_bytes);
+  c->stage_bytes_cap = 0;
   const size_t mark = c->mem.list.size();
   try {
     finalize_impl(c);

@@ -288,6 +288,23 @@ extern "C" int wl_test_layernorm(wl_ctx* c, const float* x_f32, const float* gam
   API_END(c)
 }
 
+// A tensor wl_load_tensor / wl_load_tensor_typed uploaded, as the device holds it (fp32 or fp16 bytes, after the conv
+// re-layout), before wl_finalize_weights.
+extern "C" int wl_test_read_weight(wl_ctx* c, const char* name, void* out) {
+  API_BEGIN(c)
+  WL_CHECK(name && out, WL_ERR_ARG, "wl_test_read_weight: bad arguments");
+  const std::string nm(name);
+  auto it = c->dev.find(nm);
+  WL_CHECK(it != c->dev.end(), WL_ERR_ARG, "wl_test_read_weight: no weight '%s'", name);
+  const auto& sh = c->shape[nm];
+  size_t n = 1;
+  for (auto s : sh) n *= (size_t)s;
+  const bool as_f32 = sh.size() == 1 || nm == "model.encoder.embed_positions.weight" || nm == "mel_filters";
+  WL_CUDA(cudaStreamSynchronize(c->st));
+  WL_CUDA(cudaMemcpy(out, it->second, n * (as_f32 ? sizeof(float) : sizeof(__half)), cudaMemcpyDeviceToHost));
+  API_END(c)
+}
+
 extern "C" int wl_bench_gemm(wl_ctx* c, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,
                              float* ms_out) {
   // flags: 1 transposed (swap-AB) store, 2 bias, 4 GELU, 8 fp32 output with fp32 residual (in place), 16 bias on m,

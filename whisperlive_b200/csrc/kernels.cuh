@@ -78,6 +78,15 @@ struct PartialSrc {
 void prep_features(cudaStream_t st, const float* feats, __half* out, int B, int n_mels);
 // weight upload: fp32 [a][b][k] -> fp16 [a][k][b] (conv kernels; b = k = 1 is a plain cast)
 void cast_weight_f16(cudaStream_t st, const float* in, __half* out, long a, long b, long k);
+// typed weight upload (wl_load_tensor_typed): source element types, the WL_DT_* values of wlb200.h
+enum WeightDtype { WDT_F32 = 0, WDT_F16 = 1, WDT_BF16 = 2, WDT_I8 = 3 };
+// source of type dt [a][b][k] -> fp16 [a][k][b]; int8 sources are divided by scale[i / cols] (scale of type sdt).
+// Finite values that round to +-inf in fp16 are added to *overflow.  `in` must be 16-byte aligned.
+void convert_weight_f16(cudaStream_t st, const void* in, int dt, const void* scale, int sdt, __half* out, long a, long b, long k,
+                        long cols, int* overflow, int num_sms);
+// the same to fp32, no relayout (vectors, the encoder position table, the mel filters)
+void convert_weight_f32(cudaStream_t st, const void* in, int dt, const void* scale, int sdt, float* out, long n, long cols,
+                        int* overflow, int num_sms);
 // window gather from the resident log-mel of wl_mel_device: feat[w][m][t] = t < len[w] ? mel[off[stream[w]] + m * frames[stream[w]] + seek[w] + t] : 0
 // (the reference slices features[:, seek : seek + segment_size] and zero-pads to 3000 frames on the host: transcriber_faster_whisper.py:1115-1127)
 void gather_windows(cudaStream_t st, const float* mel, const long* mel_off, const int* frames, const int* win_stream, const int* win_seek,

@@ -21,7 +21,7 @@ from __future__ import annotations
 import json
 import os
 import struct
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, Iterator, List, NamedTuple, Optional, Tuple
 
 import numpy as np
 import torch
@@ -48,36 +48,54 @@ def _write_str(f, s: str) -> None:
     f.write(b"\0")
 
 
-def read_variables(path: str) -> Tuple[Dict[str, np.ndarray], Dict[str, str], Dict[str, object]]:
-    """Return (variables, aliases, header) of a CTranslate2 model.bin.  bfloat16 payloads come back as float32."""
-    variables: Dict[str, np.ndarray] = {}
+class VarInfo(NamedTuple):
+    """A variable of a model.bin as its header describes it: where its payload lies in the file."""
+    shape: Tuple[int, ...]
+    dtype_id: int
+    offset: int
+    n_bytes: int
+
+
+_ITEMSIZE = {0: 4, 1: 1, 2: 2, 3: 4, 4: 2, 5: 2}
+
+
+def read_variables(path: str, header_only: bool = False):
+    """Return (variables, aliases, header) of a CTranslate2 model.bin.  bfloat16 payloads come back as float32.
+    ``header_only``: the variables are ``VarInfo`` records and the payloads are skipped with a seek, so the table of a
+    multi-gigabyte file is read in a few kilobytes."""
+    variables: Dict[str, object] = {}
     with open(path, "rb") as f:
         (version,) = struct.unpack("<I", f.read(4))
         if version != BINARY_VERSION:
             raise ValueError(f"model.bin: binary version {version}, this reader understands {BINARY_VERSION} only")
         spec = _read_str(f)
         revision, n_var = struct.unpack("<II", f.read(8))
+        size = os.fstat(f.fileno()).st_size
         for _ in range(n_var):
             name = _read_str(f)
             (rank,) = struct.unpack("<B", f.read(1))
             shape = struct.unpack(f"<{rank}I", f.read(4 * rank)) if rank else ()
             dtype_id, n_bytes = struct.unpack("<BI", f.read(5))
+            if dtype_id not in _ITEMSIZE:
+                raise ValueError(f"model.bin: variable {name!r} has unknown dtype id {dtype_id}")
+            count = int(np.prod(shape)) if rank else 1
+            if n_bytes != _ITEMSIZE[dtype_id] * count:
+                raise ValueError(f"model.bin: variable {name!r}: {n_bytes} bytes for {count} values of dtype id {dtype_id}")
+            if header_only:
+                offset = f.tell()
+                if offset + n_bytes > size:
+                    raise ValueError(f"model.bin: variable {name!r} truncated")
+                f.seek(n_bytes, os.SEEK_CUR)
+                variables[name] = VarInfo(tuple(shape), dtype_id, offset, n_bytes)
+                continue
             raw = f.read(n_bytes)
             if len(raw) != n_bytes:
                 raise ValueError(f"model.bin: variable {name!r} truncated")
-            count = int(np.prod(shape)) if rank else 1
             if dtype_id == _BF16:
-                if n_bytes != 2 * count:
-                    raise ValueError(f"model.bin: variable {name!r}: {n_bytes} bytes for {count} bfloat16 values")
                 u = np.frombuffer(raw, dtype=np.uint16).astype(np.uint32) << 16
                 arr = u.view(np.float32).reshape(shape)
-            elif dtype_id in _DTYPES:
-                dt = np.dtype(_DTYPES[dtype_id])
-                if n_bytes != dt.itemsize * count:
-                    raise ValueError(f"model.bin: variable {name!r}: {n_bytes} bytes for {count} x {dt}")
-                arr = np.frombuffer(raw, dtype=dt).reshape(shape).copy()
             else:
-                raise ValueError(f"model.bin: variable {name!r} has unknown dtype id {dtype_id}")
+                arr = np.frombuffer(raw, dtype=np.dtype(_DTYPES[dtype_id])).reshape(shape).copy()
             variables[name] = arr
         aliases: Dict[str, str] = {}
         tail = f.read(4)
@@ -102,13 +120,14 @@ def write_variables(path: str, variables: Dict[str, np.ndarray], aliases: Option
         f.write(struct.pack("<II", revision, len(variables)))
         for name in sorted(variables):
             arr = np.ascontiguousarray(variables[name])
-            if arr.dtype not in _DTYPE_IDS:
+            if arr.dtype not in _DTYPE_IDS and arr.dtype != np.uint16:
                 raise ValueError(f"cannot serialise {name!r} of dtype {arr.dtype}")
             _write_str(f, name)
             f.write(struct.pack("<B", arr.ndim))
             for d in arr.shape:
                 f.write(struct.pack("<I", d))
-            f.write(struct.pack("<BI", _DTYPE_IDS[arr.dtype], arr.nbytes))
+            # bfloat16 variables are handed over as their uint16 bit patterns (numpy has no bfloat16)
+            f.write(struct.pack("<BI", _BF16 if arr.dtype == np.uint16 else _DTYPE_IDS[arr.dtype], arr.nbytes))
             f.write(arr.tobytes())
         aliases = aliases or {}
         f.write(struct.pack("<I", len(aliases)))
@@ -118,85 +137,161 @@ def write_variables(path: str, variables: Dict[str, np.ndarray], aliases: Option
 
 
 # ------------------------------------------------------------------------------------------ name mapping
-def _f32(a: np.ndarray) -> torch.Tensor:
-    return torch.from_numpy(np.ascontiguousarray(a, dtype=np.float32))
+# Dequantization, a recalled upstream rule (ctranslate2 4.x ``specs/model_spec.py``, the ``int8*`` branch of the
+# quantization step, restated from memory; tests/golden/capture_ct2_convert.py records real conversions to check it):
+# a ``.../weight`` matrix W is stored as int8 ``q = round(W[r] * scale[r])`` with ``scale[r] = 127 / amax(|W[r]|)``
+# (an all-zero row gets ``amax = 127``) and its scales as the sibling variable ``.../weight_scale``, one per row.
+# CTranslate2 computes with ``W[r] = q / scale[r]``; loading at compute_type float16 rounds that value to fp16.
+# ``int16`` files (``scale`` a single 2^k) are not read: the engine has no use for them and they are rare.
+
+# Each canonical tensor is rows [r0, r1) of one CT2 variable (None: all rows): CT2 fuses the attention projections --
+# self-attention linear_0 = [q; k; v], linear_1 = out; cross-attention linear_0 = q, linear_1 = [k; v],
+# linear_2 = out.  Whisper's k_proj has no bias (CT2 stores zeros in its slice).
+Plan = List[Tuple[str, str, Optional[Tuple[int, int]]]]
 
 
-def _attention_to_hf(get, src: str, dst: str, out: Dict[str, torch.Tensor], cross: bool) -> None:
-    """CT2 fuses the projections: self-attention linear_0 = [q; k; v], linear_1 = out; cross-attention linear_0 = q,
-    linear_1 = [k; v], linear_2 = out.  Whisper's k_proj has no bias (CT2 stores zeros in its slice)."""
-    if cross:
-        wq, bq = get(f"{src}/linear_0/weight"), get(f"{src}/linear_0/bias")
-        wkv, bkv = get(f"{src}/linear_1/weight"), get(f"{src}/linear_1/bias")
-        d = wq.shape[0]
-        wk, wv, bv = wkv[:d], wkv[d:], bkv[d:]
-        wo, bo = get(f"{src}/linear_2/weight"), get(f"{src}/linear_2/bias")
-    else:
-        w, b = get(f"{src}/linear_0/weight"), get(f"{src}/linear_0/bias")
-        d = w.shape[0] // 3
-        wq, wk, wv = w[:d], w[d:2 * d], w[2 * d:]
-        bq, bv = b[:d], b[2 * d:]
-        wo, bo = get(f"{src}/linear_1/weight"), get(f"{src}/linear_1/bias")
-    out[f"{dst}.q_proj.weight"], out[f"{dst}.q_proj.bias"] = _f32(wq), _f32(bq)
-    out[f"{dst}.k_proj.weight"] = _f32(wk)
-    out[f"{dst}.v_proj.weight"], out[f"{dst}.v_proj.bias"] = _f32(wv), _f32(bv)
-    out[f"{dst}.out_proj.weight"], out[f"{dst}.out_proj.bias"] = _f32(wo), _f32(bo)
+def ct2_plan(shapes: Dict[str, Tuple[int, ...]], aliases: Optional[Dict[str, str]] = None) -> Plan:
+    """(canonical HF name, CT2 variable, row range) for every tensor the engine reads, from the variable table alone."""
+    aliases = aliases or {}
+    plan: Plan = []
 
-
-def _norm_to_hf(get, src: str, dst: str, out: Dict[str, torch.Tensor]) -> None:
-    out[f"{dst}.weight"], out[f"{dst}.bias"] = _f32(get(f"{src}/gamma")), _f32(get(f"{src}/beta"))
-
-
-def load_ct2_model_bin(path: str) -> Dict[str, torch.Tensor]:
-    """``model.bin`` (or its directory) -> the canonical HF-named fp32 dict the engine uploads (weights.load_safetensors
-    produces the same key space).  int8 / int16 quantised checkpoints are rejected: the engine computes in fp16."""
-    if os.path.isdir(path):
-        path = os.path.join(path, "model.bin")
-    variables, aliases, header = read_variables(path)
-    if header["spec"] != "WhisperSpec":
-        raise ValueError(f"model.bin holds a {header['spec']!r}, not a WhisperSpec")
-
-    def get(name: str) -> np.ndarray:
+    def var(name):
         key = aliases.get(name, name)
-        if key not in variables:
+        if key not in shapes:
             raise KeyError(f"model.bin: variable {name!r} is missing")
-        arr = variables[key]
-        if arr.dtype in (np.int8, np.int16) and arr.ndim >= 1:
-            raise ValueError(f"model.bin: {name!r} is quantised ({arr.dtype}); convert with --quantization float16")
-        return arr
+        return key
 
-    out: Dict[str, torch.Tensor] = {}
+    def whole(dst, src):
+        plan.append((dst, var(src), None))
+
+    def norm(src, dst):
+        whole(f"{dst}.weight", f"{src}/gamma")
+        whole(f"{dst}.bias", f"{src}/beta")
+
+    def attention(src, dst, cross):
+        if cross:
+            d = shapes[var(f"{src}/linear_0/weight")][0]
+            whole(f"{dst}.q_proj.weight", f"{src}/linear_0/weight")
+            whole(f"{dst}.q_proj.bias", f"{src}/linear_0/bias")
+            kv, kvb = var(f"{src}/linear_1/weight"), var(f"{src}/linear_1/bias")
+            plan.extend([(f"{dst}.k_proj.weight", kv, (0, d)), (f"{dst}.v_proj.weight", kv, (d, 2 * d)),
+                         (f"{dst}.v_proj.bias", kvb, (d, 2 * d))])
+            out = 2
+        else:
+            w, b = var(f"{src}/linear_0/weight"), var(f"{src}/linear_0/bias")
+            d = shapes[w][0] // 3
+            plan.extend([(f"{dst}.q_proj.weight", w, (0, d)), (f"{dst}.q_proj.bias", b, (0, d)),
+                         (f"{dst}.k_proj.weight", w, (d, 2 * d)),
+                         (f"{dst}.v_proj.weight", w, (2 * d, 3 * d)), (f"{dst}.v_proj.bias", b, (2 * d, 3 * d))])
+            out = 1
+        whole(f"{dst}.out_proj.weight", f"{src}/linear_{out}/weight")
+        whole(f"{dst}.out_proj.bias", f"{src}/linear_{out}/bias")
+
+    def ffn(s, h):
+        norm(f"{s}/ffn/layer_norm", f"{h}.final_layer_norm")
+        for i, fc in enumerate(("fc1", "fc2")):
+            whole(f"{h}.{fc}.weight", f"{s}/ffn/linear_{i}/weight")
+            whole(f"{h}.{fc}.bias", f"{s}/ffn/linear_{i}/bias")
+
     for conv in ("conv1", "conv2"):
-        out[f"model.encoder.{conv}.weight"] = _f32(get(f"encoder/{conv}/weight"))
-        out[f"model.encoder.{conv}.bias"] = _f32(get(f"encoder/{conv}/bias"))
-    out["model.encoder.embed_positions.weight"] = _f32(get("encoder/position_encodings/encodings"))
-    _norm_to_hf(get, "encoder/layer_norm", "model.encoder.layer_norm", out)
+        whole(f"model.encoder.{conv}.weight", f"encoder/{conv}/weight")
+        whole(f"model.encoder.{conv}.bias", f"encoder/{conv}/bias")
+    whole("model.encoder.embed_positions.weight", "encoder/position_encodings/encodings")
+    norm("encoder/layer_norm", "model.encoder.layer_norm")
     n_enc = 0
-    while f"encoder/layer_{n_enc}/self_attention/linear_0/weight" in variables:
+    while f"encoder/layer_{n_enc}/self_attention/linear_0/weight" in shapes:
         s, h = f"encoder/layer_{n_enc}", f"model.encoder.layers.{n_enc}"
-        _norm_to_hf(get, f"{s}/self_attention/layer_norm", f"{h}.self_attn_layer_norm", out)
-        _attention_to_hf(get, f"{s}/self_attention", f"{h}.self_attn", out, cross=False)
-        _norm_to_hf(get, f"{s}/ffn/layer_norm", f"{h}.final_layer_norm", out)
-        for i, fc in enumerate(("fc1", "fc2")):
-            out[f"{h}.{fc}.weight"], out[f"{h}.{fc}.bias"] = _f32(get(f"{s}/ffn/linear_{i}/weight")), _f32(get(f"{s}/ffn/linear_{i}/bias"))
+        norm(f"{s}/self_attention/layer_norm", f"{h}.self_attn_layer_norm")
+        attention(f"{s}/self_attention", f"{h}.self_attn", cross=False)
+        ffn(s, h)
         n_enc += 1
-    out["model.decoder.embed_tokens.weight"] = _f32(get("decoder/embeddings/weight"))
-    out["model.decoder.embed_positions.weight"] = _f32(get("decoder/position_encodings/encodings"))
-    _norm_to_hf(get, "decoder/layer_norm", "model.decoder.layer_norm", out)
+    whole("model.decoder.embed_tokens.weight", "decoder/embeddings/weight")
+    whole("model.decoder.embed_positions.weight", "decoder/position_encodings/encodings")
+    norm("decoder/layer_norm", "model.decoder.layer_norm")
     n_dec = 0
-    while f"decoder/layer_{n_dec}/self_attention/linear_0/weight" in variables:
+    while f"decoder/layer_{n_dec}/self_attention/linear_0/weight" in shapes:
         s, h = f"decoder/layer_{n_dec}", f"model.decoder.layers.{n_dec}"
-        _norm_to_hf(get, f"{s}/self_attention/layer_norm", f"{h}.self_attn_layer_norm", out)
-        _attention_to_hf(get, f"{s}/self_attention", f"{h}.self_attn", out, cross=False)
-        _norm_to_hf(get, f"{s}/attention/layer_norm", f"{h}.encoder_attn_layer_norm", out)
-        _attention_to_hf(get, f"{s}/attention", f"{h}.encoder_attn", out, cross=True)
-        _norm_to_hf(get, f"{s}/ffn/layer_norm", f"{h}.final_layer_norm", out)
-        for i, fc in enumerate(("fc1", "fc2")):
-            out[f"{h}.{fc}.weight"], out[f"{h}.{fc}.bias"] = _f32(get(f"{s}/ffn/linear_{i}/weight")), _f32(get(f"{s}/ffn/linear_{i}/bias"))
+        norm(f"{s}/self_attention/layer_norm", f"{h}.self_attn_layer_norm")
+        attention(f"{s}/self_attention", f"{h}.self_attn", cross=False)
+        norm(f"{s}/attention/layer_norm", f"{h}.encoder_attn_layer_norm")
+        attention(f"{s}/attention", f"{h}.encoder_attn", cross=True)
+        ffn(s, h)
         n_dec += 1
     if n_enc == 0 or n_dec == 0:
         raise ValueError("model.bin: no encoder / decoder layers found under the expected variable names")
-    return out
+    return plan
+
+
+class Ct2Checkpoint:
+    """A CTranslate2 ``model.bin`` read in place: the variable table from the header, payloads through one read-only
+    memory map.  ``tensors()`` yields ``(canonical name, array as stored, scale or None)`` one tensor at a time:
+    float32 / float16 arrays, bfloat16 as uint16 bit patterns, int8 with its per-row scales (module comment above)."""
+    layout = "ct2"
+
+    def __init__(self, path: str):
+        if os.path.isdir(path):
+            path = os.path.join(path, "model.bin")
+        self.path = path
+        variables, aliases, header = read_variables(path, header_only=True)
+        if header["spec"] != "WhisperSpec":
+            raise ValueError(f"model.bin holds a {header['spec']!r}, not a WhisperSpec")
+        self.variables, self.aliases = variables, aliases
+        self.plan = ct2_plan({k: v.shape for k, v in variables.items()}, aliases)
+        for dst, src, _ in self.plan:
+            info = variables[src]
+            if info.dtype_id == 2:
+                raise ValueError(f"model.bin: {src!r} is int16-quantised; int16 CTranslate2 files are not supported "
+                                 f"(convert with --quantization float16, int8_float16 or bfloat16)")
+            if info.dtype_id == 1:
+                sc = variables.get(src + "_scale")
+                if sc is None:
+                    raise ValueError(f"model.bin: {src!r} is int8 but its scale {src + '_scale'!r} is missing")
+                if sc.dtype_id not in (0, 4, _BF16) or int(np.prod(sc.shape)) != info.shape[0]:
+                    raise ValueError(f"model.bin: {src + '_scale'!r} must hold one float per row of {src!r} "
+                                     f"({info.shape[0]}), has shape {sc.shape} and dtype id {sc.dtype_id}")
+            elif info.dtype_id not in (0, 4, _BF16):
+                raise ValueError(f"model.bin: {src!r} has dtype id {info.dtype_id}, not a float or int8 weight")
+        self.shapes = {dst: ((r[1] - r[0],) if r else variables[src].shape[:1]) + tuple(variables[src].shape[1:])
+                       for dst, src, r in self.plan}
+        # the spec stores each stack's head count as an int16 scalar; the engine runs 64-wide heads only
+        d = self.shapes["model.encoder.conv1.weight"][0]
+        for side in ("encoder", "decoder"):
+            info = variables.get(f"{side}/num_heads")
+            if info is None:
+                continue
+            with open(path, "rb") as f:
+                f.seek(info.offset)
+                raw = f.read(info.n_bytes)
+            heads = int(np.frombuffer(raw, dtype=_DTYPES[info.dtype_id])[0])
+            if heads <= 0 or d != 64 * heads:
+                raise ValueError(f"model.bin: {side}/num_heads = {heads} with d_model {d} is a head dimension other "
+                                 f"than 64; the engine runs 64 only")
+
+    def _array(self, mm, name: str) -> np.ndarray:
+        info = self.variables[name]
+        dt = np.uint16 if info.dtype_id == _BF16 else _DTYPES[info.dtype_id]
+        count = int(np.prod(info.shape)) if info.shape else 1
+        return np.frombuffer(mm, dtype=dt, count=count, offset=info.offset).reshape(info.shape)
+
+    def tensors(self) -> Iterator[Tuple[str, np.ndarray, Optional[np.ndarray]]]:
+        mm = np.memmap(self.path, dtype=np.uint8, mode="r")
+        try:
+            for dst, src, rows in self.plan:
+                a = self._array(mm, src)
+                scale = self._array(mm, src + "_scale").reshape(-1) if a.dtype == np.int8 else None
+                if rows is not None:
+                    a = a[rows[0]:rows[1]]
+                    scale = scale[rows[0]:rows[1]] if scale is not None else None
+                yield dst, a, scale
+        finally:
+            del mm
+
+
+def load_ct2_model_bin(path: str) -> Dict[str, torch.Tensor]:
+    """``model.bin`` (or its directory) -> the canonical HF-named fp32 dict (the key space of the Hugging Face
+    readers, weights.HFCheckpoint).  int8 weights are dequantized with the rule above; int16 files are refused."""
+    from .weights import to_float32
+    return {name: torch.from_numpy(to_float32(a, scale)) for name, a, scale in Ct2Checkpoint(path).tensors()}
 
 
 def expected_ct2_names(n_enc: int, n_dec: int) -> List[str]:
@@ -224,13 +319,43 @@ def expected_ct2_names(n_enc: int, n_dec: int) -> List[str]:
     return names
 
 
-def save_ct2_model_bin(weights: Dict[str, torch.Tensor], path: str, dtype=np.float16) -> None:
-    """Inverse of load_ct2_model_bin (tests, and to hand a checkpoint to a CTranslate2 install for cross-checks)."""
+QUANTIZATIONS = {"float32": (np.float32, False), "float16": (np.float16, False), "bfloat16": ("bfloat16", False),
+                 "int8": (np.float32, True), "int8_float32": (np.float32, True), "int8_float16": (np.float16, True),
+                 "int8_bfloat16": ("bfloat16", True), "int16": (np.float32, "int16")}
+
+
+def _quantize(w: np.ndarray, bits: int = 8) -> Tuple[np.ndarray, np.ndarray]:
+    """The converter's per-row quantization (module comment above); int16 uses one power-of-two scale."""
+    w = w.astype(np.float32)
+    if bits == 16:
+        scale = np.float32(2.0 ** np.floor(np.log2(32767.0 / max(float(np.abs(w).max()), 1e-30))))
+        return np.rint(w * scale).astype(np.int16), np.asarray(scale, np.float32)
+    amax = np.abs(w).max(axis=1)
+    amax[amax == 0] = 127.0
+    scale = (127.0 / amax).astype(np.float32)
+    return np.rint(w * scale[:, None]).astype(np.int8), scale
+
+
+def save_ct2_model_bin(weights: Dict[str, torch.Tensor], path: str, dtype=np.float16,
+                       quantization: Optional[str] = None) -> None:
+    """Inverse of load_ct2_model_bin (tests, and to hand a checkpoint to a CTranslate2 install for cross-checks).
+    ``quantization`` names a CTranslate2 conversion ("float16", "bfloat16", "int8_float16", ...): float variables are
+    written in its float type, and for int8* / int16 every 2-D ``.../weight`` is quantized with a ``..._scale``
+    sibling.  Without it every variable is written as ``dtype``."""
+    quant = False
+    if quantization is not None:
+        if quantization not in QUANTIZATIONS:
+            raise ValueError(f"quantization {quantization!r}: one of {sorted(QUANTIZATIONS)}")
+        dtype, quant = QUANTIZATIONS[quantization]
+
     def npy(name):
-        return weights[name].detach().cpu().numpy().astype(dtype)
+        a = weights[name].detach().cpu().float()
+        if dtype == "bfloat16":
+            return a.bfloat16().view(torch.int16).numpy().view(np.uint16)
+        return a.numpy().astype(dtype)
 
     def zeros_like_bias(w):
-        return np.zeros((w.shape[0],), dtype=dtype)
+        return np.zeros((w.shape[0],), dtype=np.uint16 if dtype == "bfloat16" else dtype)
 
     v: Dict[str, np.ndarray] = {}
     for conv in ("conv1", "conv2"):
@@ -276,6 +401,13 @@ def save_ct2_model_bin(weights: Dict[str, torch.Tensor], path: str, dtype=np.flo
         v[f"{s}/attention/linear_2/weight"], v[f"{s}/attention/linear_2/bias"] = npy(f"{a}.out_proj.weight"), npy(f"{a}.out_proj.bias")
         ffn(h, s)
         i += 1
+    if quant:
+        for name in [k for k in v if k.endswith("/weight") and v[k].ndim == 2]:
+            w = v[name].astype(np.uint32) << 16 if v[name].dtype == np.uint16 else v[name]
+            w = w.view(np.float32) if w.dtype == np.uint32 else w
+            v[name], v[name + "_scale"] = _quantize(w, 16 if quant == "int16" else 8)
+    heads = np.int16(v["encoder/conv1/weight"].shape[0] // 64)
+    v["encoder/num_heads"] = v["decoder/num_heads"] = np.asarray(heads, dtype=np.int16)
     # the output projection is tied to the embedding: CT2 stores it once and lists the second name as an alias
     write_variables(path, v, aliases={"decoder/projection/weight": "decoder/embeddings/weight"})
 

@@ -98,6 +98,10 @@ class EncoderOutput:
         return out.astype(dtype) if dtype is not None else out
 
 
+# stored dtype -> WL_DT_* of wl_load_tensor_typed (uint16 is bfloat16 bits: weights.BF16)
+_WL_DT = {np.dtype(np.float32): 0, np.dtype(np.float16): 1, np.dtype(np.uint16): 2, np.dtype(np.int8): 3}
+
+
 def footprint_estimate(dims: WhisperDims, max_streams: int = 8, max_beam: int = 5, enc_slots: Optional[int] = None,
                        n_align_heads: Optional[int] = None, vad: bool = False, diarize: bool = False) -> int:
     """Device bytes a context of these shapes allocates through ``wl_init``, the weight load and one open decode session
@@ -271,26 +275,33 @@ class B200Whisper:
             dims = dims_for(model_size_or_path)
             return cls(dims, W.random_init(dims, seed=seed), device_index=device_index, compute_type=compute_type,
                        max_streams=max_streams, max_beam=max_beam, **kw)
-        model_dir = None
+        model_dir, metadata = None, {}
         if weights is None:
             model_dir = W.resolve_model_dir(model_size_or_path, download_root=download_root, local_files_only=local_files_only)
-            weights = W.load_model_dir(model_dir)
-            if kw.get("alignment_heads") is None:
-                from .ct2_format import read_ct2_config
-                heads = read_ct2_config(model_dir).get("alignment_heads")
-                if heads:
-                    kw["alignment_heads"] = heads
+            weights = W.open_checkpoint(model_dir)     # streamed to the device tensor by tensor, as stored
+            metadata = W.model_metadata(model_dir)
+            if kw.get("alignment_heads") is None and metadata.get("alignment_heads"):
+                kw["alignment_heads"] = metadata["alignment_heads"]
+        shapes = weights.shapes if hasattr(weights, "tensors") else weights
         try:
             dims = dims_for(model_size_or_path)
         except KeyError:
-            dims = W.infer_dims(weights, str(model_size_or_path))
+            dims = W.infer_dims(shapes, str(model_size_or_path))
         eng = cls(dims, weights, device_index=device_index, compute_type=compute_type, max_streams=max_streams,
                   max_beam=max_beam, **kw)
         eng.model_dir = model_dir
+        eng.model_metadata = metadata
         return eng
 
     def _load_weights(self, weights) -> None:
+        """``weights``: a tensor dict (uploaded as fp32 through ``wl_load_tensor``) or a checkpoint reader
+        (``weights.open_checkpoint``), whose tensors go over one at a time in their stored dtype through
+        ``wl_load_tensor_typed`` and are converted on the device."""
         from .feature_extractor import mel_filters
+        if hasattr(weights, "tensors"):
+            for name, a, scale in weights.tensors():
+                self._load_typed(name, a, scale)
+            weights = {}
         items = dict(weights)
         items["mel_filters"] = mel_filters(self.dims.n_mels)
         for name, t in items.items():
@@ -300,6 +311,19 @@ class B200Whisper:
             rc = self.lib.wl_load_tensor(self.ctx, name.encode(), _lib.ptr(a, C.c_float), _lib.ptr(shape, C.c_int64), a.ndim)
             _lib.check(self.lib, self.ctx, rc, f"wl_load_tensor({name})")
         _lib.check(self.lib, self.ctx, self.lib.wl_finalize_weights(self.ctx), "wl_finalize_weights")
+
+    def _load_typed(self, name: str, a: np.ndarray, scale: Optional[np.ndarray] = None) -> None:
+        a = np.ascontiguousarray(a)
+        if a.dtype not in _WL_DT:
+            raise ValueError(f"{name}: dtype {a.dtype} cannot be uploaded (float32, float16, bfloat16 bits or int8)")
+        shape = np.asarray(a.shape, dtype=np.int64)
+        s, sdt = None, 0
+        if scale is not None:
+            s = np.ascontiguousarray(scale).reshape(-1)
+            sdt = _WL_DT[s.dtype]
+        rc = self.lib.wl_load_tensor_typed(self.ctx, name.encode(), a.ctypes.data, _WL_DT[a.dtype],
+                                           _lib.ptr(shape, C.c_int64), a.ndim, None if s is None else s.ctypes.data, sdt)
+        _lib.check(self.lib, self.ctx, rc, f"wl_load_tensor_typed({name})")
 
     # ------------------------------------------------------------------ properties (ctranslate2 names)
     @property

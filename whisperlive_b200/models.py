@@ -255,7 +255,8 @@ def _wl_free_bytes(device: int) -> int:
 def engine_footprint(name: str, max_streams: int = 8, max_beam: int = 5, resolve: Optional[Callable[[str], str]] = None,
                      vad: bool = False, diarize: bool = False) -> Optional[int]:
     """``footprint_estimate`` of the CUDA engine for a size name, or for a model directory whose HF ``config.json``
-    gives the shapes; None when the shapes cannot be known before the weights are read.  ``vad``: the model runs the
+    or weight headers (safetensors header or index, ``pytorch_model.bin``, CTranslate2 ``model.bin`` table) give the
+    shapes; None only for a directory with no readable header.  ``vad``: the model runs the
     Silero VAD on its context (``vad="device"``); ``diarize``: it computes speaker embeddings there
     (``WLB200_DIARIZE=device``)."""
     from .config import WhisperDims, dims_for
@@ -273,6 +274,9 @@ def engine_footprint(name: str, max_streams: int = 8, max_beam: int = 5, resolve
             if "d_model" in cfg:
                 dims = WhisperDims(str(name), int(cfg["d_model"]), int(cfg["d_model"]) // 64, int(cfg["encoder_layers"]),
                                    int(cfg["decoder_layers"]), int(cfg["num_mel_bins"]), int(cfg["vocab_size"]))
+        if dims is None and isinstance(path, str) and os.path.isdir(path):
+            from .weights import checkpoint_dims
+            dims = checkpoint_dims(path, str(name))
         if dims is None:
             return None
     return footprint_estimate(dims, max_streams=max_streams, max_beam=max_beam, vad=vad, diarize=diarize)
