@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 12
+#define WL_ABI_VERSION 13
 
 typedef struct wl_ctx wl_ctx;
 
@@ -140,6 +140,13 @@ int wl_generate(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* pro
  *                      spec (num_hypotheses out of range, temperature <= 0 or not finite, negative key) fails the
  *                      whole call before anything is staged: every index stays free.  sample = 0 is the session's own
  *                      search (the other fields are ignored).
+ *                      rules[n] (ABI 13; NULL, or rules = 0 for a stream: the session's options) gives a stream its own
+ *                      logits rules -- suppress list, suppress_blank, max_initial_timestamp_index -- and its own
+ *                      length_penalty and patience (the finished hypotheses that end a beam stream; the ranking of
+ *                      wl_session_collect and wl_session_peek).  They live in per-index device tables the captured loop
+ *                      reads: admitting a stream with its own rules captures no new graph, and its result does not
+ *                      depend on the other streams.  beam_size stays the session's (0 or equal; anything else fails the
+ *                      call, like a bad patience, before anything is staged).
  *   wl_session_run     runs the device-side token loop over every admitted stream for at most max_steps steps; with
  *                      break_on_finish it also returns as soon as some stream has finished.  done_out[capacity]: 1 for
  *                      indices whose stream is finished and not yet collected.  steps_ran: token steps executed.
@@ -174,8 +181,19 @@ typedef struct wl_stream_search {
   uint32_t seed;             /* sampling noise = that of wl_generate(seed) ... */
   int32_t noise_key;         /* ... for the stream at batch position noise_key (>= 0) */
 } wl_stream_search;
+typedef struct wl_stream_rules {
+  int32_t rules;             /* 0: the session's options (the other fields are ignored); 1: the fields below */
+  int32_t beam_size;         /* 0 or the session's beam_size: rows per stream are fixed per session */
+  float patience;            /* beam search ends with round(beam_size * patience) <= 16 hypotheses */
+  float length_penalty;
+  int32_t suppress_blank;
+  int32_t max_initial_timestamp_index;
+  const int32_t* suppress_tokens;   /* ids outside the vocabulary are ignored, as in wl_gen_opts */
+  int32_t n_suppress;
+} wl_stream_rules;
 int wl_session_admit_ex(wl_ctx* ctx, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
-                        const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search);
+                        const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search,
+                        const wl_stream_rules* rules);
 int wl_session_run(wl_ctx* ctx, int32_t max_steps, int32_t break_on_finish, int32_t* done_out, int32_t* steps_ran);
 int wl_session_collect(wl_ctx* ctx, int32_t index, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
                        int32_t* out_steps);
@@ -282,6 +300,11 @@ typedef struct wl_search_script {
 int wl_test_search(wl_ctx* ctx, int32_t B, const int32_t* prompts, const int32_t* prompt_off, const wl_gen_opts* opts,
                    const wl_search_script* script, int32_t* out_ids, int32_t* out_len, float* out_score, float* out_no_speech,
                    int32_t* out_steps, int32_t* out_hyp_count, float* out_logits);
+/* Test hook: with script != NULL, the open decode session's streams are decoded on the scripted logits of
+ * wl_test_search instead of the decoder, from the next admission on (slots are not read; the stream starts at its last
+ * prompt token, as with opts->prefill = 1); NULL goes back to the decoder.  Only while no stream is decoding;
+ * wl_session_open resets it. */
+int wl_test_session_script(wl_ctx* ctx, const wl_search_script* script);
 /* device-resident timing of the GEMM kernel: C = A(MxK) * B(NxK)^T, `iters` launches between CUDA events;
  * bn = 0 picks the tile like the engine does. ms_out = average milliseconds per launch. */
 int wl_bench_gemm(wl_ctx* ctx, int32_t M, int32_t N, int32_t K, int32_t batch, int32_t iters, int32_t flags,

@@ -10,7 +10,7 @@ import threading
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libwlb200.so")
-ABI_VERSION = 12
+ABI_VERSION = 13
 
 c_i32p = C.POINTER(C.c_int32)
 c_i64p = C.POINTER(C.c_int64)
@@ -44,6 +44,14 @@ class WlStreamSearch(C.Structure):
     _fields_ = [
         ("sample", C.c_int32), ("num_hypotheses", C.c_int32), ("temperature", C.c_float), ("seed", C.c_uint32),
         ("noise_key", C.c_int32),
+    ]
+
+
+class WlStreamRules(C.Structure):
+    _fields_ = [
+        ("rules", C.c_int32), ("beam_size", C.c_int32), ("patience", C.c_float), ("length_penalty", C.c_float),
+        ("suppress_blank", C.c_int32), ("max_initial_timestamp_index", C.c_int32), ("suppress_tokens", c_i32p),
+        ("n_suppress", C.c_int32),
     ]
 
 
@@ -88,7 +96,7 @@ SIGNATURES = {
     "wl_session_open": (C.c_int, [C.c_void_p, C.POINTER(WlGenOpts), C.c_int32]),
     "wl_session_admit": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p]),
     "wl_session_admit_ex": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_i32p, c_i32p,
-                                      C.POINTER(WlStreamSearch)]),
+                                      C.POINTER(WlStreamSearch), C.POINTER(WlStreamRules)]),
     "wl_session_run": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, c_i32p, c_i32p]),
     "wl_session_collect": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_f32p, c_f32p, c_i32p]),
     "wl_session_peek": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, c_i32p, c_f32p, c_f32p, c_i32p, c_i32p]),
@@ -115,6 +123,7 @@ SIGNATURES = {
     "wl_test_layernorm": (C.c_int, [C.c_void_p, c_f32p, c_f32p, c_f32p, c_f32p, c_f32p, C.c_int32, C.c_int32]),
     "wl_test_search": (C.c_int, [C.c_void_p, C.c_int32, c_i32p, c_i32p, C.POINTER(WlGenOpts), C.POINTER(WlSearchScript),
                                  c_i32p, c_i32p, c_f32p, c_f32p, c_i32p, c_i32p, c_f32p]),
+    "wl_test_session_script": (C.c_int, [C.c_void_p, C.POINTER(WlSearchScript)]),
     "wl_bench_gemm": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, c_f32p]),
     "wl_kernel_launches": (C.c_int64, [C.c_void_p]),
     "wl_last_device_ms": (C.c_float, [C.c_void_p, C.c_int32]),

@@ -280,6 +280,10 @@ struct wl_ctx {
     std::vector<int> hp, meta;          // host shadows: prompts [cap][T_MAX], per-stream metadata [META_ROWS][cap]
     std::vector<char> used, finished;   // index holds an admitted stream / that stream has finished decoding
     std::vector<int> nh;                // hypotheses the index's stream returns: N when it samples, else NH
+    std::vector<int> rules;             // host shadow of the per-stream rule rows [RULE_ROWS][cap] (engine.cu)
+    std::vector<float> lp;              // length penalty of the index's stream (collect / peek ranking)
+    bool script_on = false;             // wl_test_session_script: scripted logits replace the decoder
+    SearchScript script{};
     int live = 0;                       // admitted and still decoding
     long steps = 0, runs = 0, admitted = 0;
   } sess;

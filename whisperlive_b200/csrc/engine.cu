@@ -81,7 +81,15 @@ static void alloc_decode_state(wl_ctx* c, DecodeState& s) {
   s.nrows = c->mem.alloc<int>(B);
   s.pre_n = c->mem.alloc<int>(B); s.pre_last = c->mem.alloc<int>(B); s.pre_penult = c->mem.alloc<int>(B); s.pre_lts = c->mem.alloc<int>(B);
   s.brk = c->mem.alloc<int>(2);
+  s.r_max_initial = s.r_suppress_blank = s.r_max_cand = nullptr;   // the call's SearchOpts (a session adds its own)
+  s.r_length_penalty = nullptr;
+  s.r_mask = nullptr;
+  s.mask_words = 0;
 }
+
+// Rows of a decode session's per-stream rule table (host shadow Session::rules -> DecodeState::r_*): max initial
+// timestamp index, suppress_blank, max_cand, length penalty (float bits)
+constexpr int RULE_ROWS = 4;
 
 // ------------------------------------------------------------------------------------------ init
 extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
@@ -1443,6 +1451,12 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
     ss.kcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
     ss.vcache = c->mem.alloc<__half>((size_t)c->Ld * c->cache_layer_stride, false);
     ss.mask = c->mem.alloc<unsigned>((c->V + 31) / 32 + 1);
+    // per-stream logits rules: the captured loop reads them, admission writes them (6.5 KB of mask per index at 51866)
+    DecodeState& sd = ss.ds;
+    sd.mask_words = (c->V + 31) / 32 + 1;
+    sd.r_max_initial = c->mem.alloc<int>(c->Bm); sd.r_suppress_blank = c->mem.alloc<int>(c->Bm);
+    sd.r_max_cand = c->mem.alloc<int>(c->Bm); sd.r_length_penalty = c->mem.alloc<float>(c->Bm);
+    sd.r_mask = c->mem.alloc<unsigned>((size_t)c->Bm * sd.mask_words);
     ss.idx_dev = c->mem.alloc<int>(c->Bm);
     ss.peek_dev = c->mem.alloc<int>((size_t)c->Bm * PEEK_STRIDE);
     ss.allocated = true;
@@ -1471,6 +1485,9 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
   ss.used.assign(cap, 0);
   ss.finished.assign(cap, 0);
   ss.nh.assign(cap, ss.NH);
+  ss.rules.assign((size_t)RULE_ROWS * cap, 0);
+  ss.lp.assign(cap, ss.length_penalty);
+  ss.script_on = false;
   ss.live = 0;
   cudaStream_t st = c->st;
   const DecodeState& s = ss.ds;
@@ -1489,11 +1506,31 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
 
 extern "C" int wl_session_admit(wl_ctx* c, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
                                 const int32_t* prompt_off, const int32_t* max_length) {
-  return wl_session_admit_ex(c, n, index, slots, prompts, prompt_off, max_length, nullptr);
+  return wl_session_admit_ex(c, n, index, slots, prompts, prompt_off, max_length, nullptr, nullptr);
+}
+
+// a stream's own logits rules, checked before anything is staged; every message names the field
+static void check_stream_rules(const wl_ctx::Session& ss, int i, const wl_stream_rules& q) {
+  WL_CHECK(q.rules == 1, WL_ERR_ARG, "wl_session_admit: stream %d: rules must be 0 or 1, got %d", i, q.rules);
+  WL_CHECK(q.beam_size == 0 || q.beam_size == ss.K, WL_ERR_ARG,
+           "wl_session_admit: stream %d: beam_size %d differs from the session's %d (rows per stream are fixed per session)",
+           i, q.beam_size, ss.K);
+  WL_CHECK(std::isfinite(q.patience) && q.patience > 0.f, WL_ERR_ARG, "wl_session_admit: stream %d: patience %g must be finite and > 0",
+           i, (double)q.patience);
+  char who[64];
+  snprintf(who, sizeof(who), "wl_session_admit: stream %d: patience", i);
+  max_candidates(ss.K, q.patience, who);
+  WL_CHECK(std::isfinite(q.length_penalty), WL_ERR_ARG, "wl_session_admit: stream %d: length_penalty %g is not finite", i,
+           (double)q.length_penalty);
+  WL_CHECK(q.max_initial_timestamp_index >= 0, WL_ERR_ARG, "wl_session_admit: stream %d: negative max_initial_timestamp_index %d",
+           i, q.max_initial_timestamp_index);
+  WL_CHECK(q.n_suppress >= 0 && (q.n_suppress == 0 || q.suppress_tokens), WL_ERR_ARG,
+           "wl_session_admit: stream %d: suppress_tokens is null for n_suppress %d", i, q.n_suppress);
 }
 
 extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, const int32_t* slots, const int32_t* prompts,
-                                   const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search) {
+                                   const int32_t* prompt_off, const int32_t* max_length, const wl_stream_search* search,
+                                   const wl_stream_rules* rules) {
   API_BEGIN(c)
   wl_ctx::Session& ss = c->sess;
   WL_CHECK(ss.open, WL_ERR_STATE, "wl_session_admit: no open session");
@@ -1512,34 +1549,75 @@ extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, c
                "wl_session_admit: stream %d: sampling temperature %g must be finite and > 0", i, (double)q.temperature);
       WL_CHECK(q.noise_key >= 0, WL_ERR_ARG, "wl_session_admit: stream %d: negative noise key %d", i, q.noise_key);
     }
+    if (rules && rules[i].rules) check_stream_rules(ss, i, rules[i]);
   }
   // validate + stage everything before touching the session (a bad prompt must not leave a half-admitted stream)
-  std::vector<int> hp = ss.hp, meta = ss.meta;
+  std::vector<int> hp = ss.hp, meta = ss.meta, rl = ss.rules;
+  const int nwords = ss.ds.mask_words;
+  std::vector<unsigned> masks;   // [n][nwords]: the own suppress lists, in admission order (empty rows unused)
+  if (rules) masks.assign((size_t)n * nwords, 0u);
   for (int i = 0; i < n; ++i) {
     stream_meta(c, i, slots[i], prompts + prompt_off[i], prompt_off[i + 1] - prompt_off[i], max_length[i], false,
-                hp.data() + (size_t)index[i] * T_MAX, meta.data(), index[i], cap, nullptr);
+                hp.data() + (size_t)index[i] * T_MAX, meta.data(), index[i], cap, nullptr, !ss.script_on);
     const bool sample = search && search[i].sample;
     search_meta(meta.data(), index[i], cap, sample ? 1 : 0, sample ? search[i].temperature : 0.f, sample ? search[i].seed : 0u,
                 sample ? search[i].noise_key : index[i], sample ? search[i].num_hypotheses : ss.Kr);
+    const bool own = rules && rules[i].rules;
+    const float lp = own ? rules[i].length_penalty : ss.length_penalty;
+    int lbits;
+    memcpy(&lbits, &lp, 4);
+    const int b = index[i];
+    rl[0 * cap + b] = own ? rules[i].max_initial_timestamp_index : ss.so.max_initial_ts;
+    rl[1 * cap + b] = own ? (rules[i].suppress_blank ? 1 : 0) : ss.so.suppress_blank;
+    rl[2 * cap + b] = own ? max_candidates(ss.K, rules[i].patience, "wl_session_admit") : ss.so.max_cand;
+    rl[3 * cap + b] = lbits;
+    if (own)
+      for (int k = 0; k < rules[i].n_suppress; ++k) {
+        const int t = rules[i].suppress_tokens[k];
+        if (t >= 0 && t < c->V) masks[(size_t)i * nwords + (t >> 5)] |= 1u << (t & 31);
+      }
   }
   ss.hp.swap(hp);
   ss.meta.swap(meta);
-  for (int i = 0; i < n; ++i) ss.nh[index[i]] = (search && search[i].sample) ? search[i].num_hypotheses : ss.NH;
-  ensure_host(c, (size_t)cap * (T_MAX + 16) + n, 16);
+  ss.rules.swap(rl);
+  for (int i = 0; i < n; ++i) {
+    ss.nh[index[i]] = (search && search[i].sample) ? search[i].num_hypotheses : ss.NH;
+    ss.lp[index[i]] = (rules && rules[i].rules) ? rules[i].length_penalty : ss.length_penalty;
+  }
+  ensure_host(c, (size_t)cap * (T_MAX + 16) + n + (size_t)RULE_ROWS * cap, 16);
   int* php = c->h_int;
   int* pmeta = php + (size_t)cap * T_MAX;
   int* pidx = pmeta + (size_t)META_ROWS * cap;
+  int* prules = pidx + n;
   memcpy(php, ss.hp.data(), ss.hp.size() * 4);
   memcpy(pmeta, ss.meta.data(), ss.meta.size() * 4);
   memcpy(pidx, index, (size_t)n * 4);
-  SessScope scope(c);
+  memcpy(prules, ss.rules.data(), ss.rules.size() * 4);
   cudaStream_t st = c->st;
   WL_CUDA(cudaEventRecord(c->ev0, st));
+  {
+    // the rule tables of the session state (written like the others with what the streams in flight already hold) and
+    // each admitted index's suppress mask: its own list, or a copy of the session's
+    const DecodeState& sd = ss.ds;
+    void* dst[RULE_ROWS] = {sd.r_max_initial, sd.r_suppress_blank, sd.r_max_cand, sd.r_length_penalty};
+    for (int k = 0; k < RULE_ROWS; ++k) WL_CUDA(cudaMemcpyAsync(dst[k], prules + (size_t)k * cap, cap * 4, cudaMemcpyHostToDevice, st));
+    for (int i = 0; i < n; ++i) {
+      unsigned* m = sd.r_mask + (size_t)index[i] * nwords;
+      if (rules && rules[i].rules)
+        WL_CUDA(cudaMemcpyAsync(m, masks.data() + (size_t)i * nwords, (size_t)nwords * 4, cudaMemcpyHostToDevice, st));
+      else
+        WL_CUDA(cudaMemcpyAsync(m, ss.mask, (size_t)nwords * 4, cudaMemcpyDeviceToDevice, st));
+    }
+  }
+  SessScope scope(c);
   // the tables of the streams in flight are rewritten with the values they already hold (nothing runs between two calls)
   upload_state_tables(c, php, pmeta, cap);
   WL_CUDA(cudaMemcpyAsync(ss.idx_dev, pidx, (size_t)n * 4, cudaMemcpyHostToDevice, st));
-  WL_CUDA(cudaStreamSynchronize(st));
-  prefill_forward(c, n, ss.Kr, ss.hp.data(), ss.meta.data() + 1 * cap, ss.meta.data() + 2 * cap, slots, index);
+  WL_CUDA(cudaStreamSynchronize(st));   // `masks` goes out of scope
+  if (ss.script_on)   // scripted logits: no decoder pass; the no-speech probability comes from the script
+    scripted_no_speech(st, c->ds, vocab_ids(c), ss.script, n, ss.idx_dev);
+  else
+    prefill_forward(c, n, ss.Kr, ss.hp.data(), ss.meta.data() + 1 * cap, ss.meta.data() + 2 * cap, slots, index);
   decode_init(st, c->ds, ss.so, vocab_ids(c), n, cap * ss.Kr, 1, ss.idx_dev);
   WL_CUDA(cudaEventRecord(c->ev1, st));
   WL_CUDA(cudaStreamSynchronize(st));
@@ -1547,6 +1625,21 @@ extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, c
   for (int i = 0; i < n; ++i) { ss.used[index[i]] = 1; ss.finished[index[i]] = 0; }
   ss.live += n;
   ss.admitted += n;
+  API_END(c)
+}
+
+extern "C" int wl_test_session_script(wl_ctx* c, const wl_search_script* script) {
+  API_BEGIN(c)
+  wl_ctx::Session& ss = c->sess;
+  WL_CHECK(ss.open, WL_ERR_STATE, "wl_test_session_script: no open session");
+  WL_CHECK(ss.live == 0, WL_ERR_STATE, "wl_test_session_script: %d streams are still decoding", ss.live);
+  if (script) {
+    WL_CHECK(script->pattern >= -1 && script->pattern <= 5, WL_ERR_ARG, "wl_test_session_script: pattern %d out of range",
+             script->pattern);
+    ss.script.seed = script->seed;
+    ss.script.pattern = script->pattern;
+  }
+  ss.script_on = script != nullptr;
   API_END(c)
 }
 
@@ -1570,7 +1663,7 @@ extern "C" int wl_session_run(wl_ctx* c, int32_t max_steps, int32_t break_on_fin
     WL_CUDA(cudaEventRecord(c->ev0, st));
     if (ss.use_graph) {
       long kernels = 0;
-      cudaGraphExec_t exec = decode_graph(c, "s", cap, ss.Kr, ss.K, ss.so, vi, ss.nsplit, &kernels);
+      cudaGraphExec_t exec = decode_graph(c, "s", cap, ss.Kr, ss.K, ss.so, vi, ss.nsplit, &kernels, ss.script_on ? &ss.script : nullptr);
       WL_CUDA(cudaGraphLaunch(exec, st));
       WL_CUDA(cudaMemcpyAsync(h + 4, c->ds.steps_left, 4, cudaMemcpyDeviceToHost, st));
       WL_CUDA(cudaMemcpyAsync(h + 8, c->ds.done, (size_t)cap * 4, cudaMemcpyDeviceToHost, st));
@@ -1580,7 +1673,7 @@ extern "C" int wl_session_run(wl_ctx* c, int32_t max_steps, int32_t break_on_fin
       c->graph_launched += kernels * (long)ran;
     } else {   // graph-less (profiling / bisecting): the same loop condition evaluated on the host after every step
       for (;;) {
-        decode_step(c, cap, ss.Kr, ss.so, vi, ss.nsplit, false);
+        token_step(c, cap, ss.Kr, ss.so, vi, ss.nsplit, ss.script_on ? &ss.script : nullptr);
         ++ran;
         WL_CUDA(cudaMemcpyAsync(h + 5, c->ds.n_done, 4, cudaMemcpyDeviceToHost, st));
         WL_CUDA(cudaStreamSynchronize(st));
@@ -1624,7 +1717,7 @@ extern "C" int wl_session_collect(wl_ctx* c, int32_t index, int32_t* out_ids, in
   WL_CUDA(cudaMemcpyAsync(h_cum, s.hyp_cum + (size_t)index * MAX_HYPS, MAX_HYPS * 4, cudaMemcpyDeviceToHost, st));
   WL_CUDA(cudaMemcpyAsync(h_ns, s.no_speech + index, 4, cudaMemcpyDeviceToHost, st));
   WL_CUDA(cudaStreamSynchronize(st));
-  emit_hyps(ss.nh[index], ss.length_penalty, h_cnt[0], h_len, h_cum, h_tok, out_ids, out_len, out_score);
+  emit_hyps(ss.nh[index], ss.lp[index], h_cnt[0], h_len, h_cum, h_tok, out_ids, out_len, out_score);
   if (out_no_speech) *out_no_speech = h_ns[0];
   if (out_steps) *out_steps = h_steps[0];
   ss.used[index] = 0;
@@ -1671,7 +1764,7 @@ extern "C" int wl_session_peek(wl_ctx* c, int32_t n, const int32_t* index, int32
       for (int k = 0; k < e[6]; ++k) {
         float ck;
         memcpy(&ck, e + PEEK_TAB + MAX_HYPS + k, 4);
-        const float sc = hyp_score(ck, e[PEEK_TAB + k], ss.length_penalty);
+        const float sc = hyp_score(ck, e[PEEK_TAB + k], ss.lp[index[i]]);
         if (k == 0 || sc > bs) { best = k; bs = sc; }
       }
     }
@@ -1685,7 +1778,7 @@ extern "C" int wl_session_peek(wl_ctx* c, int32_t n, const int32_t* index, int32
       memcpy(out_ids + (size_t)i * T_MAX, e + PEEK_HDR, (size_t)len * 4);
     }
     out_len[i] = len;
-    out_score[i] = len < 0 ? 0.f : hyp_score(cum, len, ss.length_penalty);
+    out_score[i] = len < 0 ? 0.f : hyp_score(cum, len, ss.lp[index[i]]);
     if (out_no_speech) out_no_speech[i] = ns;
     if (out_step) out_step[i] = e[3];
     if (out_final) out_final[i] = e[4];

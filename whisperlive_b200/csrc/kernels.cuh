@@ -149,6 +149,14 @@ struct DecodeState {
   unsigned* nseed;   // [B] sampling noise seed
   int* nkey;         // [B] noise key: the stream index that goes into the noise hash
   int* nrows;        // [B] rows the stream uses (<= rows_per_stream); rows nrows .. rows_per_stream-1 stay inactive
+  // per-stream logits rules (decode sessions only; null in the one-shot state, whose streams take SearchOpts).  Written
+  // at admission -- the session's own options for a stream admitted without rules -- and read by the captured loop.
+  int* r_max_initial;   // [B] max_initial_timestamp_index
+  int* r_suppress_blank;// [B]
+  int* r_max_cand;      // [B] round(beam * patience): finished hypotheses that end a beam stream
+  float* r_length_penalty; // [B] (session_peek's ranking)
+  unsigned* r_mask;     // [B][mask_words] suppress bitmask
+  int mask_words;
   int* brk;         // [2] decode sessions (step-level admission): [0] != 0 -> the device-side loop also ends as soon as a
                      //   stream finishes (so the host can hand its result out and refill the index); [1] = n_done at launch
   // teacher-forced mode (detect_language / align / logits test hook)
@@ -203,8 +211,10 @@ struct SearchScript {
 void scripted_logits(cudaStream_t st, const DecodeState& s, const SearchOpts& o, const VocabIds& v, const SearchScript& sc,
                      float* logits, int R);
 // no_speech[b] = softmax(scripted logits of prompt[0 .. sot])[no_speech] for every stream whose sot precedes its last
-// prompt token (what the batched prefill writes in production)
-void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B);
+// prompt token (what the batched prefill writes in production).  index != null (device, B entries): only those stream
+// indices of a decode session; a listed index without such a sot gets 0.
+void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B,
+                        const int* index = nullptr);
 
 // Last node of the loop body of the conditional WHILE graph: keep iterating while some stream is still decoding and the
 // step budget is not used up (one thread; it runs after search_streams, so n_done is final for this step).

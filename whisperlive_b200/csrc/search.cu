@@ -13,6 +13,14 @@ struct MaskCtx {
   int eot, no_timestamps, ts_begin, blank;
 };
 
+// The logits rules of stream b: its own (a decode session's state carries them per stream) or the call's.
+__device__ __forceinline__ void stream_rules(const DecodeState& s, const SearchOpts& o, int b, MaskCtx& c, int glen) {
+  const bool own = s.r_mask != nullptr;
+  c.suppress = own ? s.r_mask + (long)b * s.mask_words : o.suppress_mask;
+  c.suppress_blank = (own ? s.r_suppress_blank[b] : o.suppress_blank) && glen == 0;
+  c.max_initial = own ? s.r_max_initial[b] : o.max_initial_ts;
+}
+
 // the rule-based part of the logits processors (everything but the user's suppress list)
 __device__ __forceinline__ bool rule_masked(int t, const MaskCtx& c) {
   if (c.suppress_blank && (t == c.blank || t == c.eot)) return true;
@@ -133,11 +141,9 @@ __global__ void __launch_bounds__(SR_THREADS) search_rows_kernel(DecodeState s, 
   // timestamp rules.  Blank suppression is keyed to the first GENERATED step.
   const int npre = s.pre_n[b], nhist = glen + npre;
   MaskCtx c;
-  c.suppress = o.suppress_mask;
+  stream_rules(s, o, b, c, glen);
   c.first = nhist == 0;
-  c.suppress_blank = o.suppress_blank && glen == 0;
   c.use_ts = s.use_ts[b];
-  c.max_initial = o.max_initial_ts;
   c.eot = v.eot; c.no_timestamps = v.no_timestamps; c.ts_begin = v.ts_begin; c.blank = v.blank;
   const int last = glen > 0 ? hist[glen - 1] : s.pre_last[b];
   const int penult = glen > 1 ? hist[glen - 2] : (glen == 1 ? s.pre_last[b] : s.pre_penult[b]);
@@ -470,7 +476,8 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
     s.hyp_count[b] = hc + nh;
     s.step[b] = step + 1;
     n_newalive = na; n_newhyp = nh;
-    finished = (hc + nh >= o.max_cand || last_step || na == 0) ? 1 : 0;
+    const int max_cand = s.r_max_cand ? s.r_max_cand[b] : o.max_cand;
+    finished = (hc + nh >= max_cand || last_step || na == 0) ? 1 : 0;
   }
   __syncthreads();
   for (int i = 0; i < n_newhyp; ++i) {
@@ -602,11 +609,9 @@ __global__ void __launch_bounds__(256) scripted_logits_kernel(DecodeState s, Sea
     // the rules of search_rows_kernel for this row
     MaskCtx& c = w.c;
     const int npre = s.pre_n[b], nhist = glen + npre;
-    c.suppress = o.suppress_mask;
+    stream_rules(s, o, b, c, glen);
     c.first = nhist == 0;
-    c.suppress_blank = o.suppress_blank && glen == 0;
     c.use_ts = s.use_ts[b];
-    c.max_initial = o.max_initial_ts;
     const int penult = glen > 1 ? hist[glen - 2] : (glen == 1 ? s.pre_last[b] : s.pre_penult[b]);
     const int plast = glen > 0 ? last : s.pre_last[b];
     c.last_is_ts = nhist > 0 && plast >= v.ts_begin;
@@ -625,10 +630,14 @@ void scripted_logits(cudaStream_t st, const DecodeState& s, const SearchOpts& o,
   note_launch(1);
 }
 
-__global__ void __launch_bounds__(256) scripted_no_speech_kernel(DecodeState s, VocabIds v, SearchScript sc) {
-  const int b = blockIdx.x, tid = threadIdx.x;
+__global__ void __launch_bounds__(256) scripted_no_speech_kernel(DecodeState s, VocabIds v, SearchScript sc,
+                                                                 const int* __restrict__ index) {
+  const int b = index ? index[blockIdx.x] : blockIdx.x, tid = threadIdx.x;
   const int sot = s.sot_index[b];
-  if (sot < 0 || sot >= s.prompt_len[b] - 1) return;
+  if (sot < 0 || sot >= s.prompt_len[b] - 1) {
+    if (index && tid == 0) s.no_speech[b] = 0.f;   // a session index: clear what its previous stream left
+    return;
+  }
   __shared__ ScriptRow w;
   __shared__ float red[2 * 8];
   if (tid == 0) {
@@ -648,8 +657,9 @@ __global__ void __launch_bounds__(256) scripted_no_speech_kernel(DecodeState s, 
   }
 }
 
-void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B) {
-  scripted_no_speech_kernel<<<B, 256, 0, st>>>(s, v, sc);
+void scripted_no_speech(cudaStream_t st, const DecodeState& s, const VocabIds& v, const SearchScript& sc, int B,
+                        const int* index) {
+  scripted_no_speech_kernel<<<B, 256, 0, st>>>(s, v, sc, index);
   WL_CUDA(cudaGetLastError());
   note_launch(1);
 }
@@ -723,8 +733,9 @@ void decode_init(cudaStream_t st, const DecodeState& s, const SearchOpts& o, con
 // live beam there; greedy), or for a sampling stream the alive row with the highest cum (lowest row on ties).  A finished
 // stream reports the hypothesis wl_session_collect would put first: the best cum / len^length_penalty, lowest slot on
 // ties (emit_hyps' stable sort), and its whole hypothesis table, so the host can rank it with the host's own powf (the
-// device's may differ in the last bit for a penalty other than 0 or 1).  Reads the decode state only.
-__global__ void __launch_bounds__(128) session_peek_kernel(DecodeState s, SearchOpts o, float length_penalty,
+// device's may differ in the last bit for a penalty other than 0 or 1).  The penalty is the stream's own when the state
+// carries per-stream rules.  Reads the decode state only.
+__global__ void __launch_bounds__(128) session_peek_kernel(DecodeState s, SearchOpts o, float session_length_penalty,
                                                            const int* __restrict__ index, int* __restrict__ out) {
   const int b = index[blockIdx.x], tid = threadIdx.x;
   const int Kr = o.rows_per_stream, row0 = b * Kr;
@@ -737,6 +748,7 @@ __global__ void __launch_bounds__(128) session_peek_kernel(DecodeState s, Search
     float cum;
     const int* tok;
     if (fin) {
+      const float length_penalty = s.r_length_penalty ? s.r_length_penalty[b] : session_length_penalty;
       const int cnt = min(s.hyp_count[b], MAX_HYPS);
       int best = -1;
       float bs = 0.f;

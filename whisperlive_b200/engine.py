@@ -13,7 +13,7 @@ import os
 import threading
 import weakref
 from dataclasses import dataclass, field
-from typing import Dict, List, Optional, Sequence, Tuple, Union
+from typing import Any, Dict, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -974,6 +974,11 @@ class B200Whisper:
         return {1: "classic", 2: "pingpong"}[v.value]
 
 
+# the generate keywords a stream may bring to a decode session of its own (DecodeSession.admit(rules=...))
+STREAM_RULE_KEYS = ("suppress_tokens", "suppress_blank", "max_initial_timestamp_index", "length_penalty", "patience",
+                    "beam_size")
+
+
 class DecodeSession:
     """Step-level continuous batching on one engine context (``include/wlb200.h``: ``wl_session_*``).
 
@@ -1018,7 +1023,8 @@ class DecodeSession:
             max_initial_timestamp_index=int(max_initial_timestamp_index), sampling_topk=1, sampling_temperature=1.0, seed=0,
             suppress_tokens=_lib.ptr(self._sup, C.c_int32) if len(self._sup) else None, n_suppress=len(self._sup),
             use_cuda_graph=int(engine.use_cuda_graph), max_length_per_stream=None, prefill=1)
-        self._held: Dict[int, EncoderOutput] = {}     # index -> the encoder view its stream decodes against
+        self._held: Dict[int, Any] = {}               # index -> the encoder view its stream decodes against
+        self.scripted = False
         self._finished: List[int] = []
         self.steps = 0
         self.runs = 0
@@ -1027,7 +1033,24 @@ class DecodeSession:
             rc = engine.lib.wl_session_open(engine.ctx, C.byref(self._opts), self.capacity)
             _lib.check(engine.lib, engine.ctx, rc, "wl_session_open")
 
+    def script(self, script: Optional[Tuple[int, int]]) -> None:
+        """Test hook (``wl_test_session_script``): decode the streams admitted from now on over the scripted logits
+        ``(seed, pattern)`` of ``B200Whisper.test_search`` instead of the decoder; None goes back.  Only while nothing
+        is in flight."""
+        eng = self.engine
+        sc = None if script is None else _lib.WlSearchScript(seed=int(script[0]) & 0xFFFFFFFF, pattern=int(script[1]))
+        with eng._lock:
+            rc = eng.lib.wl_test_session_script(eng.ctx, None if sc is None else C.byref(sc))
+            _lib.check(eng.lib, eng.ctx, rc, "wl_test_session_script")
+        self.scripted = script is not None
+
     # -- bookkeeping -------------------------------------------------------------------------------
+    supports_rules = True            # admit(rules=...): per-stream logits rules
+
+    @property
+    def beam_size(self) -> int:
+        return int(self._opts.beam_size)
+
     @property
     def live(self) -> int:
         """streams admitted and not yet collected"""
@@ -1039,14 +1062,20 @@ class DecodeSession:
     # -- admission ---------------------------------------------------------------------------------
     def admit(self, features: Sequence[EncoderOutput], prompts: Sequence[Sequence[int]], max_lengths: Sequence[int],
               indices: Optional[Sequence[int]] = None,
-              sampling: Optional[Sequence[Optional[Tuple[float, int, int, int]]]] = None) -> List[int]:
+              sampling: Optional[Sequence[Optional[Tuple[float, int, int, int]]]] = None,
+              rules: Optional[Sequence[Optional[dict]]] = None) -> List[int]:
         """Admit one stream per (single-stream encoder view, prompt, max_length); returns the indices they decode in.
-        ``sampling``: per stream None (the session's search) or ``(temperature, num_hypotheses, seed, noise_key)``."""
+        ``sampling``: per stream None (the session's search) or ``(temperature, num_hypotheses, seed, noise_key)``.
+        ``rules``: per stream None (the session's options) or a dict of ``generate`` keywords the stream decodes under
+        instead -- ``suppress_tokens``, ``suppress_blank``, ``max_initial_timestamp_index``, ``length_penalty``,
+        ``patience`` (missing keys take ``generate``'s defaults) and optionally ``beam_size``, which must be the
+        session's.  ``features`` entries may be None when the session runs on scripted logits (``script``)."""
         n = len(prompts)
         if n == 0:
             return []
-        if len(features) != n or len(max_lengths) != n or (sampling is not None and len(sampling) != n):
-            raise ValueError("admit: features / prompts / max_lengths / sampling differ in length")
+        if len(features) != n or len(max_lengths) != n or (sampling is not None and len(sampling) != n) or (
+                rules is not None and len(rules) != n):
+            raise ValueError("admit: features / prompts / max_lengths / sampling / rules differ in length")
         free = self.free_indices()
         if indices is None:
             if n > len(free):
@@ -1054,6 +1083,9 @@ class DecodeSession:
             indices = free[:n]
         slots = []
         for f in features:
+            if f is None and self.scripted:
+                slots.append(0)
+                continue
             if not isinstance(f, EncoderOutput) or len(f) != 1:
                 raise TypeError("admit: every stream needs its own single-stream EncoderOutput view")
             slots.append(int(f.slots[0]))
@@ -1071,11 +1103,26 @@ class DecodeSession:
                 t, nh, seed, key = sp
                 q.sample, q.num_hypotheses, q.temperature = 1, int(nh), float(t)
                 q.seed, q.noise_key = int(seed) & 0xFFFFFFFF, int(key)
+        rl = (_lib.WlStreamRules * n)()
+        keep = []                                      # the suppress arrays the structs point into
+        for q, r in zip(rl, rules if rules is not None else [None] * n):
+            if r is not None:
+                unknown = set(r) - set(STREAM_RULE_KEYS)
+                if unknown:
+                    raise ValueError(f"admit: {sorted(unknown)} cannot differ from stream to stream in a decode session")
+                sup = np.asarray(sorted({int(t) for t in (r.get("suppress_tokens", (-1,)) or ()) if t >= 0}), dtype=np.int32)
+                keep.append(sup)
+                q.rules, q.beam_size = 1, int(r.get("beam_size", 0))
+                q.patience, q.length_penalty = float(r.get("patience", 1)), float(r.get("length_penalty", 1))
+                q.suppress_blank = int(bool(r.get("suppress_blank", True)))
+                q.max_initial_timestamp_index = int(r.get("max_initial_timestamp_index", 50))
+                q.suppress_tokens = _lib.ptr(sup, C.c_int32) if len(sup) else None
+                q.n_suppress = len(sup)
         eng = self.engine
         with eng._lock:
             rc = eng.lib.wl_session_admit_ex(eng.ctx, n, _lib.ptr(idx, C.c_int32), _lib.ptr(sl, C.c_int32),
                                              _lib.ptr(flat, C.c_int32), _lib.ptr(off, C.c_int32), _lib.ptr(ml, C.c_int32),
-                                             search if sampling is not None else None)
+                                             search if sampling is not None else None, rl if rules is not None else None)
             _lib.check(eng.lib, eng.ctx, rc, "wl_session_admit")
         for i, f, sp in zip(idx.tolist(), features, specs):
             self._held[i] = f

@@ -141,6 +141,29 @@ class BatchRequest:
         return kw
 
 
+@dataclass
+class FileRequest:
+    """One ``BatchedInferencePipeline`` file decoded by the running loop (``BatchedInferencePipeline(model,
+    scheduler=...)``): ``run`` holds its speech chunks (``transcriber._ChunkRun``).  Its chunks hold at most
+    ``max_share`` of the decode indices, and none is admitted while a live request waits.  ``settled`` receives the
+    segments in chunk order as chunks settle; ``future`` is set when the file is done, failed (``error``) or was
+    cancelled; ``steps`` holds every chunk's token steps."""
+    run: Any
+    max_share: float = 0.5
+    future: threading.Event = field(default_factory=threading.Event)
+    error: Optional[Exception] = None
+    cancelled: bool = False
+    settled: Settled = field(default_factory=Settled)
+    admitted: threading.Event = field(default_factory=threading.Event)
+    steps: List[int] = field(default_factory=list)
+    submitted_at: float = 0.0
+    finished_at: float = 0.0
+
+    def cancel(self) -> None:
+        """The scheduler takes the file's chunks out of the loop at its next round boundary."""
+        self.cancelled = True
+
+
 class EmbeddingRequest:
     """A speaker-embedding request (``RoundScheduler.embed``): ``wait()`` returns the [256] float32 vector or raises the
     error of the call that failed it."""
@@ -173,6 +196,7 @@ class RoundScheduler:
         self.linger_s = (batch_window_ms if linger_ms is None else linger_ms) / 1000.0
         self._inbox: Deque[BatchRequest] = collections.deque()
         self._embeds: List[EmbeddingRequest] = []
+        self._files: List[FileRequest] = []
         self._cv = threading.Condition()
         self._stop = False
         self._thread: Optional[threading.Thread] = None
@@ -182,12 +206,15 @@ class RoundScheduler:
         self.max_in_flight = 0
         self.admitted_mid_flight = 0   # streams that joined while others were already decoding
         self.embedding_calls = 0
+        self.files_in_flight = 0       # batched files the owner thread holds (admitted, not yet finished or dropped)
+        self.rule_admissions = 0       # streams that joined the decode loop with logits rules of their own
 
     # ------------------------------------------------------------------ client side
-    def submit(self, request: BatchRequest) -> None:
+    def submit(self, request) -> None:
+        """Queue a ``BatchRequest`` (a live chunk or an upload) or a ``FileRequest`` (a batched file's chunks)."""
         request.submitted_at = time.monotonic()
         with self._cv:
-            self._inbox.append(request)
+            (self._files if isinstance(request, FileRequest) else self._inbox).append(request)
             self._cv.notify()
 
     def embed(self, audio: np.ndarray) -> EmbeddingRequest:
@@ -218,7 +245,7 @@ class RoundScheduler:
     def _take(self, room: int, block: bool) -> List[BatchRequest]:
         with self._cv:
             if block:
-                while not self._inbox and not self._embeds and not self._stop:
+                while not self._inbox and not self._embeds and not self._files and not self._stop:
                     self._cv.wait(timeout=0.5)
                 if self.linger_s > 0 and self._inbox and len(self._inbox) < room and not self._stop:
                     end = time.monotonic() + self.linger_s      # idle engine, first request: optionally wait for company
@@ -235,15 +262,21 @@ class RoundScheduler:
     def _owner_loop(self) -> None:
         session = self.transcriber.open_session() if hasattr(self.transcriber, "open_session") else _OneShotSession(self.transcriber)
         in_flight: Dict[int, BatchRequest] = {}
+        files: Dict[int, FileRequest] = {}
+        self._rules_before = 0         # rule admissions of sessions replaced after a failed round
         while True:
             with self._cv:
-                if self._stop and not in_flight and not self._inbox and not self._embeds:
+                if self._stop and not in_flight and not files and not self._inbox and not self._embeds and not self._files:
                     close = getattr(session, "close", None)
                     if close is not None:
                         close()             # hands the engine's decode session back
                     return
-            room = self.capacity - len(in_flight)
-            new = self._take(room, block=not in_flight) if room > 0 else []
+            # a file's chunks take indices (and encoder slots) from the same capacity as the live streams
+            room = self.capacity - len(in_flight) - (session.file_streams() if files else 0)
+            new = self._take(room, block=not in_flight and not files) if room > 0 else []
+            self._admit_files(session, files)
+            if hasattr(session, "live_waiting"):
+                session.live_waiting = len(self._inbox) > 0     # live requests first: no new chunk while one waits
             for r in [r for r in new if r.cancelled]:
                 new.remove(r)
                 self._finish(r, None, None, RequestCancelled("request cancelled before admission"))
@@ -263,7 +296,9 @@ class RoundScheduler:
             self._answer_embeddings()
             self.max_in_flight = max(self.max_in_flight, len(in_flight))
             self._drop_cancelled(session, in_flight)
-            if not in_flight:
+            self._drop_cancelled_files(session, files)
+            self.files_in_flight = len(files)
+            if not in_flight and not files:
                 continue
             step = self.step_tokens > 0 and hasattr(session, "step_round")
             try:
@@ -277,6 +312,11 @@ class RoundScheduler:
                 for h, r in list(in_flight.items()):
                     self._finish(r, None, None, e)
                 in_flight.clear()
+                for r in files.values():
+                    self._finish_file(r, e)
+                files.clear()
+                self.files_in_flight = 0
+                self._rules_before += getattr(session, "rule_admissions", 0)
                 session = self.transcriber.open_session() if hasattr(self.transcriber, "open_session") else _OneShotSession(self.transcriber)
                 continue
             for entry in session.pop_finished():
@@ -291,6 +331,50 @@ class RoundScheduler:
             if step:
                 self._publish_partials(session, in_flight)
             self._publish_settled(session, in_flight)
+            self._publish_files(session, files)
+            self.files_in_flight = len(files)
+            self.rule_admissions = self._rules_before + getattr(session, "rule_admissions", 0)
+
+    # ------------------------------------------------------------------ batched files
+    def _admit_files(self, session, files: Dict[int, FileRequest]) -> None:
+        with self._cv:
+            new, self._files = self._files, []
+        for r in new:
+            if r.cancelled:
+                self._finish_file(r, RequestCancelled("request cancelled before admission"))
+            elif not hasattr(session, "add_file"):
+                self._finish_file(r, NotImplementedError("this transcriber cannot decode batched files in its loop"))
+            else:
+                files[session.add_file(r.run, r.max_share, capacity=self.capacity)] = r
+                r.admitted.set()
+
+    def _drop_cancelled_files(self, session, files: Dict[int, FileRequest]) -> None:
+        for h, r in [(h, r) for h, r in files.items() if r.cancelled]:
+            del files[h]
+            try:
+                session.drop_file(h)
+            except Exception as e:
+                log.error("cancel of a file failed: %s", e)
+            self._finish_file(r, RequestCancelled("request cancelled"))
+
+    def _publish_files(self, session, files: Dict[int, FileRequest]) -> None:
+        for h, r in list(files.items()):
+            segs = session.file_segments(h, len(r.settled))
+            if segs:
+                r.settled.extend(segs)
+            if session.file_done(h):
+                r.steps = list(session.files[h].steps)
+                err = session.file_error(h)
+                session.drop_file(h)
+                del files[h]
+                self._finish_file(r, err)
+
+    def _finish_file(self, r: FileRequest, error) -> None:
+        r.error = error
+        r.finished_at = time.monotonic()
+        r.future.set()
+        r.settled.event.set()
+        r.admitted.set()
 
     def _announce_admitted(self, session, admitted) -> None:
         """``info`` (language resolved) for the admitted requests that want segments, then their ``admitted`` event.  A

@@ -33,6 +33,7 @@ from typing import Any, Dict, Iterable, List, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
+from .engine import STREAM_RULE_KEYS as _RULE_KEYS   # the keywords a stream may bring to a decode session of its own
 from .tokenizer import LANGUAGE_CODES, Tokenizer
 
 logger = logging.getLogger("whisperlive_b200")
@@ -327,6 +328,11 @@ class _StreamJob:
         o = self.opt
         return dict(self._shared_kwargs(), beam_size=o.beam_size, patience=o.patience, num_hypotheses=1)
 
+    def stream_rules(self) -> dict:
+        """The logits rules this stream decodes under when it joins a decode session opened with other options."""
+        skw = self.session_kwargs()
+        return {k: skw[k] for k in _RULE_KEYS if k in skw}
+
     def accept(self, result) -> bool:
         """Record one decode; True when the window is settled (else retry at the next temperature)."""
         o = self.opt
@@ -476,11 +482,12 @@ class _StreamJob:
 
 # --------------------------------------------------------------------------- rounds
 class _Entry:
-    __slots__ = ("job", "window", "state", "parent", "index", "handle", "prepared", "error")
+    __slots__ = ("job", "window", "state", "parent", "index", "handle", "prepared", "error", "file")
 
     def __init__(self, job, handle, prepared=None):
         self.job, self.handle, self.prepared = job, handle, prepared
         self.window, self.state, self.parent, self.index, self.error = None, "window", None, -1, None
+        self.file: Optional["_FileRun"] = None        # the batched file this chunk belongs to (None: a live stream)
 
 
 class _EncGroup:
@@ -520,7 +527,13 @@ class TranscribeSession:
         self._dsess = None
         self._dsess_key: Optional[str] = None
         self._running: Dict[int, _Entry] = {}
+        self._dsess_files = False            # the open decode session was opened for a batched file's chunks
         self.admitted_steps: List[int] = []   # session step count at each admission (tests: > 0 = joined a running loop)
+        # batched files (add_file): their chunks enter as entries, at most max_share of the indices each, never while
+        # a live stream waits (live_waiting: set by a scheduler whose inbox holds live requests)
+        self.files: Dict[int, "_FileRun"] = {}
+        self.live_waiting = False
+        self.rule_admissions = 0             # streams that joined the decode session with logits rules of their own
 
     # -- admission -------------------------------------------------------------------------------
     def add_job(self, job: _StreamJob, prepared: Optional[dict] = None) -> int:
@@ -655,9 +668,11 @@ class TranscribeSession:
     def round(self) -> None:
         """Window-level round: encode, ONE generate call per option set run to completion, settle."""
         self.rounds += 1
+        self._feed_files()
         self._encode_pending()
         settled = self._generate_groups([e for e in self.entries if e.state == "decode"])
         self._settle(settled)
+        self._finalise_files()
 
     def step_round(self, max_steps: int = 16) -> None:
         """Token-step-level round (N2): the streams whose windows are ready JOIN the decode loop that is already running
@@ -676,9 +691,10 @@ class TranscribeSession:
             return self.round()
         tm = getattr(m, "last_timing", None) or {}
         self.rounds += 1
+        self._feed_files()
         self._encode_pending()
         one_shot: List[_Entry] = []
-        joining: List[Tuple[_Entry, int, Optional[tuple]]] = []
+        joining: List[Tuple[_Entry, int, Optional[tuple], Optional[dict]]] = []
         waiting = [e for e in self.entries if e.state == "decode"]
         for e in waiting:
             try:
@@ -694,32 +710,44 @@ class TranscribeSession:
                     ds.close()
                 ds = self._dsess = m.model.open_decode_session(**skw)
                 self._dsess_key = key
+                self._dsess_files = e.file is not None
+            rules = None
+            if key != self._dsess_key and (e.file is not None or self._dsess_files) and _rules_fit(ds, skw):
+                # a file's chunk in a live session, or a live stream in a session a file opened: the stream joins the
+                # running loop with its own logits rules (DecodeSession.admit(rules=...)) instead of waiting for it to drain
+                rules = e.job.stream_rules()
             spec = None
             if kw.get("beam_size", 1) == 1 and kw.get("sampling_topk", 1) != 1 and kw.get("sampling_temperature", 0) > 0:
                 # a session model without per-stream sampling has no rows_per_stream: its rungs stay one-shot
-                if key != self._dsess_key or kw["num_hypotheses"] > getattr(ds, "rows_per_stream", 0):
+                if (key != self._dsess_key and rules is None) or kw["num_hypotheses"] > getattr(ds, "rows_per_stream", 0):
                     one_shot.append(e)
                     continue
                 spec = (kw["sampling_temperature"], kw["num_hypotheses"],
                         session_noise_seed(e.handle, e.job.seek, e.job.temp_idx), 0)
-            if key != self._dsess_key or len(joining) >= len(ds.free_indices()):
+            if (key != self._dsess_key and rules is None) or len(joining) >= len(ds.free_indices()):
                 continue                                   # next step_round: the loop has to drain / free an index first
-            joining.append((e, kw["max_length"], spec))
+            joining.append((e, kw["max_length"], spec, rules))
         if joining:                                        # ONE admission = one batched prefill pass for all of them
             ds = self._dsess
-            specs = [sp for _, _, sp in joining]
+            specs = [sp for _, _, sp, _ in joining]
+            rls = [r for _, _, _, r in joining]
+            extra = {}
+            if any(sp is not None for sp in specs):
+                extra["sampling"] = specs
+            if any(r is not None for r in rls):
+                extra["rules"] = rls
             try:
-                idxs = ds.admit([e.job.enc for e, _, _ in joining], [e.job.prompt for e, _, _ in joining],
-                                [ml for _, ml, _ in joining],
-                                **({"sampling": specs} if any(sp is not None for sp in specs) else {}))
+                idxs = ds.admit([e.job.enc for e, _, _, _ in joining], [e.job.prompt for e, _, _, _ in joining],
+                                [ml for _, ml, _, _ in joining], **extra)
             except Exception as ex:
-                for e, _, _ in joining:
+                for e, _, _, _ in joining:
                     self._fail(e, ex)
                 idxs = []
-            for idx, (e, _, _) in zip(idxs, joining):
+            for idx, (e, _, _, r) in zip(idxs, joining):
                 e.state = "running"
                 self._running[idx] = e
                 self.admitted_steps.append(getattr(ds, "steps", 0))
+                self.rule_admissions += r is not None
         settled = self._generate_groups(one_shot)
         ds = self._dsess
         if ds is not None and ds.live:
@@ -748,6 +776,7 @@ class TranscribeSession:
                 except Exception as ex:
                     self._fail(e, ex)
         self._settle(settled)
+        self._finalise_files()
 
     def close(self) -> None:
         if self._dsess is not None:
@@ -811,6 +840,97 @@ class TranscribeSession:
             e.parent.done_one()
             e.parent = None
         self.entries.remove(e)
+
+    # -- batched files: a file's speech chunks as streams of this session ------------------------------------
+    def add_file(self, run: "_ChunkRun", max_share: float = 0.5, capacity: Optional[int] = None) -> int:
+        """Take the chunks of one ``BatchedInferencePipeline`` file (``run``); they enter as indices free up, at most
+        ``max_share`` of ``capacity`` streams at once (a scheduler's capacity; never more than the engine's
+        ``max_streams``), and never while a live stream waits.  Returns the file's handle: ``file_segments`` /
+        ``file_done`` / ``file_error`` / ``drop_file``."""
+        cap = int(getattr(self.m.model, "max_streams", 0) or 0) or 8
+        if capacity is not None:
+            cap = min(cap, int(capacity))
+        h = self._next_handle
+        self._next_handle += 1
+        self.files[h] = _FileRun(run, h, max(1, int(max_share * cap)))
+        return h
+
+    def file_streams(self) -> int:
+        """Streams the files' chunks count for: those in the session, and decoded ones that still hold an encoder slot
+        (word timestamps on an engine whose outputs cannot be joined keep it until the chunk is finalised)."""
+        return sum(f.held() for f in self.files.values())
+
+    def file_segments(self, handle: int, n: int) -> List[Segment]:
+        """The file's finalised segments after the first ``n``, in chunk order, ids counted on, original time axis."""
+        return self.files[handle].segments[n:]
+
+    def file_done(self, handle: int) -> bool:
+        return self.files[handle].done
+
+    def file_error(self, handle: int) -> Optional[Exception]:
+        return self.files[handle].error
+
+    def drop_file(self, handle: int) -> None:
+        """Forget a finished file, or cancel one in flight: its chunks leave the decode session and their slots go back."""
+        f = self.files.pop(handle, None)
+        if f is None:
+            return
+        for e in list(f.active):
+            self.cancel(e.handle)
+        for e in f.decoded.values():
+            if e.parent is not None:
+                e.parent.done_one()
+                e.parent = None
+        f.active, f.decoded = [], {}
+
+    def _feed_files(self) -> None:
+        if not self.files:
+            return
+        if self.live_waiting or any(e.file is None and e.state in ("window", "decode") for e in self.entries):
+            return                                       # live streams first
+        for f in self.files.values():
+            n = len(f.run.features)
+            while f.error is None and f.next_chunk < n and f.held() < f.limit:
+                job = _ChunkJob(f.run, f.next_chunk)
+                f.next_chunk += 1
+                f.run.jobs.append(job)
+                self.add_job(job)
+                e = self.entries[-1]
+                e.file = f
+                f.active.append(e)
+
+    def _finalise_files(self) -> None:
+        """Segments and words of every file's decoded chunks, in chunk order: the word-timestamp carry-over
+        (``last_speech_timestamp``) runs through them as through the one-shot pipeline's groups."""
+        from . import vad as vad_mod
+        sr = self.m.feature_extractor.sampling_rate
+        for f in self.files.values():
+            for e in list(f.active):
+                if e.state == "done" and e.error is not None and f.error is None:
+                    f.error = e.error
+            while f.error is None and f.next_final in f.decoded:
+                e = f.decoded.pop(f.next_final)
+                j = e.job
+                try:
+                    j.finish_window()
+                except Exception as ex:
+                    f.error = ex
+                j.enc = None
+                if e.parent is not None:
+                    e.parent.done_one()
+                    e.parent = None
+                f.next_final += 1
+                f.steps.append(j.steps)
+                if f.error is not None:
+                    break
+                for s in j.segments:
+                    f.n_ids += 1
+                    s.id = f.n_ids
+                f.segments.extend(restore_speech_timestamps(j.segments, f.run.clips, sr, vad_mod))
+            if f.error is not None:
+                for e in list(f.active):
+                    self.cancel(e.handle)
+                f.active = []
 
     # -- the three parts of a round -----------------------------------------------------------------
     def _encode_pending(self) -> None:
@@ -896,6 +1016,17 @@ class TranscribeSession:
             settled = []
         for e in settled:
             j = e.job
+            if e.file is not None:
+                # a file's chunk: its segments and words are finalised in chunk order (_finalise_files); the encoder
+                # slot goes back now unless word timestamps still need it (an engine whose outputs cannot be joined)
+                if not (j.opt.word_timestamps and j._align_result is None):
+                    j.enc = None
+                    e.parent.done_one()
+                    e.parent = None
+                e.file.decoded[j.index] = e
+                e.file.active.remove(e)
+                e.state = "done"
+                continue
             try:
                 j.finish_window()
                 if j.single_window:
@@ -933,6 +1064,43 @@ def session_noise_seed(handle: int, seek: int, rung: int) -> int:
     window's ``seek`` (frames) and the rung's index in the temperature ladder.  A stream's draws therefore depend only
     on the stream itself -- not on which streams share its rounds or when it arrived."""
     return _lowbias32(_lowbias32(_lowbias32(handle) ^ (seek & 0xFFFFFFFF)) ^ (rung & 0xFFFFFFFF))
+
+
+ENGINE_MAX_INITIAL_TIMESTAMP_INDEX = 50     # generate's default, which BatchedInferencePipeline's chunks decode under
+
+
+def _rules_fit(ds, skw: dict) -> bool:
+    """Whether a stream with session options ``skw`` can join the open session ``ds`` with rules of its own: the session
+    takes per-stream rules and decodes with the same beam width (rows per stream are fixed per session)."""
+    if not getattr(ds, "supports_rules", False):
+        return False
+    if any(skw.get(k, d) != d for k, d in (("repetition_penalty", 1), ("no_repeat_ngram_size", 0))):
+        return False
+    return int(skw.get("beam_size", 5)) == int(ds.beam_size) and int(skw.get("num_hypotheses", 1)) == 1
+
+
+class _FileRun:
+    """A batched file in a ``TranscribeSession``: which chunks have started, are decoding, wait for an earlier chunk,
+    or are finalised."""
+
+    def __init__(self, run: "_ChunkRun", handle: int, limit: int):
+        self.run, self.handle, self.limit = run, handle, int(limit)   # limit: streams the file may hold at once
+        self.next_chunk = 0                      # next chunk to enter the session
+        self.active: List[_Entry] = []           # chunks in the session, not yet decoded
+        self.decoded: Dict[int, _Entry] = {}     # chunk index -> decoded chunk waiting for the earlier ones
+        self.next_final = 0                      # next chunk to finalise
+        self.segments: List[Segment] = []
+        self.n_ids = 0
+        self.steps: List[int] = []
+        self.error: Optional[Exception] = None
+
+    @property
+    def done(self) -> bool:
+        return self.error is not None or self.next_final >= len(self.run.features)
+
+    def held(self) -> int:
+        """Chunks in the session, plus decoded chunks waiting for an earlier one that still hold an encoder slot."""
+        return len(self.active) + sum(1 for e in self.decoded.values() if e.parent is not None)
 
 
 def _join_encoded(views: List[Any]):
@@ -1553,6 +1721,22 @@ class _ChunkJob:
                     return_scores=True, return_no_speech_prob=True, sampling_temperature=o.temperatures[0],
                     repetition_penalty=o.repetition_penalty, no_repeat_ngram_size=o.no_repeat_ngram_size)
 
+    temp_idx = 0      # one rung
+
+    def session_kwargs(self) -> dict:
+        """Options of a decode session opened for this chunk (``TranscribeSession.step_round``)."""
+        kw = self.generate_kwargs()
+        for k in ("max_length", "sampling_temperature"):
+            kw.pop(k)
+        return dict(kw, num_hypotheses=1)
+
+    def stream_rules(self) -> dict:
+        """What the chunk decodes under when it joins a session opened with other options."""
+        o = self.opt
+        return dict(beam_size=o.beam_size, patience=o.patience, length_penalty=o.length_penalty,
+                    suppress_blank=o.suppress_blank, suppress_tokens=o.suppress_tokens,
+                    max_initial_timestamp_index=ENGINE_MAX_INITIAL_TIMESTAMP_INDEX)
+
     def accept(self, result) -> bool:
         n = len(result.sequences_ids[0])
         self.result = result
@@ -1604,10 +1788,17 @@ class BatchedInferencePipeline:
     (``word_timestamps``), driven by ``TranscribeSession`` rounds.  The calls are one-shot, so a ``TranscribeSession``
     with an open step-level decode session on the same model keeps its streams."""
 
-    def __init__(self, model: "B200WhisperModel"):
+    def __init__(self, model: "B200WhisperModel", scheduler=None, max_share: float = 0.5):
+        """``scheduler``: a running ``RoundScheduler`` on the same model.  Its owner thread then decodes the file's
+        chunks as streams of its running decode loop, beside the live connections, instead of one-shot calls on the
+        caller's thread: a chunk enters as soon as an index is free (at most ``max_share`` of the indices, and live
+        requests first), and the segments come out in chunk order as chunks settle.  The result is the same."""
         self.model = model
+        self.scheduler = scheduler
+        self.max_share = float(max_share)
         self.resident_features = True        # False: features always go through the host (tests compare the paths)
         self.group_steps: List[List[int]] = []   # token steps of every chunk, per group of the last transcribe call
+        self.last_request = None             # the FileRequest of the last file sent to the scheduler
 
     def transcribe(self, audio, language: Optional[str] = None, task: str = "transcribe", log_progress: bool = False,
                    beam_size: int = 5, best_of: int = 5, patience: float = 1, length_penalty: float = 1,
@@ -1668,7 +1859,7 @@ class BatchedInferencePipeline:
             # ONE mel call for every chunk; resident in HBM when the chunks fit one call and nothing needs host values
             cap = int(getattr(m.model, "max_streams", 0) or 0)
             resident = (self.resident_features and hasattr(fe, "batch_resident") and len(audio_chunks) <= cap
-                        and not detect)
+                        and not detect and self.scheduler is None)
             feats = fe.batch_resident(audio_chunks) if resident else fe.batch(audio_chunks)
             features = [f[..., :-1] for f in feats]
 
@@ -1709,7 +1900,38 @@ class BatchedInferencePipeline:
                                  vad_options=vad_parameters, all_language_probs=all_language_probs)
         run = _ChunkRun(m, tokenizer, options, audio_chunks, metadata, features, clip_timestamps)
         self.group_steps = []
+        if self.scheduler is not None:
+            return self._scheduled_segments(run), info
         return self._segments(run, batch_size), info
+
+    def _scheduled_segments(self, run: _ChunkRun):
+        """The file as one request of the scheduler: segments as its chunks settle, in chunk order.  Closing the
+        generator early cancels the chunks still in flight."""
+        if not run.features:
+            return
+        from .scheduler import FileRequest
+        req = self.last_request = FileRequest(run=run, max_share=self.max_share)
+        self.scheduler.submit(req)
+        n = 0
+        try:
+            while True:
+                req.settled.event.clear()
+                segs = req.settled.since(n)
+                if segs:
+                    n += len(segs)
+                    yield from segs
+                    continue
+                if req.future.is_set():
+                    if len(req.settled) > n:
+                        continue
+                    if req.error is not None:
+                        raise req.error
+                    break
+                req.settled.event.wait(1.0)
+        finally:
+            if not req.future.is_set():
+                req.cancel()
+            self.group_steps = [list(req.steps)]
 
     def _segments(self, run: _ChunkRun, batch_size: int):
         """Reference :534-571, one ``TranscribeSession`` run per group; ids count on across groups."""
