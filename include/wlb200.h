@@ -31,7 +31,7 @@
 extern "C" {
 #endif
 
-#define WL_ABI_VERSION 13
+#define WL_ABI_VERSION 14
 
 typedef struct wl_ctx wl_ctx;
 
@@ -143,14 +143,18 @@ int wl_generate(wl_ctx* ctx, const int32_t* slots, int32_t B, const int32_t* pro
  *                      rules[n] (ABI 13; NULL, or rules = 0 for a stream: the session's options) gives a stream its own
  *                      logits rules -- suppress list, suppress_blank, max_initial_timestamp_index -- and its own
  *                      length_penalty and patience (the finished hypotheses that end a beam stream; the ranking of
- *                      wl_session_collect and wl_session_peek).  They live in per-index device tables the captured loop
- *                      reads: admitting a stream with its own rules captures no new graph, and its result does not
- *                      depend on the other streams.  beam_size stays the session's (0 or equal; anything else fails the
- *                      call, like a bad patience, before anything is staged).
+ *                      wl_session_collect and wl_session_peek), and (ABI 14) its own beam_size: 1 .. the session's rows
+ *                      per stream.  A stream of width 1 is wl_generate's greedy search over the session's num_hypotheses
+ *                      rows; a wider one a beam search over its first beam_size rows, the others staying inactive.  They
+ *                      live in per-index device tables the captured loop reads: admitting a stream with its own rules or
+ *                      width captures no new graph, and its result does not depend on the other streams.  A width above
+ *                      the rows per stream, round(beam_size * patience) above 16, or any other bad field fails the call
+ *                      before anything is staged, with the field named.
  *   wl_session_run     runs the device-side token loop over every admitted stream for at most max_steps steps; with
  *                      break_on_finish it also returns as soon as some stream has finished.  done_out[capacity]: 1 for
  *                      indices whose stream is finished and not yet collected.  steps_ran: token steps executed.
- *   wl_session_collect hypotheses of one finished index (outputs like one stream of wl_generate); the index goes idle.
+ *   wl_session_collect hypotheses of one finished index (outputs like one stream of wl_generate at the stream's own
+ *                      search and width); the index goes idle.
  *                      out_ids / out_len / out_score hold the index's own hypothesis count: the sampled stream's
  *                      num_hypotheses, else the session's.
  *   wl_session_peek    the interim hypothesis of n indices (index[n]), for text before a stream finishes: out_ids
@@ -183,8 +187,9 @@ typedef struct wl_stream_search {
 } wl_stream_search;
 typedef struct wl_stream_rules {
   int32_t rules;             /* 0: the session's options (the other fields are ignored); 1: the fields below */
-  int32_t beam_size;         /* 0 or the session's beam_size: rows per stream are fixed per session */
-  float patience;            /* beam search ends with round(beam_size * patience) <= 16 hypotheses */
+  int32_t beam_size;         /* 0: the session's; else 1 (greedy) .. the session's rows per stream (its beam_size, or its
+                                num_hypotheses when its beam_size is 1) */
+  float patience;            /* beam search ends with round(beam_size * patience) <= 16 hypotheses (this stream's width) */
   float length_penalty;
   int32_t suppress_blank;
   int32_t max_initial_timestamp_index;

@@ -12,11 +12,16 @@ Three cases over one engine context and one ``RoundScheduler`` (step-level round
       a time, so the scheduler's rounds wait while a group is decoded.
 
 The file is ``--file-seconds`` of synthetic speech cut into 30 s chunks by ``clip_timestamps`` (no VAD model is
-needed); its decode options are the pipeline's defaults.  Live cycles continue until the file has finished (at least
+needed); its decode options are the pipeline's defaults at beam ``--file-beam`` (default: ``--beam``).  A file beam
+narrower than the live streams' joins their decode loop with that width; each case reports how many times the decode
+session was opened, which counts the drains a waiting chunk needs.  ``--equal-width-only`` restores the admission
+rule before per-stream widths (a chunk joins with rules only at the session's own width), so one build gives both
+arms of a before / after comparison.  Live cycles continue until the file has finished (at least
 ``--cycles``).  Reports the live p50 / p90 chunk latency of each case, the file's audio-s/s in (b) and (c), and the
-card's name and power limit, read in the same run.  Random weights and the synthetic tokenizer; needs a CUDA device.
+card's name, power limit and SM clocks (maximum, and current at setup and after the last case), read in the same run.  Random weights and the synthetic tokenizer; needs a CUDA device.
 
     python tools/batched_live_load.py --model large-v3 --streams 16 --file-seconds 600 --batch-size 16
+    python tools/batched_live_load.py --model large-v3 --streams 16 --file-seconds 600 --beam 5 --file-beam 1
 """
 import argparse
 import json
@@ -41,11 +46,16 @@ def main():
     ap.add_argument("--file-seconds", type=float, default=600.0)
     ap.add_argument("--batch-size", type=int, default=16, help="the file's batch_size (one-shot: chunks per call)")
     ap.add_argument("--max-share", type=float, default=0.5, help="case (b): share of the decode indices the file may hold")
-    ap.add_argument("--beam", type=int, default=5, help="beam of the live chunks and of the file")
+    ap.add_argument("--beam", type=int, default=5, help="beam of the live chunks")
+    ap.add_argument("--file-beam", type=int, default=None, help="beam of the file (default: --beam)")
+    ap.add_argument("--equal-width-only", action="store_true",
+                    help="a chunk joins the open decode session with rules only at the session's own beam width (the "
+                         "admission rule before per-stream widths): the 'before' arm of a comparison in one build")
     ap.add_argument("--cycles", type=int, default=3, help="live cycles per case, at least (more while the file runs)")
     ap.add_argument("--cases", default="abc")
     ap.add_argument("--out", default=None, help="also write the JSON result here")
     args = ap.parse_args()
+    file_beam = args.beam if args.file_beam is None else args.file_beam
 
     import torch
     if not torch.cuda.is_available():
@@ -57,13 +67,17 @@ def main():
     from whisperlive_b200.feature_extractor import FeatureExtractor
     from whisperlive_b200.scheduler import RoundScheduler
     from whisperlive_b200.tokenizer import build_synthetic_tokenizer
+    from whisperlive_b200 import transcriber
     from whisperlive_b200.transcriber import B200WhisperModel, BatchedInferencePipeline
     from whisperlive_b200.weights import random_init
 
+    if args.equal_width_only:
+        fits = transcriber._rules_fit
+        transcriber._rules_fit = lambda ds, skw: fits(ds, skw) and int(skw.get("beam_size", 5)) == int(ds.beam_size)
     dims = dims_for(args.model)
     n = args.streams
     cap = n + args.batch_size                   # the live streams and a whole one-shot group fit the decode capacity
-    eng = B200Whisper(dims, random_init(dims, seed=0), max_streams=cap, max_beam=max(args.beam, 5),
+    eng = B200Whisper(dims, random_init(dims, seed=0), max_streams=cap, max_beam=max(args.beam, file_beam, 5),
                       enc_slots=2 * cap + 2)
     model = B200WhisperModel(args.model, engine=eng, hf_tokenizer=build_synthetic_tokenizer(dims.vocab),
                              feature_extractor=FeatureExtractor(eng, dims.n_mels))
@@ -77,7 +91,14 @@ def main():
     audio = synth.speech_like(args.file_seconds, seed=777)
     n_chunks = int(args.file_seconds // 30)
     clips = [{"start": 30 * sr * i, "end": min(len(audio), 30 * sr * (i + 1))} for i in range(n_chunks)]
-    file_kw = dict(language="en", vad_filter=False, clip_timestamps=clips, batch_size=args.batch_size, beam_size=args.beam)
+    file_kw = dict(language="en", vad_filter=False, clip_timestamps=clips, batch_size=args.batch_size, beam_size=file_beam)
+    opens = [0]
+    open_session = eng.open_decode_session
+
+    def counted_open(*a, **k):
+        opens[0] += 1
+        return open_session(*a, **k)
+    eng.open_decode_session = counted_open
 
     model.transcribe_batch(waves, kws)                       # warm-up, then the batch step the load is sized on
     t0 = time.perf_counter()
@@ -87,7 +108,8 @@ def main():
 
     result = {"card": card(), "model": args.model, "live_streams": n, "offered_load": args.load,
               "arrival_period_ms": round(1000.0 * period, 1), "file_seconds": args.file_seconds, "file_chunks": n_chunks,
-              "batch_size": args.batch_size, "max_share": args.max_share, "decode_capacity": cap, "cases": {}}
+              "batch_size": args.batch_size, "max_share": args.max_share,
+              "live_beam": args.beam, "file_beam": file_beam, "equal_width_only": args.equal_width_only, "decode_capacity": cap, "cases": {}}
     print("setup", json.dumps(result), flush=True)
     lock = threading.Lock()
     for case in args.cases:
@@ -95,6 +117,7 @@ def main():
         sch = RoundScheduler(served, max_batch_size=cap, step_tokens=16)
         sch.start()
         up = {}
+        opens_before = opens[0]
         try:
             live_cycles(sch, waves, kws, period, 1, lambda: True, random.Random(1))     # warm-up cycle
             thread = None
@@ -134,10 +157,12 @@ def main():
                 live["file_mean_chunk_steps"] = round(sum(up["chunk_steps"]) / max(1, len(up["chunk_steps"])), 1)
             live["admitted_mid_flight"] = sch.admitted_mid_flight
             live["rule_admissions"] = sch.rule_admissions
+            live["session_opens"] = opens[0] - opens_before
         finally:
             sch.stop()
         result["cases"][case] = live
         print(case, json.dumps(live), flush=True)
+    result["card_after"] = card()                 # the clock right after the last case
     line = json.dumps(result)
     print(line)
     if args.out:

@@ -31,14 +31,19 @@ sys.path.insert(0, ROOT)
 
 
 def card():
+    """The card's name, power limit, maximum SM clock and the SM clock at the moment of the call."""
     import torch
     name = torch.cuda.get_device_name(0)
+    keys = ("power_limit", "sm_clock_max", "sm_clock")
     try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", "0"],
-                             capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:          # the figure is reported as unknown rather than guessed
-        out = f"unknown ({e})"
-    return {"name": name, "power_limit": out}
+        out = subprocess.run(["nvidia-smi", "--query-gpu=power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader",
+                              "-i", "0"], capture_output=True, text=True, timeout=30).stdout.strip()
+        vals = [v.strip() for v in out.split(",")]
+        if len(vals) != len(keys):
+            raise ValueError(out)
+    except Exception as e:          # the figures are reported as unknown rather than guessed
+        vals = [f"unknown ({e})"] * len(keys)
+    return {"name": name, **dict(zip(keys, vals))}
 
 
 class _Req:

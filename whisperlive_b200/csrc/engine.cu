@@ -81,15 +81,15 @@ static void alloc_decode_state(wl_ctx* c, DecodeState& s) {
   s.nrows = c->mem.alloc<int>(B);
   s.pre_n = c->mem.alloc<int>(B); s.pre_last = c->mem.alloc<int>(B); s.pre_penult = c->mem.alloc<int>(B); s.pre_lts = c->mem.alloc<int>(B);
   s.brk = c->mem.alloc<int>(2);
-  s.r_max_initial = s.r_suppress_blank = s.r_max_cand = nullptr;   // the call's SearchOpts (a session adds its own)
+  s.r_max_initial = s.r_suppress_blank = s.r_max_cand = s.r_beam = nullptr;   // the call's SearchOpts (a session adds its own)
   s.r_length_penalty = nullptr;
   s.r_mask = nullptr;
   s.mask_words = 0;
 }
 
 // Rows of a decode session's per-stream rule table (host shadow Session::rules -> DecodeState::r_*): max initial
-// timestamp index, suppress_blank, max_cand, length penalty (float bits)
-constexpr int RULE_ROWS = 4;
+// timestamp index, suppress_blank, max_cand, length penalty (float bits), beam width
+constexpr int RULE_ROWS = 5;
 
 // ------------------------------------------------------------------------------------------ init
 extern "C" int wl_init(const wl_config* cfg, wl_ctx** out) {
@@ -1456,6 +1456,7 @@ extern "C" int wl_session_open(wl_ctx* c, const wl_gen_opts* o, int32_t capacity
     sd.mask_words = (c->V + 31) / 32 + 1;
     sd.r_max_initial = c->mem.alloc<int>(c->Bm); sd.r_suppress_blank = c->mem.alloc<int>(c->Bm);
     sd.r_max_cand = c->mem.alloc<int>(c->Bm); sd.r_length_penalty = c->mem.alloc<float>(c->Bm);
+    sd.r_beam = c->mem.alloc<int>(c->Bm);
     sd.r_mask = c->mem.alloc<unsigned>((size_t)c->Bm * sd.mask_words);
     ss.idx_dev = c->mem.alloc<int>(c->Bm);
     ss.peek_dev = c->mem.alloc<int>((size_t)c->Bm * PEEK_STRIDE);
@@ -1509,17 +1510,27 @@ extern "C" int wl_session_admit(wl_ctx* c, int32_t n, const int32_t* index, cons
   return wl_session_admit_ex(c, n, index, slots, prompts, prompt_off, max_length, nullptr, nullptr);
 }
 
+// beam width of a stream admitted with these rules (nullptr: none): its own, or 0 for the session's
+static int stream_width(const wl_ctx::Session& ss, const wl_stream_rules* q) {
+  return q && q->rules && q->beam_size ? q->beam_size : ss.K;
+}
+
 // a stream's own logits rules, checked before anything is staged; every message names the field
 static void check_stream_rules(const wl_ctx::Session& ss, int i, const wl_stream_rules& q) {
   WL_CHECK(q.rules == 1, WL_ERR_ARG, "wl_session_admit: stream %d: rules must be 0 or 1, got %d", i, q.rules);
-  WL_CHECK(q.beam_size == 0 || q.beam_size == ss.K, WL_ERR_ARG,
-           "wl_session_admit: stream %d: beam_size %d differs from the session's %d (rows per stream are fixed per session)",
-           i, q.beam_size, ss.K);
+  // a width needs that many rows of the stream's index; a greedy stream runs the session's num_hypotheses rows, as
+  // wl_generate(beam_size = 1) does
+  WL_CHECK(q.beam_size >= 0 && q.beam_size <= ss.Kr, WL_ERR_ARG,
+           "wl_session_admit: stream %d: beam_size %d must be 0 (the session's) or 1 .. %d (rows per stream)", i,
+           q.beam_size, ss.Kr);
+  WL_CHECK(q.beam_size != 1 || ss.NH <= ss.Kr, WL_ERR_ARG,
+           "wl_session_admit: stream %d: beam_size 1 decodes num_hypotheses = %d greedy rows, more than the %d rows per stream",
+           i, ss.NH, ss.Kr);
   WL_CHECK(std::isfinite(q.patience) && q.patience > 0.f, WL_ERR_ARG, "wl_session_admit: stream %d: patience %g must be finite and > 0",
            i, (double)q.patience);
-  char who[64];
-  snprintf(who, sizeof(who), "wl_session_admit: stream %d: patience", i);
-  max_candidates(ss.K, q.patience, who);
+  char who[80];
+  snprintf(who, sizeof(who), "wl_session_admit: stream %d: patience x beam_size", i);
+  max_candidates(stream_width(ss, &q), q.patience, who);
   WL_CHECK(std::isfinite(q.length_penalty), WL_ERR_ARG, "wl_session_admit: stream %d: length_penalty %g is not finite", i,
            (double)q.length_penalty);
   WL_CHECK(q.max_initial_timestamp_index >= 0, WL_ERR_ARG, "wl_session_admit: stream %d: negative max_initial_timestamp_index %d",
@@ -1560,17 +1571,20 @@ extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, c
     stream_meta(c, i, slots[i], prompts + prompt_off[i], prompt_off[i + 1] - prompt_off[i], max_length[i], false,
                 hp.data() + (size_t)index[i] * T_MAX, meta.data(), index[i], cap, nullptr, !ss.script_on);
     const bool sample = search && search[i].sample;
-    search_meta(meta.data(), index[i], cap, sample ? 1 : 0, sample ? search[i].temperature : 0.f, sample ? search[i].seed : 0u,
-                sample ? search[i].noise_key : index[i], sample ? search[i].num_hypotheses : ss.Kr);
     const bool own = rules && rules[i].rules;
+    const int width = stream_width(ss, rules ? rules + i : nullptr);
+    // rows a stream without a beam uses: its samples, or greedy's num_hypotheses (= Kr in a greedy session)
+    search_meta(meta.data(), index[i], cap, sample ? 1 : 0, sample ? search[i].temperature : 0.f, sample ? search[i].seed : 0u,
+                sample ? search[i].noise_key : index[i], sample ? search[i].num_hypotheses : (width == 1 ? ss.NH : ss.Kr));
     const float lp = own ? rules[i].length_penalty : ss.length_penalty;
     int lbits;
     memcpy(&lbits, &lp, 4);
     const int b = index[i];
     rl[0 * cap + b] = own ? rules[i].max_initial_timestamp_index : ss.so.max_initial_ts;
     rl[1 * cap + b] = own ? (rules[i].suppress_blank ? 1 : 0) : ss.so.suppress_blank;
-    rl[2 * cap + b] = own ? max_candidates(ss.K, rules[i].patience, "wl_session_admit") : ss.so.max_cand;
+    rl[2 * cap + b] = own ? max_candidates(width, rules[i].patience, "wl_session_admit") : ss.so.max_cand;
     rl[3 * cap + b] = lbits;
+    rl[4 * cap + b] = width;
     if (own)
       for (int k = 0; k < rules[i].n_suppress; ++k) {
         const int t = rules[i].suppress_tokens[k];
@@ -1599,7 +1613,7 @@ extern "C" int wl_session_admit_ex(wl_ctx* c, int32_t n, const int32_t* index, c
     // the rule tables of the session state (written like the others with what the streams in flight already hold) and
     // each admitted index's suppress mask: its own list, or a copy of the session's
     const DecodeState& sd = ss.ds;
-    void* dst[RULE_ROWS] = {sd.r_max_initial, sd.r_suppress_blank, sd.r_max_cand, sd.r_length_penalty};
+    void* dst[RULE_ROWS] = {sd.r_max_initial, sd.r_suppress_blank, sd.r_max_cand, sd.r_length_penalty, sd.r_beam};
     for (int k = 0; k < RULE_ROWS; ++k) WL_CUDA(cudaMemcpyAsync(dst[k], prules + (size_t)k * cap, cap * 4, cudaMemcpyHostToDevice, st));
     for (int i = 0; i < n; ++i) {
       unsigned* m = sd.r_mask + (size_t)index[i] * nwords;

@@ -153,7 +153,8 @@ struct DecodeState {
   // at admission -- the session's own options for a stream admitted without rules -- and read by the captured loop.
   int* r_max_initial;   // [B] max_initial_timestamp_index
   int* r_suppress_blank;// [B]
-  int* r_max_cand;      // [B] round(beam * patience): finished hypotheses that end a beam stream
+  int* r_beam;          // [B] beam width K_b <= rows_per_stream (1: greedy); a beam stream leaves rows K_b .. Kr-1 inactive
+  int* r_max_cand;      // [B] round(K_b * patience): finished hypotheses that end a beam stream
   float* r_length_penalty; // [B] (session_peek's ranking)
   unsigned* r_mask;     // [B][mask_words] suppress bitmask
   int mask_words;
@@ -167,7 +168,7 @@ struct DecodeState {
 // Options shared by every stream of a call / session.  Whether a stream samples, at what temperature and with which
 // noise is per stream: DecodeState::smode / temp / nseed / nkey / nrows.
 struct SearchOpts {
-  int beam;            // K (1 = greedy, or sampling when the stream's smode says so)
+  int beam;            // K (1 = greedy, or sampling when the stream's smode says so); a session stream's is r_beam
   int rows_per_stream; // Kr
   int max_cand;        // round(K * patience)
   int suppress_blank;

@@ -21,6 +21,11 @@ __device__ __forceinline__ void stream_rules(const DecodeState& s, const SearchO
   c.max_initial = own ? s.r_max_initial[b] : o.max_initial_ts;
 }
 
+// The beam width of stream b: its own (a decode session's state carries it per stream, <= rows_per_stream) or the call's.
+__device__ __forceinline__ int stream_beam(const DecodeState& s, const SearchOpts& o, int b) {
+  return s.r_beam ? s.r_beam[b] : o.beam;
+}
+
 // the rule-based part of the logits processors (everything but the user's suppress list)
 __device__ __forceinline__ bool rule_masked(int t, const MaskCtx& c) {
   if (c.suppress_blank && (t == c.blank || t == c.eot)) return true;
@@ -201,8 +206,11 @@ __global__ void __launch_bounds__(SR_THREADS) search_rows_kernel(DecodeState s, 
 
   // selection keys in place: log-prob (beam / greedy) or log-prob / T + Gumbel noise (sampling); rule e drops text.
   // The noise of row j of a sampling stream is keyed by (seed, noise key, j, step) -- wl_generate: key = batch position.
+  // Only the stream's own 2 K_b candidates: the rounds are sequential, so they are the first 2 K_b entries of the list
+  // the session's width would give, and a narrower stream's row runs fewer rounds instead of the session's 2 K.
   const bool sampling = s.smode[b] != 0;
-  const int NC = (!sampling && o.beam > 1) ? 2 * o.beam : 1;
+  const int K = stream_beam(s, o, b);
+  const int NC = (!sampling && K > 1) ? 2 * K : 1;
   const float temperature = s.temp[b];
   uint32_t gkey = 0;
   if (sampling)
@@ -302,9 +310,10 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
   if (s.done[b]) return;
   const int Kr = o.rows_per_stream, row0 = b * Kr;
   const int P = s.prompt_len[b], fed = s.fed[b];
-  // greedy / sampling: every row is an independent hypothesis, over the stream's own N <= Kr rows (a sampling stream
-  // of a beam session included)
-  const bool independent = o.beam == 1 || s.smode[b] != 0;
+  // greedy / sampling: every row is an independent hypothesis, over the stream's own N <= Kr rows (a sampling or
+  // width-1 stream of a beam session included); otherwise a beam of the stream's own width K <= Kr
+  const int K = stream_beam(s, o, b);
+  const bool independent = K == 1 || s.smode[b] != 0;
   const int N = s.nrows[b];
   __shared__ int sh_hist[MAX_ROWS_PER_STREAM][T_MAX];
   __shared__ short sh_src[MAX_ROWS_PER_STREAM][T_MAX];
@@ -402,8 +411,7 @@ __global__ void __launch_bounds__(128) search_streams_kernel(DecodeState s, Sear
     return;
   }
 
-  // ---- beam search (CT2 walk, see oracle/search.py)
-  const int K = o.beam;
+  // ---- beam search (CT2 walk, see oracle/search.py) over rows 0 .. K-1; rows K .. Kr-1 stay inactive
   const int n_alive = s.n_alive[b];
   const int pos_old = s.pos[row0];
   const int len_old = s.gen_len[row0];
@@ -692,7 +700,7 @@ __global__ void decode_init_kernel(DecodeState s, SearchOpts o, VocabIds v, int 
   const int fed0 = (prefilled && s.force_len[b] == 0) ? P - 1 : 0;
   // independent sampling rows all continue from the prompt cache of row 0 (what search_streams does when the feeding
   // reaches the last prompt token); a stream that uses N < Kr rows leaves rows N .. Kr-1 inactive for its whole life
-  const bool fan_out = (o.beam == 1 || s.smode[b] != 0) && s.force_len[b] == 0 && fed0 == P - 1;
+  const bool fan_out = (stream_beam(s, o, b) == 1 || s.smode[b] != 0) && s.force_len[b] == 0 && fed0 == P - 1;
   const int N = fan_out ? s.nrows[b] : 1;
   if (tid < Kr) {
     const int r = row0 + tid;

@@ -999,7 +999,8 @@ class DecodeSession:
     The session's own search is beam or greedy.  A stream may instead be admitted for Gumbel-max sampling (a
     temperature-fallback rung): ``admit(..., sampling=[(temperature, num_hypotheses, seed, noise_key), ...])`` decodes it
     over ``num_hypotheses <= rows_per_stream`` independent rows with exactly the draws ``generate(seed=seed)`` gives the
-    stream at batch position ``noise_key``, whoever else is in the loop."""
+    stream at batch position ``noise_key``, whoever else is in the loop.  A stream admitted with ``rules`` brings its
+    own logits rules, length penalty, patience and beam width (``beam_size <= rows_per_stream``; width 1 is greedy)."""
 
     def __init__(self, engine: B200Whisper, capacity: int, *, beam_size: int = 5, patience: float = 1, num_hypotheses: int = 1,
                  length_penalty: float = 1, repetition_penalty: float = 1, no_repeat_ngram_size: int = 0,
@@ -1013,7 +1014,7 @@ class DecodeSession:
         self.engine = engine
         self.capacity = int(capacity)
         self.num_hypotheses = int(num_hypotheses)
-        # decoder rows per stream: the most hypotheses a sampled stream may ask for
+        # decoder rows per stream: the most hypotheses a sampled stream, or the widest beam a stream's rules, may ask for
         self.rows_per_stream = int(beam_size) if int(beam_size) > 1 else self.num_hypotheses
         self._nh: Dict[int, int] = {}                 # index -> hypotheses its stream returns
         self._sup = np.asarray(sorted({int(t) for t in (suppress_tokens or ()) if t >= 0}), dtype=np.int32)
@@ -1068,8 +1069,10 @@ class DecodeSession:
         ``sampling``: per stream None (the session's search) or ``(temperature, num_hypotheses, seed, noise_key)``.
         ``rules``: per stream None (the session's options) or a dict of ``generate`` keywords the stream decodes under
         instead -- ``suppress_tokens``, ``suppress_blank``, ``max_initial_timestamp_index``, ``length_penalty``,
-        ``patience`` (missing keys take ``generate``'s defaults) and optionally ``beam_size``, which must be the
-        session's.  ``features`` entries may be None when the session runs on scripted logits (``script``)."""
+        ``patience`` (missing keys take ``generate``'s defaults) and optionally ``beam_size``, from 1 (greedy) to
+        ``rows_per_stream``: the stream decodes as ``generate(beam_size=...)`` would decode it alone, and ``collect`` /
+        ``peek`` return its hypotheses.  ``features`` entries may be None when the session runs on scripted logits
+        (``script``)."""
         n = len(prompts)
         if n == 0:
             return []

@@ -1071,12 +1071,16 @@ ENGINE_MAX_INITIAL_TIMESTAMP_INDEX = 50     # generate's default, which BatchedI
 
 def _rules_fit(ds, skw: dict) -> bool:
     """Whether a stream with session options ``skw`` can join the open session ``ds`` with rules of its own: the session
-    takes per-stream rules and decodes with the same beam width (rows per stream are fixed per session)."""
+    takes per-stream rules, and the stream's beam width fits the session's rows per stream (a session that does not
+    report ``rows_per_stream`` takes only its own width)."""
     if not getattr(ds, "supports_rules", False):
         return False
     if any(skw.get(k, d) != d for k, d in (("repetition_penalty", 1), ("no_repeat_ngram_size", 0))):
         return False
-    return int(skw.get("beam_size", 5)) == int(ds.beam_size) and int(skw.get("num_hypotheses", 1)) == 1
+    width = int(skw.get("beam_size", 5))
+    rows = getattr(ds, "rows_per_stream", None)
+    fits = width <= int(rows) if rows is not None else width == int(ds.beam_size)
+    return fits and int(skw.get("num_hypotheses", 1)) == 1
 
 
 class _FileRun:
